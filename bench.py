@@ -3,7 +3,7 @@
 bench.py -- ResNet-50 gossip-SGD throughput (BASELINE.json headline metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--algo sgp|osgp|dpsgd|ar]
-                    [--batch-size B] [--impl ours|reference]
+                    [--batch-size B] [--impl ours|reference] [--dump-outputs DIR]
 
 N > 1 is launched by the driver as
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N \
@@ -12,7 +12,7 @@ N > 1 is launched by the driver as
 
 What is timed (our arm):
   * `value`  : K replays of the captured training step -- forward + fused softmax-xent /
-    prec@1 / prec@5 + backward + ONE fused sm_100a kernel (SGD-momentum + push-sum publish +
+    prec@1 / prec@5 + backward + ONE fused sm_90a kernel (SGD-momentum + push-sum publish +
     P2P pull over NVLink + mix + de-bias) -- inputs resident on the device, CUDA events on
     the launching stream, barrier + synchronize on both sides, max over ranks.  Whole-job
     images/s.  Default precision = the reference arm's: fp32 activations / weights / master
@@ -49,7 +49,7 @@ def parse():
     ap.add_argument('--batch-size', '--batch_size', dest='batch_size', type=int, default=256,
                     help='per-agent batch; 256 = every shipped job script of the reference '
                          '(job_scripts/submit_*.sh: --batch_size 256 per gossip agent); one agent '
-                         'per B200 here')
+                         'per GPU here')
     ap.add_argument('--dtype', default='fp32', choices=['bf16', 'fp32'],
                     help='fp32 (default): fp32 activations / weights with TF32 tensor-core convolutions, '
                          'the precision of the reference arm; bf16: reported as a labelled secondary line')
@@ -70,11 +70,15 @@ def parse():
     ap.add_argument('--skip-e2e', action='store_true')
     ap.add_argument('--skip-local', action='store_true',
                     help='skip the gossip-disabled re-measurement behind `exposed_comm` (N > 1)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last timed step computed as DIR/<name>.npy '
+                         '(loss / prec@1 / prec@5, a fixed seeded sample of the parameters, the BatchNorm '
+                         'running statistics) so that two builds can be compared output for output')
     return ap.parse_args()
 
 
 # --------------------------------------------------------------------------- #
-# clocks sampling (B200_PROFILING.md recipe)
+# clocks sampling
 # --------------------------------------------------------------------------- #
 class ClockSampler(object):
     QUERY = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,'
@@ -180,7 +184,30 @@ def _build(args, dtype, bs, rank, world, dev):
     return net, model, trainer, graph_name
 
 
-def measure(args, dtype, bs, K, W, rank, world, dev, sample_clocks):
+PARAM_SAMPLE = 1 << 22          # 16 MB of the ~100 MB fp32 parameter vector
+
+
+def dump_outputs(out_dir, trainer, net, rank):
+    """Write what the last timed step left for its caller: [loss, prec@1 %, prec@5 %], a fixed
+    seeded sample of the updated parameters and the BatchNorm running statistics (float32)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    sfx = '' if rank == 0 else '_rank%d' % rank
+    out = {}
+    metrics = getattr(trainer, 'static_metrics', None)
+    if metrics is not None:
+        out['metrics'] = metrics.detach().float().cpu()
+    params = torch.cat([p.detach().reshape(-1).float() for p in net.parameters()])
+    idx = torch.randperm(params.numel(), generator=torch.Generator().manual_seed(0))[:PARAM_SAMPLE]
+    out['params_sample'] = params[idx.sort().values.to(params.device)].cpu()
+    out['bn_running_stats'] = torch.cat([b.detach().reshape(-1).float() for n, b in net.named_buffers()
+                                         if n.endswith(('running_mean', 'running_var'))]).cpu()
+    for name, t in out.items():
+        np.save(os.path.join(out_dir, name + sfx + '.npy'), t.numpy().astype(np.float32))
+
+
+def measure(args, dtype, bs, K, W, rank, world, dev, sample_clocks, dump_dir=None):
     """One configuration: W warm-up steps, K device-timed replays (`value`), then K steps through
     the public API with H2D of the inputs and D2H of [loss, prec@1, prec@5] every step (`e2e`)."""
     import torch
@@ -229,6 +256,8 @@ def measure(args, dtype, bs, K, W, rank, world, dev, sample_clocks):
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
     ms = ms.item()
     value = bs * world * K / (ms / 1e3)
+    if dump_dir:
+        dump_outputs(dump_dir, trainer, net, rank)
 
     # ---- end-to-end timed region (public API, H2D + D2H every step) ---------
     e2e = None
@@ -347,14 +376,13 @@ def run_ours(args):
     torch.backends.cudnn.allow_tf32 = True
 
     bs, K, W = args.batch_size, args.steps, args.warmup
-    main = measure(args, args.dtype, bs, K, W, rank, world, dev, sample_clocks=True)
+    main = measure(args, args.dtype, bs, K, W, rank, world, dev, sample_clocks=True, dump_dir=args.dump_outputs)
     # secondary, clearly labelled lines: the other precision at the headline batch, and the
     # reference's per-GPU batch (32 images per GPU in its 8-GPU-per-node job scripts), where the
     # gossip step is a larger share of the iteration
     secondary = {}
     # (multi-GPU runs measure the headline configuration only -- one model / one symmetric-memory
-    # rendezvous per process; pass --secondary to force the extra lines there.  Batch-32 and bf16
-    # multi-GPU numbers: profiles/bench_r2_n2_*_bs32_*, profiles/bench_n8_sgp_bs32_r2_fp32.json)
+    # rendezvous per process; pass --secondary to force the extra lines there)
     if not args.no_secondary and (world == 1 or args.secondary):
         other = 'bf16' if args.dtype == 'fp32' else 'fp32'
         for key, (dt, b) in (('%s_bs%d' % (other, bs), (other, bs)), ('%s_bs32' % args.dtype, (args.dtype, 32))):
@@ -376,17 +404,17 @@ def run_ours(args):
                        'peers_per_itr': args.ppi, 'per_gpu_batch': bs, 'global_batch': bs * world,
                        'image': '3x224x224', 'parallelism': 'dp%d-gossip' % world,
                        'master_weights': 'fp32 flat arena', 'layout': 'NHWC',
-                       'compute_path': ('fp32 activations and weights; TF32 tcgen05 / cuDNN convolutions'
+                       'compute_path': ('fp32 activations and weights; TF32 wgmma / cuDNN convolutions'
                                         if args.dtype == 'fp32' else
                                         ('autocast' if (args.autocast or args.algo == 'ar') else
                                          'bf16 shadow weights written by the gossip kernel')),
                        'cuda_graph': not args.no_graph,
-                       'conv1x1': ('tcgen05 GEMM (TMA/TMEM, kind::%s), BN statistics and skip gradient '
-                                   'fused into its epilogues' % ('tf32' if args.dtype == 'fp32' else 'f16')
+                       'conv1x1': ('wgmma GEMM (TMA, %s), BN statistics and skip gradient '
+                                   'fused into its epilogues' % ('tf32' if args.dtype == 'fp32' else 'bf16')
                                    if _fb.USE_TCGEN05_CONV1X1 else 'library'),
                        'loss': 'fused softmax-xent + prec@1/5 kernel inside the captured step',
                        'l2': 'per-step working set (activations+weights > 1 GB) exceeds the '
-                             '126 MB L2; no explicit flush'},
+                             '50 MB L2; no explicit flush'},
             'clocks': main['clocks'], 'e2e': main['e2e'], 'exposed_comm': main['exposed_comm'],
             'gossip_rounds_completed_rank0': main['gossip_rounds'],
             'gpu_launches': (main['launches_per_step'] or 0) * K,

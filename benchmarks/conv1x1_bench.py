@@ -1,7 +1,7 @@
 """Per-layer A/B of the ResNet-50 1x1 convolutions (forward, training mode):
 
     library conv  + fused-BN (stats pass + finalize + apply)      <- default path
-    tcgen05 GEMM with the statistics in its epilogue + finalize + apply
+    wgmma GEMM with the statistics in its epilogue + finalize + apply
 
 and of the conv1 dgrad of every bottleneck (library dgrad + gradient-accumulation add vs the
 same GEMM with the skip gradient added in its epilogue).
@@ -77,7 +77,7 @@ def main():
         C = native.load()
         out = {}
         with torch.no_grad():
-            for name, use in (('library', False), ('tcgen05', True)):
+            for name, use in (('library', False), ('wgmma', True)):
                 fused_bn.USE_TCGEN05_CONV1X1 = use
                 fn = lambda: conv_bn_act(conv, bn, x, residual=res, relu=True)   # noqa: E731
                 for _ in range(3):
@@ -92,12 +92,12 @@ def main():
                          gemm_tbps=gemm_bytes / out['tc_gemm_only'] / 1e9,
                          lib_conv_tbps=gemm_bytes / out['lib_conv_only'] / 1e9, **out))
         tot_lib += mult * out['library']
-        tot_tc += mult * out['tcgen05']
-        print('%3dx%-3d %4d->%-4d add=%d x%d | conv+bn: lib %.3f ms  tcgen05 %.3f ms | conv only: lib %.3f '
-              '(%.2f TB/s)  tcgen05 %.3f (%.2f TB/s), +stats %.3f' % (
-                  hw, hw, cin, cout, add, mult, out['library'], out['tcgen05'], out['lib_conv_only'],
+        tot_tc += mult * out['wgmma']
+        print('%3dx%-3d %4d->%-4d add=%d x%d | conv+bn: lib %.3f ms  wgmma %.3f ms | conv only: lib %.3f '
+              '(%.2f TB/s)  wgmma %.3f (%.2f TB/s), +stats %.3f' % (
+                  hw, hw, cin, cout, add, mult, out['library'], out['wgmma'], out['lib_conv_only'],
                   rows[-1]['lib_conv_tbps'], out['tc_gemm_only'], rows[-1]['gemm_tbps'], out['tc_gemm_stats']), flush=True)
-    print('ResNet-50 fwd 1x1 conv+BN total: library %.3f ms, tcgen05 %.3f ms' % (tot_lib, tot_tc))
+    print('ResNet-50 fwd 1x1 conv+BN total: library %.3f ms, wgmma %.3f ms' % (tot_lib, tot_tc))
 
     # backward of the first 1x1 convolution of every bottleneck: dX = dY . W (+ skip gradient)
     drows, d_lib, d_tc = [], 0.0, 0.0
@@ -123,17 +123,17 @@ def main():
             for _ in range(3):
                 lib(); fused()
             t_lib, t_tc = timed(lib, args.iters, flush), timed(fused, args.iters, flush)
-        drows.append(dict(hw=hw, width=width, cin=cin, mult=mult, library=t_lib, tcgen05=t_tc))
+        drows.append(dict(hw=hw, width=width, cin=cin, mult=mult, library=t_lib, wgmma=t_tc))
         d_lib += mult * t_lib
         d_tc += mult * t_tc
-        print('dgrad %3dx%-3d %4d->%-4d x%d | lib dgrad + add %.3f ms | tcgen05 dgrad(+skip) %.3f ms' % (
+        print('dgrad %3dx%-3d %4d->%-4d x%d | lib dgrad + add %.3f ms | wgmma dgrad(+skip) %.3f ms' % (
             hw, hw, width, cin, mult, t_lib, t_tc), flush=True)
-    print('ResNet-50 conv1 dgrad + skip-gradient accumulation total: library %.3f ms, tcgen05 %.3f ms' % (d_lib, d_tc))
+    print('ResNet-50 conv1 dgrad + skip-gradient accumulation total: library %.3f ms, wgmma %.3f ms' % (d_lib, d_tc))
     if args.out:
         os.makedirs(os.path.dirname(args.out) or '.', exist_ok=True)
         with open(args.out, 'w') as f:
-            json.dump(dict(batch=args.batch, dtype=args.dtype, total_library_ms=tot_lib, total_tcgen05_ms=tot_tc, layers=rows,
-                           dgrad_library_ms=d_lib, dgrad_tcgen05_ms=d_tc, dgrad_layers=drows), f, indent=1)
+            json.dump(dict(batch=args.batch, dtype=args.dtype, total_library_ms=tot_lib, total_wgmma_ms=tot_tc, layers=rows,
+                           dgrad_library_ms=d_lib, dgrad_wgmma_ms=d_tc, dgrad_layers=drows), f, indent=1)
 
 
 if __name__ == '__main__':

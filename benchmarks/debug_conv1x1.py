@@ -1,4 +1,4 @@
-"""Blind-debug aid for the tcgen05 1x1-conv GEMM: prints error maps (which row groups /
+"""Blind-debug aid for the wgmma 1x1-conv GEMM: prints error maps (which row groups /
 column chunks / k-blocks are wrong) instead of a bare pass/fail."""
 import os
 import sys

@@ -2,7 +2,7 @@
 // devices (cuMulticastCreate / AddDevice / BindMem), maps unicast + multicast views, then checks
 // multimem.ld_reduce (in-switch sum) and multimem.st (in-switch broadcast) from a kernel, and
 // whether the handles can be exported as POSIX file descriptors (what the multi-process
-// rendezvous needs).   nvcc -arch=sm_100a -o nvls_probe nvls_probe.cu -lcuda
+// rendezvous needs).   nvcc -arch=sm_90a -o nvls_probe nvls_probe.cu -lcuda
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cstdio>

@@ -1,4 +1,4 @@
-"""Drop-in alias: ``import gossip`` resolves to the B200-native implementation
+"""Drop-in alias: ``import gossip`` resolves to the H100-native implementation
 with the reference's export list (``gossip/__init__.py:8-21``)."""
 from stochastic_gradient_push_b200.parallel.ad_psgd import BilatGossipDataParallel
 from stochastic_gradient_push_b200.parallel.distributed import GossipDataParallel

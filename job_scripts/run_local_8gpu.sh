@@ -1,5 +1,5 @@
 #!/bin/bash
-# One 8xB200 box, no scheduler: torchrun, one rank per GPU.
+# One 8xH100 box, no scheduler: torchrun, one rank per GPU.
 #   ./job_scripts/run_local_8gpu.sh sgp|osgp|dpsgd|ar|adpsgd [extra flags...]
 set -euo pipefail
 ALGO=${1:-sgp}; shift || true

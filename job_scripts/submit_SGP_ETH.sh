@@ -1,6 +1,6 @@
 #!/bin/bash
 # SGP_ETH: ResNet-50 / ImageNet, 90 epochs (recipe of the reference's job_scripts/submit_SGP_ETH.sh),
-# re-targeted at 8xB200 nodes: ONE RANK PER GPU (the reference ran one process per
+# re-targeted at 8xH100 nodes: ONE RANK PER GPU (the reference ran one process per
 # 8-GPU node), NVLink/NVSwitch gossip inside a node.
 #
 #SBATCH --job-name=SGP_ETH

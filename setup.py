@@ -1,7 +1,7 @@
 """
-Packaging for the B200-native gossip-SGD framework.
+Packaging for the H100-native gossip-SGD framework.
 
-    pip install -e . --no-build-isolation          # builds the sm_100a extension in-tree first
+    pip install -e . --no-build-isolation          # builds the sm_90a extension in-tree first
 
 The CUDA extension is NOT a setuptools ``Extension``: it is compiled by
 ``stochastic_gradient_push_b200/ops/build.py`` (nvcc for the kernels, g++ for the torch
@@ -42,7 +42,7 @@ if __name__ == '__main__':
         name='stochastic_gradient_push_b200',
         version='0.1.0',
         description='Gossip-based decentralised data-parallel training (SGP / OSGP / D-PSGD / AD-PSGD) '
-                    'with hand-written sm_100a kernels over NVLink peer memory.',
+                    'with hand-written sm_90a kernels over NVLink peer memory.',
         long_description=readme,
         long_description_content_type='text/markdown',
         python_requires='>=3.9',
@@ -54,7 +54,7 @@ if __name__ == '__main__':
         extras_require={'parse': ['pandas', 'matplotlib']},
         scripts=['gossip_sgd.py', 'gossip_sgd_adpsgd.py'],
         cmdclass={'build_py': build_py_with_native},
-        keywords=['deep learning', 'pytorch', 'decentralized optimization', 'gossip', 'CUDA', 'Blackwell'],
+        keywords=['deep learning', 'pytorch', 'decentralized optimization', 'gossip', 'CUDA', 'Hopper'],
         classifiers=['Programming Language :: Python :: 3', 'Environment :: GPU :: NVIDIA CUDA',
                      'Topic :: Scientific/Engineering :: Artificial Intelligence'],
     )

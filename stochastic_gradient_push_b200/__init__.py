@@ -1,5 +1,5 @@
 """
-stochastic_gradient_push_b200 -- B200-native gossip-SGD (SGP / OSGP / D-PSGD /
+stochastic_gradient_push_b200 -- H100-native gossip-SGD (SGP / OSGP / D-PSGD /
 AD-PSGD / AllReduce-SGD) with the API surface of
 facebookresearch/stochastic_gradient_push (``gossip/__init__.py:8-21``).
 """

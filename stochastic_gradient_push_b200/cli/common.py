@@ -45,7 +45,7 @@ def str2bool(v):
 
 
 def build_parser(adpsgd: bool = False) -> argparse.ArgumentParser:
-    p = argparse.ArgumentParser(description='Gossip SGD (B200-native)')
+    p = argparse.ArgumentParser(description='Gossip SGD (H100-native)')
     B = dict(type=str2bool, nargs='?', const=True)
     p.add_argument('--all_reduce', default=False, **B, help='all-reduce instead of gossip')
     p.add_argument('--batch_size', default=32, type=int, help='per-agent batch size')
@@ -90,7 +90,7 @@ def build_parser(adpsgd: bool = False) -> argparse.ArgumentParser:
         p.add_argument('--overwrite_checkpoints', default=True, **B)
         p.add_argument('--num_itr_ignore', type=int, default=10)
         p.add_argument('--no_cuda_streams', action='store_true')
-    # ---- B200-native additions (all optional) ----
+    # ---- H100-native additions (all optional) ----
     p.add_argument('--synthetic', default=None, **B,
                    help='synthetic 3x224x224 data (default: True when --dataset_dir is unset)')
     p.add_argument('--synthetic_len', default=1281167, type=int, help='images per synthetic epoch')

@@ -13,7 +13,7 @@ Launch (one rank per GPU):
         --schedule 30 0.1 60 0.1 80 0.1 --checkpoint_dir ./ckpt/ [--dataset_dir /imagenet]
 or under SLURM with the scripts in ``job_scripts/`` (SLURM_PROCID / SLURM_NTASKS).
 
-B200-native execution: parameters in a flat arena, SGD fused into the gossip
+H100-native execution: parameters in a flat arena, SGD fused into the gossip
 kernel (``--fused True``), bf16 NHWC compute (``--amp/--channels_last``),
 device-side metrics read out once per ``--print_freq`` instead of three host
 syncs per iteration, optional whole-step CUDA graph (``--cuda_graph True``).

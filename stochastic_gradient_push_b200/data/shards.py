@@ -1,11 +1,11 @@
 """
-Pre-decoded image shards + GPU-side augmentation: the input pipeline that keeps up with a B200.
+Pre-decoded image shards + GPU-side augmentation: the input pipeline that keeps up with an H100.
 
 The reference feeds its trainer with ``torchvision.datasets.ImageFolder`` + ``DataLoader`` workers
 (``gossip_sgd.py:539-583``): JPEG decode, ``RandomResizedCrop``, flip, ``ToTensor``, ``Normalize`` on
-the CPU, 602 KB of fp32 per image over PCIe.  That is ~1-2 k images/s per process; one B200 trains
-ResNet-50 at 6.6 k images/s (fp32/TF32) to 12.5 k (bf16), i.e. the stock pipeline would leave the
-GPU idle most of the time.  (The stock pipeline stays available: ``--data_format folder``.)
+the CPU, 602 KB of fp32 per image over PCIe.  That is ~1-2 k images/s per process; one H100 trains
+ResNet-50 at 2.8 k images/s (fp32/TF32) to 5.8 k (bf16) at batch 256 (measured at a 400 W power
+limit), i.e. the stock pipeline would leave the GPU idle much of the time.  (The stock pipeline stays available: ``--data_format folder``.)
 
 Here the dataset is decoded ONCE into uint8 shards (``write_shards``: short side resized to
 ``store_size``, centre crop, raw RGB, ``.npy`` files that are memory-mapped at training time):

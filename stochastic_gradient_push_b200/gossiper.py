@@ -15,7 +15,7 @@ What is different underneath:
   2-rank process group per edge.  Here a gossiper owns a *transport*:
 
   - ``PeerMemoryTransport`` (CUDA, engine in ``ops/peer_mix.py``): the message lives in
-    NVSwitch-mapped symmetric memory and ``mix`` is ONE sm_100a kernel that
+    NVSwitch-mapped symmetric memory and ``mix`` is ONE sm_90a kernel that
     publishes the message, waits on the in-neighbours' sequence flags and
     accumulates their buffers with weighted 16-byte P2P loads.  No NCCL.
   - ``C10dTransport`` (any backend, CPU/gloo capable): true ``isend/irecv``
@@ -165,7 +165,7 @@ class _PolledRecv(object):
 
 
 class PeerMemoryTransport(object):
-    """sm_100a data plane for STAND-ALONE gossipers (``README.md:67-68`` of the
+    """sm_90a data plane for STAND-ALONE gossipers (``README.md:67-68`` of the
     reference uses ``PushSum``/``PushPull`` directly on a tensor): the message is
     staged into a chunk-padded buffer whose outbox lives in NVSwitch peer-mapped
     memory and ``mix`` becomes kernel launches of :class:`~.ops.peer_mix.GossipEngine`

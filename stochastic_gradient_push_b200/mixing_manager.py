@@ -5,7 +5,7 @@ API parity with ``gossip/mixing_manager.py:19-56`` (``MixingManager``,
 ``UniformMixing``; ``get_mixing_weights`` returns a dict with ``'lo'``,
 ``'uniform'`` and one entry per out-peer rank).  In addition every manager can
 answer :meth:`scalar_weights` -- plain Python floats ``(self_weight,
-{out_peer: weight})`` -- which is what the fused sm_100a kernels consume: the
+{out_peer: weight})`` -- which is what the fused sm_90a kernels consume: the
 sender publishes its per-edge weight next to its outbox and the *receiver*
 applies it while it accumulates the P2P loads, so no "scale the message"
 kernel (reference K6, ``gossip/gossiper.py:139-147``) ever runs.

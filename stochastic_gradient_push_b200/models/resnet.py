@@ -1,11 +1,11 @@
 """
 ResNet family (v1.5 bottleneck: the stride sits on the 3x3 conv), written for
-the B200 execution model: NHWC (channels_last) activations and weights, bf16
+the H100 execution model: NHWC (channels_last) activations and weights, bf16
 tensor-core math under autocast with fp32 master weights in the gossip arena,
 BatchNorm statistics and affine parameters kept in fp32.
 
 Every BatchNorm is a :class:`~..ops.fused_bn.FusedBatchNormAct2d`: BN, the
-residual add and the ReLU of a block run as one fused sm_100a op (2 reads + 1
+residual add and the ReLU of a block run as one fused sm_90a op (2 reads + 1
 write forward) instead of three framework kernels; parameters, buffers and
 ``state_dict`` keys are those of ``nn.BatchNorm2d``.
 

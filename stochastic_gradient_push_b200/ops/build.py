@@ -1,5 +1,5 @@
 """
-In-tree build of the sm_100a extension (no JIT cache: the .so must travel with
+In-tree build of the sm_90a extension (no JIT cache: the .so must travel with
 the source tree to the GPU box).
 
     python -m stochastic_gradient_push_b200.ops.build [--force] [--verbose]
@@ -24,7 +24,7 @@ OBJ_DIR = os.path.join(HERE, '_obj')
 EXT_NAME = '_C'
 
 NVCC_FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a',
+    '-gencode', 'arch=compute_90a,code=sm_90a',
     '-lineinfo', '-O3', '-std=c++17', '--use_fast_math',
     '-Xcompiler', '-fPIC', '-Xptxas', '-v',
 ]

@@ -184,6 +184,8 @@ public:
         const char* env = std::getenv("SGP_B200_PIPE");
         use_pipe_ = !(env && env[0] == '0');
         args_.segments = 4;
+        c10::cuda::CUDAGuard guard(device_);
+        SGP_CUDA_CHECK(sgp_preload_kernels());
     }
 
     void set_schedule(torch::Tensor table, torch::Tensor wtable)
@@ -609,7 +611,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, mod)
     bind_bn(mod);
     bind_vmm(mod);
     bind_data(mod);
-    mod.doc() = "sm_100a gossip kernels + symmetric-memory runtime";
+    mod.doc() = "sm_90a gossip kernels + symmetric-memory runtime";
     mod.def("symm_alloc", &symm_alloc, "allocate IPC-exportable device memory -> (uint8 tensor, handle)");
     mod.def("symm_open", &symm_open, "map a peer's allocation -> uint8 tensor");
     mod.def("enable_peer_access", &enable_peer_access);

@@ -269,7 +269,7 @@ static torch::Tensor stem_wgrad(torch::Tensor x, torch::Tensor dy)
 }
 
 // ---------------------------------------------------------------------------
-// 1x1 convolution as a tcgen05 GEMM, BatchNorm statistics fused into its epilogue
+// 1x1 convolution as a wgmma GEMM, BatchNorm statistics fused into its epilogue
 // (conv1x1_kernels.cu)
 // ---------------------------------------------------------------------------
 extern "C" {
@@ -453,7 +453,7 @@ void bind_bn(py::module& mod)
     mod.def("xent_forward", &xent_forward);
     mod.def("xent_backward", &xent_backward);
     mod.def("conv1x1_can_fuse", &conv1x1_can_fuse);
-    mod.def("conv1x1_plan", &conv1x1_plan, py::arg("M"), py::arg("N"), py::arg("K"), py::arg("num_sms") = 148,
+    mod.def("conv1x1_plan", &conv1x1_plan, py::arg("M"), py::arg("N"), py::arg("K"), py::arg("num_sms") = 132,
             py::arg("residual") = false, py::arg("f32") = false);
     mod.def("conv1x1_forward", &conv1x1_forward, py::arg("x"), py::arg("w"), py::arg("with_stats") = false,
             py::arg("residual") = py::none());

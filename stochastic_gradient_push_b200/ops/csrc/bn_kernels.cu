@@ -1,8 +1,7 @@
 // Fused NHWC BatchNorm (+residual add) (+ReLU), training forward and backward,
-// for sm_100a.  An ncu launch list of the ResNet-50 step (profiles/) showed the
-// framework's native channels-last BatchNorm + separate ReLU / add kernels
-// taking ~70 % of the step at batch 256 while the tensor-core convolutions took
-// ~15 %: these kernels are memory-bound, so the fix is fewer passes over HBM.
+// for sm_90a.  The framework's native channels-last BatchNorm + separate ReLU / add
+// kernels take most of the ResNet-50 step at batch 256, far more than the tensor-core
+// convolutions: these kernels are memory-bound, so the fix is fewer passes over HBM.
 //
 //   forward :  stats (1 read of x)  ->  finalize (C threads)  ->  apply
 //              y = relu(x*scale + shift [+ res])   (1 read of x [+res], 1 write)
@@ -27,8 +26,7 @@
 // rows in flight per thread and tensor.  A thread's vector is 8 channels = 16 B of bf16 but 32 B
 // of fp32 (8 registers per load), so fp32 uses half the unroll: the same bytes in flight and the
 // same register footprint as bf16.  (With the bf16 unroll the fp32 instantiations spilled 250-460
-// bytes per thread under their 64 / 80-register caps and ran at 58-71 % of the HBM roofline
-// instead of 78-94 %: profiles/launches_r2_fp32_bs256_before_tf32_gemm_summary.json.)
+// bytes per thread under their 64 / 80-register caps.)
 template <typename T> struct Unroll {
     static constexpr int N = sizeof(T) == 4 ? 2 : 4;        // stats / apply / dx
     static constexpr int RED = sizeof(T) == 4 ? 1 : 2;      // backward reduce (up to 3 tensors)
@@ -146,8 +144,8 @@ __device__ __forceinline__ void sum_partials(const float* __restrict__ partial, 
     const int lane = threadIdx.x >> 5;
     ch = blockIdx.x * 32 + cl;
     // All of a lane's rows are requested before any is consumed: the partials sit in L2, each
-    // dependent load costs ~0.7 us, and a two-deep loop made these kernels 8-13 us each --
-    // 106 launches, ~5 % of the training step (profiles/launches_r1_bs256_final.csv).
+    // dependent load is an L2 round trip, and a two-deep loop made these 106 launches per step
+    // latency-bound.
     float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
     if (ch < C) {
         for (int g0 = lane; g0 < G; g0 += 32 * BN_FIN_ILP) {
@@ -407,7 +405,7 @@ static inline int bn_grid(long long M, int C, int per_sm)
     const int rpi = BN_THREADS / tpr;
     long long iters = (M + rpi - 1) / rpi;
     long long g = (iters + BN_UNROLL - 1) / BN_UNROLL;
-    const long long cap = 148LL * per_sm;
+    const long long cap = 132LL * per_sm;
     if (g > cap) g = cap;
     if (g < 1) g = 1;
     return (int)g;

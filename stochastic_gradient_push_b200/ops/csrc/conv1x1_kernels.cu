@@ -1,5 +1,5 @@
-// 1x1 convolution (NHWC) as a tcgen05 GEMM with the BatchNorm statistics (forward) or the
-// skip-branch gradient accumulation (backward) fused into the epilogue -- sm_100a only.
+// 1x1 convolution (NHWC) as a wgmma GEMM with the BatchNorm statistics (forward) or the
+// skip-branch gradient accumulation (backward) fused into the epilogue -- sm_90a (Hopper).
 //
 //   Y[M, N] = X[M, K] . W[N, K]^T        M = batch*H*W, K = C_in, N = C_out, bf16 in / fp32 acc
 //
@@ -9,42 +9,41 @@
 // GEMMs are HBM-bound (K is 64..2048 and M is up to 802,816), so the kernel is
 // organised around the epilogue, not the MMA:
 //
-//   warp 0   TMA producer   X tiles -> 128B-swizzled smem ring (cp.async.bulk.tensor, mbarrier
-//                           complete_tx).  The CTA's W block [BN, K] is loaded ONCE and stays
-//                           resident whenever it fits next to a >= 3-deep X ring (K*BN <= 64K
-//                           elements); otherwise W tiles travel through the ring with X.
-//   warp 1   MMA issuer     one thread: tcgen05.mma.cta_group::1.kind::f16, 128 x BN x 16,
-//                           accumulators in TMEM, double-buffered (2 x BN columns) so the
-//                           MMAs of tile i+1 run under the epilogue of tile i
-//   warp 2-9 epilogue       two sets of four warps, set h drains accumulator stage h (every other
-//                           tile).  Each warp owns 32 tile rows (its TMEM lane quadrant) end to end:
-//                           tcgen05.ld (32 lanes x 64 columns) -> bf16 -> its own 4 KB swizzled
-//                           slab -> its own TMA store (box 64 x 32), then the statistics of
-//                           exactly those rows are read back from the slab (lane = channel pair):
-//                           n / shifted sum / shifted sum of squares of the ROUNDED outputs
-//                           (what BatchNorm will read).  No CTA-wide barrier in the loop; slabs
-//                           recycle through the issuing lane's bulk-group counter.
+//   warp 8     TMA producer   X tiles -> 128B-swizzled smem ring (cp.async.bulk.tensor, mbarrier
+//                             complete_tx).  The CTA's W block [BN, K] is loaded ONCE and stays
+//                             resident whenever it fits next to a >= 3-deep X ring (K*BN <= 64K
+//                             elements); otherwise W tiles travel through the ring with X.
+//   warps 0-7  two warpgroups, each: wgmma.mma_async m64 x BN x 16 (bf16) / x 8 (tf32) on rows
+//                             [64g, 64g+64) of the 128-row tile, fp32 accumulators in registers,
+//                             then the epilogue.  Each warp owns the 16 tile rows its accumulator
+//                             fragment holds end to end: registers -> bf16 -> its own 2 KB
+//                             swizzled slab -> its own TMA store (box 64 x 16), then the
+//                             statistics of exactly those rows are read back from the slab (lane =
+//                             channel pair): n / shifted sum / shifted sum of squares of the
+//                             ROUNDED outputs (what BatchNorm will read).  No CTA-wide barrier in
+//                             the loop; slabs recycle through the issuing lane's bulk-group counter.
 //
 // The grid is persistent: CTA (nb, j) owns output-channel block nb for its whole life
 // and walks the row tiles j, j + ctas_per_n, ...; its statistics therefore stay in
-// registers until the end: each epilogue warp keeps (n, K, sum(y-K), sum((y-K)^2)) with its
+// registers until the end: each warp keeps (n, K, sum(y-K), sum((y-K)^2)) with its
 // own shift K (its first output row), the eight warps are merged in shared memory into one
-// (n, mean, M2) row per CTA, and c1_stats_finalize_kernel merges the <= 148 rows with the
-// pairwise (Chan) update and emits mean / invstd / scale / shift and the running-statistics
-// update, exactly what bn_stats_finalize_kernel does for the stand-alone statistics pass.
+// (n, mean, M2) row per CTA, and c1_stats_finalize_kernel merges the rows (one per CTA, at most
+// one per SM) with the pairwise (Chan) update and emits mean / invstd / scale / shift and the
+// running-statistics update, exactly what bn_stats_finalize_kernel does for the stand-alone
+// statistics pass.
 //
 // Three epilogue modes share the producer / MMA pipeline:
 //   MODE 0  Y = X.W^T
 //   MODE 1  + the BatchNorm statistics above (forward of conv + BN: no separate statistics pass)
-//   MODE 2  Y = X.W^T + R, R's 4 KB slab prefetched by TMA one sub-tile ahead (own mbarrier per
+//   MODE 2  Y = X.W^T + R, R's 2 KB slab prefetched by TMA one sub-tile ahead (own mbarrier per
 //           slab), summed in fp32 before the single bf16 rounding.  Used as the dgrad of the first
 //           convolution of a residual block with R = the skip-branch gradient, which replaces
 //           autograd's read-read-write accumulation pass over the block's widest tensor.
 //
-// Measured on B200 (benchmarks/conv1x1_bench.py, profiles/conv1x1_bench_*.log).
+// Timing: benchmarks/conv1x1_bench.py.
 //
-// Reference call site: torchvision Bottleneck conv1/conv3 + BatchNorm2d inside
-// /root/reference/gossip_sgd.py (models.resnet50()).
+// Reference call site: torchvision Bottleneck conv1/conv3 + BatchNorm2d in the reference
+// gossip_sgd.py (models.resnet50()).
 
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -54,23 +53,24 @@
 
 namespace {
 
-constexpr int BM = 128;                 // rows per tile == TMEM lanes == UMMA_M
+constexpr int BM = 128;                 // rows per tile: two warpgroups x wgmma M = 64
 constexpr int ROW_BYTES = 128;          // one k-block row == one 128-byte swizzle row: 64 bf16 or 32 fp32
 constexpr int A_BYTES = BM * ROW_BYTES; // 16 KB
-constexpr int SLAB_BYTES = 32 * 128;    // one epilogue warp's store slab: 32 rows x 128 B (64 bf16 / 32 fp32), 4 KB
+constexpr int SLAB_BYTES = 16 * 128;    // one warp's store slab: 16 rows x 128 B (64 bf16 / 32 fp32), 2 KB
 // Element-type dependent tile geometry.  F32 = fp32 activations / weights multiplied on the tensor
-// cores as TF32 (tcgen05.mma.kind::tf32 reads fp32 words from shared memory and uses their top 19
+// cores as TF32 (wgmma .tf32 reads fp32 words from shared memory and uses their top 19
 // bits: the same arithmetic as the reference's cuDNN TF32 convolutions), fp32 accumulate, fp32 out.
 template <bool F32> struct Elt {
     static constexpr int BYTES = F32 ? 4 : 2;
     static constexpr int BK = ROW_BYTES / BYTES;      // elements per k-block: 32 / 64
-    static constexpr int UMMA_K = 32 / BYTES;         // 8 (tf32) / 16 (bf16): 32 bytes of K per instruction
+    static constexpr int MMA_K = 32 / BYTES;          // 8 (tf32) / 16 (bf16): 32 bytes of K per instruction
     static constexpr int COLS = ROW_BYTES / BYTES;    // output columns per store slab: 32 / 64
 };
-constexpr int kThreads = 320;           // producer warp, MMA warp, 2 x 4 epilogue warps
+constexpr int kMmaWarps = 8;            // two warpgroups: MMA + epilogue
+constexpr int kThreads = kMmaWarps * 32 + 32;   // + the producer warp
 constexpr int MAX_STAGES = 8;
-constexpr int SMEM_LIMIT = 227 * 1024;  // opt-in dynamic shared memory per CTA on sm_100
-constexpr int SMEM_FIXED = 1024 + 512;  // alignment slack + barriers / TMEM slot
+constexpr int SMEM_LIMIT = 227 * 1024;  // opt-in dynamic shared memory per CTA on sm_90
+constexpr int SMEM_FIXED = 1024 + 512;  // alignment slack + barriers
 
 // cute::TMA::CacheHintSm90 encodings
 constexpr uint64_t L2_EVICT_NORMAL = 0x1000000000000000ull;
@@ -153,62 +153,161 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tm)
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tm)) : "memory");
 }
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] . B[smem]^T, issued by ONE thread for the whole CTA
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait()
 {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate)
+// keeps the compiler from moving accumulator reads / writes across wgmma issue and wait
+template <int R> __device__ __forceinline__ void fence_operands(float (&d)[R])
 {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on an mbarrier once every MMA issued so far has retired (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                     smem_u32(bar))
-                 : "memory");
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// K-major operand tile, rows of 64 bf16 (128 B) in the TMA 128B-swizzle layout, 8-row
-// groups 1024 B apart.  (cute::UMMA::SmemDescriptor: start>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version=1 [46,48), layout SWIZZLE_128B=2 [61,64).)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr)
+// K-major operand tile, rows of 128 B (64 bf16 / 32 fp32) in the TMA 128B-swizzle layout, 8-row
+// groups 1024 B apart.  (cute::GMMA::GmmaDescriptor: start>>4 [0,14), LBO>>4 [16,30) (unused for a
+// swizzled K-major operand), SBO>>4 [32,46), layout SWIZZLE_128B = 1 at [62,64).)
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr)
 {
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) |
-           (2ull << 61);
+    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
 
-// 32 TMEM lanes (this warp's quadrant) x 32 consecutive fp32 columns -> 32 registers / thread
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* v)
+// D[64 x N] (+)= A[64 x K-step] . B[N x K-step]^T, both operands K-major in shared memory, fp32
+// accumulators in registers; issued by one warpgroup.  bf16: k16 per instruction; tf32: k8.
+__device__ __forceinline__ void wgmma_bf16(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate)
 {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]),
-          "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]),
-          "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+        " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31},"
+        " %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_bf16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+        " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+        " %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+        " %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63},"
+        " %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_bf16(float (&d)[128], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+        " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+        " %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+        " %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63,"
+        " %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79,"
+        " %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95,"
+        " %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111,"
+        " %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127},"
+        " %128, %129, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_tf32(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+        " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31},"
+        " %32, %33, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+        " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+        " %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+        " %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63},"
+        " %64, %65, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_tf32(float (&d)[128], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+        " %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+        " %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+        " %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63,"
+        " %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79,"
+        " %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95,"
+        " %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111,"
+        " %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127},"
+        " %128, %129, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
 
 __device__ __forceinline__ uint32_t pack_bf16(uint32_t lo_f32, uint32_t hi_f32)
 {
@@ -237,10 +336,11 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
     constexpr bool STATS = MODE == 1;
     constexpr bool RES = MODE == 2;
     constexpr int BK = Elt<F32>::BK;
-    constexpr int UMMA_K = Elt<F32>::UMMA_K;
+    constexpr int MMA_K = Elt<F32>::MMA_K;
     constexpr int COLS = Elt<F32>::COLS;
     constexpr int B_BYTES = BN * ROW_BYTES;
     constexpr int NS = BN / COLS;             // store-slab wide sub-tiles per tile (64 bf16 / 32 fp32 columns)
+    constexpr int G8 = COLS / 8;              // 8-column accumulator groups per sub-tile
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 
@@ -263,34 +363,21 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
     uint8_t* sO = ring + stages * stage_bytes;
     uint64_t* full = reinterpret_cast<uint64_t*>(sO + 8 * nbuf * SLAB_BYTES);
     uint64_t* empty = full + MAX_STAGES;
-    uint64_t* tfull = empty + MAX_STAGES;    // accumulator stage ready for the epilogue
-    uint64_t* tempty = tfull + 2;            // accumulator stage drained
-    uint64_t* wfull = tempty + 2;            // resident W landed
+    uint64_t* wfull = empty + MAX_STAGES;    // resident W landed
     uint64_t* rbar0 = wfull + 1;             // MODE 2: residual slab landed, [8 warps][2 slots]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(rbar0 + 16);
 
-    if (warp == 0 && lane == 0) {
+    if (warp == kMmaWarps && lane == 0) {
         tma_prefetch_desc(&tm_x);
         tma_prefetch_desc(&tm_w);
         tma_prefetch_desc(&tm_y);
-        for (int i = 0; i < stages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 4); }
+        for (int i = 0; i < stages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kMmaWarps); }
         mbar_init(wfull, 1);
         if (RES) { tma_prefetch_desc(&tm_r); for (int i = 0; i < 16; ++i) mbar_init(&rbar0[i], 1); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                     "r"((uint32_t)(2 * BN))
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
 
-    if (warp == 0) {
+    if (warp == kMmaWarps) {
         // ===================== TMA producer =====================
         if (lane == 0) {
             if (resident) {
@@ -312,89 +399,76 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        if (lane == 0) {
-            // cute::UMMA::InstrDescriptor: D=f32 [4,6)=1, A=bf16 [7,10)=1, B=bf16 [10,13)=1,
-            // A/B K-major (bits 15,16 = 0), N>>3 at [17,23), M>>4 at [24,29)
-            // (tf32: A/B format code 2)
-            constexpr uint32_t fmt = F32 ? 2u : 1u;
-            constexpr uint32_t idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(BN >> 3) << 17) |
-                                       ((uint32_t)(BM >> 4) << 24);
-            if (resident) { mbar_wait(wfull, 0); tc_fence_after(); }
-            int stage = 0;
-            uint32_t phase = 0;
-            int as = 0;
-            uint32_t aphase = 0;
-            for (int mt = j; mt < m_tiles; mt += ctas_per_n) {
-                mbar_wait(&tempty[as], aphase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(as * BN);
-                for (int kb = 0; kb < k_blocks; ++kb) {
-                    mbar_wait(&full[stage], phase);
-                    tc_fence_after();
-                    const uint8_t* a_ptr = ring + stage * stage_bytes;
-                    const uint8_t* b_ptr = resident ? sW + kb * B_BYTES : a_ptr + A_BYTES;
-                    const uint64_t a_desc = umma_desc_sw128(smem_u32(a_ptr));
-                    const uint64_t b_desc = umma_desc_sw128(smem_u32(b_ptr));
-#pragma unroll
-                    for (int k = 0; k < BK / UMMA_K; ++k) {    // +32 B per UMMA_K inside the swizzle row
-                        if (F32)
-                            umma_tf32(d_tmem, a_desc + (uint64_t)(k * 2), b_desc + (uint64_t)(k * 2), idesc,
-                                      (uint32_t)((kb | k) != 0));
-                        else
-                            umma_bf16(d_tmem, a_desc + (uint64_t)(k * 2), b_desc + (uint64_t)(k * 2), idesc,
-                                      (uint32_t)((kb | k) != 0));
-                    }
-                    umma_commit(&empty[stage]);                 // smem slot free once these MMAs retire
-                    if (++stage == stages) { stage = 0; phase ^= 1; }
-                }
-                umma_commit(&tfull[as]);
-                as ^= 1;
-                if (as == 0) aphase ^= 1;
-            }
-        }
     } else {
-        // ===================== epilogue =====================
-        // Two sets of four warps; set h drains accumulator stage h, i.e. every other tile, so each
-        // SM sub-partition has two epilogue warps to interleave (a lone warp per scheduler exposes
-        // every TMEM / shared-memory latency) and one stage drains while the other fills.
-        // Within a set, warp q owns tile rows [32q, 32q+32) (its TMEM lane quadrant) end to end:
-        // TMEM -> bf16 -> its own 4 KB swizzled slab -> its own TMA store (box 64 x 32) ->
-        // statistics of exactly those rows read back from the slab.  No CTA-wide barrier; slabs
-        // are recycled through the issuing lane's bulk-group counter.
-        const int set = (warp - 2) >> 2;
-        const int q = warp & 3;
-        const uint32_t slab0 = smem_u32(sO) + (uint32_t)((set * 4 + q) * nbuf * SLAB_BYTES);
-        const uint32_t wr_off = (uint32_t)(lane * 128);                    // this lane's row in the slab
+        // ===================== MMA + epilogue =====================
+        // Warpgroup g multiplies rows [64g, 64g+64) of every tile with the whole W block.  In the
+        // accumulator layout of wgmma warp q of the group holds rows [16q, 16q+16) of that half:
+        // d[4c + i] is row lane/4 + 8*(i/2), column 8c + 2*(lane%4) + i%2.  Each warp then carries
+        // its 16 rows end to end: registers -> bf16 -> its own 2 KB swizzled slab -> its own TMA
+        // store (box 64 x 16) -> statistics of exactly those rows read back from the slab.  No
+        // CTA-wide barrier in the loop; slabs recycle through the issuing lane's bulk-group counter.
+        // While a tile drains, the producer keeps the ring filling with the next tile's X.
+        const int g = warp >> 2;
+        const int e = warp;                                                // 0..7: this warp's 16 rows
+        const int row0 = 64 * g + 16 * (warp & 3);                         // first tile row of this warp
+        const uint32_t slab0 = smem_u32(sO) + (uint32_t)(e * nbuf * SLAB_BYTES);
         const uint32_t rd_off = (uint32_t)((lane & 3) * 4);                // this lane's bf16 pair in a row
         const int rd_chunk = lane >> 2;
+        const int r0 = lane >> 2;                                          // accumulator rows r0, r0 + 8
+        const uint32_t wr_off = (uint32_t)(r0 * 128);
+        float acc[BN / 2];
         int slot = 0;
         float cnt = 0.f;
         float k0[NS], k1[NS], s0[NS], s1[NS], q0[NS], q1[NS];
 #pragma unroll
         for (int s = 0; s < NS; ++s) { k0[s] = k1[s] = s0[s] = s1[s] = q0[s] = q1[s] = 0.f; }
         bool have_k = false;
-        const int as = set;
-        uint32_t aphase = 0;
+        int stage = 0;
+        uint32_t phase = 0;
         // MODE 2: the residual slab of sub-tile i+1 is fetched (TMA, own mbarrier per slab) while
         // sub-tile i is converted; the sum is formed in fp32 in place and stored from the same slab.
-        const uint32_t rbar = smem_u32(rbar0 + (set * 4 + q) * 2);
+        const uint32_t rbar = smem_u32(rbar0 + e * 2);
         uint32_t rphase = 0;                                     // bit b: parity of slab b's barrier
-        const int tile_step = 2 * ctas_per_n;
+        const int tile_step = ctas_per_n;
         if (RES && lane == 0) {
-            const int mt0 = j + set * ctas_per_n;
-            if (mt0 < m_tiles && M - mt0 * BM - q * 32 > 0) {
+            const int mt0 = j;
+            if (mt0 < m_tiles && M - mt0 * BM - row0 > 0) {
                 asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(rbar), "r"(SLAB_BYTES)
                              : "memory");
-                tma_load_2d_s(&tm_r, rbar, slab0, nb * BN, mt0 * BM + q * 32, L2_EVICT_FIRST);
+                tma_load_2d_s(&tm_r, rbar, slab0, nb * BN, mt0 * BM + row0, L2_EVICT_FIRST);
             }
         }
-        for (int mt = j + set * ctas_per_n; mt < m_tiles; mt += tile_step) {
-            mbar_wait(&tfull[as], aphase);
-            tc_fence_after();
-            const int nrows = min(32, M - mt * BM - q * 32);       // rows of this slab that exist (<= 0: none)
-            const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * BN);
+        if (resident) mbar_wait(wfull, 0);
+        for (int mt = j; mt < m_tiles; mt += tile_step) {
+            // ---- MMA: one commit group per k-block; a stage is released once its group retired ----
+            int prev = -1;
+            for (int kb = 0; kb < k_blocks; ++kb) {
+                mbar_wait(&full[stage], phase);
+                const uint8_t* a_ptr = ring + stage * stage_bytes;
+                const uint8_t* b_ptr = resident ? sW + kb * B_BYTES : a_ptr + A_BYTES;
+                const uint64_t a_desc = gmma_desc_sw128(smem_u32(a_ptr + g * (A_BYTES / 2)));
+                const uint64_t b_desc = gmma_desc_sw128(smem_u32(b_ptr));
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / MMA_K; ++k) {     // +32 B per MMA_K inside the swizzle row
+                    if (F32) wgmma_tf32(acc, a_desc + (uint64_t)(k * 2), b_desc + (uint64_t)(k * 2),
+                                        (uint32_t)((kb | k) != 0));
+                    else wgmma_bf16(acc, a_desc + (uint64_t)(k * 2), b_desc + (uint64_t)(k * 2),
+                                    (uint32_t)((kb | k) != 0));
+                }
+                wgmma_commit();
+                wgmma_wait<1>();
+                if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
+                prev = stage;
+                if (++stage == stages) { stage = 0; phase ^= 1; }
+            }
+            wgmma_wait<0>();
+            fence_operands(acc);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[prev]);
+
+            // ---- epilogue ----
+            const int nrows = min(16, M - mt * BM - row0);         // rows of this slab that exist (<= 0: none)
 #pragma unroll
             for (int s = 0; s < NS; ++s) {
                 const uint32_t slab = slab0 + (uint32_t)(slot * SLAB_BYTES);
@@ -404,15 +478,6 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
                         else asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
                     }
                     __syncwarp();
-                }
-                uint32_t v[64];
-                tmem_ld32(t_row + (uint32_t)(s * COLS), v);
-                if (!F32) tmem_ld32(t_row + (uint32_t)(s * COLS + 32), v + 32);
-                tmem_ld_wait();
-                if (s == NS - 1) {                                 // accumulator fully read: hand it back
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&tempty[as]);
                 }
                 if (RES && nrows > 0) {
                     const uint32_t bar = rbar + (uint32_t)(slot * 8);
@@ -430,53 +495,57 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
                 }
                 if (!RES || nrows > 0) {
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        const uint32_t addr = slab + wr_off + (uint32_t)((i ^ (lane & 7)) * 16);
-                        if (RES) {
-                            uint32_t r0, r1, r2, r3;
-                            asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
-                                         : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr) : "memory");
-                            const uint32_t rr[4] = {r0, r1, r2, r3};
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                if (F32) {
-                                    v[4 * i + e] = __float_as_uint(__uint_as_float(v[4 * i + e]) +
-                                                                   __uint_as_float(rr[e]));
-                                } else {
-                                    v[8 * i + 2 * e] = __float_as_uint(__uint_as_float(v[8 * i + 2 * e]) +
-                                                                       __uint_as_float(rr[e] << 16));
-                                    v[8 * i + 2 * e + 1] = __float_as_uint(__uint_as_float(v[8 * i + 2 * e + 1]) +
-                                                                           __uint_as_float(rr[e] & 0xFFFF0000u));
-                                }
+                    for (int c = 0; c < G8; ++c) {
+                        const float* d = acc + 4 * (s * G8 + c);
+                        // 16-byte chunk of the 128-byte row and byte offset in it; rows r0 and r0 + 8
+                        // share the swizzle phase (row & 7), so the second address is + 1024
+                        const uint32_t chunk = F32 ? (uint32_t)(2 * c + ((lane & 3) >> 1)) : (uint32_t)c;
+                        const uint32_t addr = slab + wr_off + ((chunk ^ (uint32_t)(r0 & 7)) << 4) +
+                                              (F32 ? (uint32_t)((lane & 1) * 8) : rd_off);
+                        if (F32) {
+                            float v0 = d[0], v1 = d[1], v2 = d[2], v3 = d[3];
+                            if (RES) {
+                                float a0, a1, a2, a3;
+                                asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(a0), "=f"(a1) : "r"(addr) : "memory");
+                                asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(a2), "=f"(a3) : "r"(addr + 1024u)
+                                             : "memory");
+                                v0 += a0; v1 += a1; v2 += a2; v3 += a3;
                             }
+                            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v0), "f"(v1) : "memory");
+                            asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr + 1024u), "f"(v2), "f"(v3)
+                                         : "memory");
+                        } else {
+                            float v0 = d[0], v1 = d[1], v2 = d[2], v3 = d[3];
+                            if (RES) {
+                                uint32_t a, b;
+                                asm volatile("ld.shared.b32 %0, [%1];" : "=r"(a) : "r"(addr) : "memory");
+                                asm volatile("ld.shared.b32 %0, [%1];" : "=r"(b) : "r"(addr + 1024u) : "memory");
+                                v0 += __uint_as_float(a << 16); v1 += __uint_as_float(a & 0xFFFF0000u);
+                                v2 += __uint_as_float(b << 16); v3 += __uint_as_float(b & 0xFFFF0000u);
+                            }
+                            asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr),
+                                         "r"(pack_bf16(__float_as_uint(v0), __float_as_uint(v1))) : "memory");
+                            asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr + 1024u),
+                                         "r"(pack_bf16(__float_as_uint(v2), __float_as_uint(v3))) : "memory");
                         }
-                        if (F32)
-                            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v[4 * i + 0]),
-                                         "r"(v[4 * i + 1]), "r"(v[4 * i + 2]), "r"(v[4 * i + 3])
-                                         : "memory");
-                        else
-                            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr),
-                                         "r"(pack_bf16(v[8 * i + 0], v[8 * i + 1])), "r"(pack_bf16(v[8 * i + 2], v[8 * i + 3])),
-                                         "r"(pack_bf16(v[8 * i + 4], v[8 * i + 5])), "r"(pack_bf16(v[8 * i + 6], v[8 * i + 7]))
-                                         : "memory");
                     }
                 }
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> TMA reads
                 __syncwarp();
                 if (lane == 0) {
-                    if (nrows > 0) tma_store_2d(&tm_y, slab, nb * BN + s * COLS, mt * BM + q * 32);
+                    if (nrows > 0) tma_store_2d(&tm_y, slab, nb * BN + s * COLS, mt * BM + row0);
                     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
                     if (RES) {                                     // fetch the next residual slab
                         const int nmt = (s + 1 < NS) ? mt : mt + tile_step;
                         const int ns = (s + 1 < NS) ? s + 1 : 0;
-                        if (nmt < m_tiles && M - nmt * BM - q * 32 > 0) {
+                        if (nmt < m_tiles && M - nmt * BM - row0 > 0) {
                             asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");   // other slab is free
                             const uint32_t nbar = rbar + (uint32_t)((slot ^ 1) * 8);
                             asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(nbar),
                                          "r"(SLAB_BYTES)
                                          : "memory");
                             tma_load_2d_s(&tm_r, nbar, slab0 + (uint32_t)((slot ^ 1) * SLAB_BYTES), nb * BN + ns * COLS,
-                                          nmt * BM + q * 32, L2_EVICT_FIRST);
+                                          nmt * BM + row0, L2_EVICT_FIRST);
                         }
                     }
                 }
@@ -488,9 +557,9 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
                         k0[s] = F32 ? __uint_as_float(u) : __uint_as_float(u << 16);
                         k1[s] = __uint_as_float(u & 0xFFFF0000u);
                     }
-                    if (nrows == 32) {
+                    if (nrows == 16) {
 #pragma unroll
-                        for (int r8 = 0; r8 < 32; r8 += 8) {
+                        for (int r8 = 0; r8 < 16; r8 += 8) {
                             uint32_t u[8];
 #pragma unroll
                             for (int i = 0; i < 8; ++i)
@@ -523,16 +592,14 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
                 slot = (slot + 1) & (nbuf - 1);      // nbuf is 1 or 2
             }
             if (nrows > 0) { cnt += (float)nrows; have_k = true; }
-            aphase ^= 1;
         }
         if (STATS) {
             // Merge the eight warps' partials (each with its own shift) into ONE row per CTA,
             // partial[j][field][N] with fields = n, mean, M2 (Chan et al.), so the finalize kernel
-            // reads <= 148 rows.  The store slabs double as scratch once their stores have drained.
-            if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-            float4* sc = reinterpret_cast<float4*>(sO);
-            const int e = set * 4 + q;
+            // reads one row per CTA.  Every X load has landed and been consumed, so the ring is
+            // free to serve as scratch.
+            asm volatile("bar.sync 1, %0;" ::"n"(kMmaWarps * 32) : "memory");
+            float4* sc = reinterpret_cast<float4*>(ring);
 #pragma unroll
             for (int s = 0; s < NS; ++s) {
                 if (F32) {
@@ -542,8 +609,8 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
                     sc[e * BN + s * COLS + 2 * lane + 1] = make_float4(cnt, k1[s], s1[s], q1[s]);
                 }
             }
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-            const int t = (int)threadIdx.x - 64;
+            asm volatile("bar.sync 1, %0;" ::"n"(kMmaWarps * 32) : "memory");
+            const int t = (int)threadIdx.x;
             if (t < BN) {
                 float n_tot = 0.f, m_sum = 0.f;
 #pragma unroll
@@ -571,15 +638,6 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         }
         if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
     }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        __syncwarp();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                     "r"((uint32_t)(2 * BN))
-                     : "memory");
-    }
 }
 
 // ---------------------------------------------------------------------------
@@ -601,7 +659,7 @@ c1_stats_finalize_kernel(const float* __restrict__ partial, int R, int C, const 
     const bool live = ch < C;
     if (blockIdx.x == 0 && threadIdx.x == 0 && nbt != nullptr) *nbt += 1;
 
-    // every row of this lane is loaded up front (R <= 148 -> at most 5 rows per lane per batch), so
+    // every row of this lane is loaded up front (R <= 160 -> at most 5 rows per lane per batch), so
     // the kernel pays one L2 round trip instead of one per row
     constexpr int ILP = 5;
     float n_sum = 0.f, m_sum = 0.f;
@@ -865,7 +923,7 @@ cudaError_t c1_launch_gemm(const void* x, const void* w, void* y, long long M, i
     grid_shape(M, N, K, num_sms, f, bn, per, grid);
     CUtensorMap tx, tw, ty, tr;
     if (!make_map(&tx, x, M, K, BM, true, f) || !make_map(&tw, w, N, K, bn, true, f) ||
-        !make_map(&ty, y, M, N, 32, false, f) || !make_map(&tr, residual ? residual : y, M, N, 32, false, f))
+        !make_map(&ty, y, M, N, 16, false, f) || !make_map(&tr, residual ? residual : y, M, N, 16, false, f))
         return cudaErrorInvalidValue;
     if (f) {
         switch (bn) {

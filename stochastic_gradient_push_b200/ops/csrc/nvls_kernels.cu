@@ -1,4 +1,4 @@
-// NVLS (NVSwitch multicast) collectives fused with the optimizer -- sm_100a, multimem.* PTX.
+// NVLS (NVSwitch multicast) collectives fused with the optimizer -- sm_90a, multimem.* PTX.
 //
 // The buffers live in VMM symmetric memory with a multicast mapping (csrc/vmm_symm.cpp): a load
 // from the multicast address can be REDUCED INSIDE THE SWITCH over all GPUs

@@ -1,9 +1,7 @@
-// NHWC max-pooling for sm_100a (forward + backward).
+// NHWC max-pooling for sm_90a (forward + backward).
 //
-// The framework's channels-last max-pool pair cost 2.5 ms per ResNet-50 step at
-// batch 256 (profiles/launches_r1_bs256_fused_bn.csv: forward 0.75 ms, backward
-// 1.73 ms -- it keeps int64 argmax indices, 8 bytes per output element, and the
-// backward is a scatter).  Here:
+// The framework's channels-last max-pool pair keeps int64 argmax indices, 8 bytes per
+// output element, and its backward is a scatter.  Here:
 //   forward : one thread = 8 channels of one output pixel, 16-byte loads of the
 //             <= k*k window, writes y and a 1-BYTE window-local argmax code;
 //   backward: a GATHER -- one thread = 8 channels of one INPUT pixel, visits the
@@ -103,7 +101,7 @@ maxpool_bwd_kernel(const T* __restrict__ dy, const uint8_t* __restrict__ code, T
 static inline int pool_grid(long long total)
 {
     long long g = (total + POOL_THREADS - 1) / POOL_THREADS;
-    if (g > 148LL * 16) g = 148LL * 16;
+    if (g > 132LL * 16) g = 132LL * 16;
     if (g < 1) g = 1;
     return (int)g;
 }

@@ -1,4 +1,4 @@
-// Shared definitions for the sm_100a gossip kernels.
+// Shared definitions for the sm_90a gossip kernels.
 //
 // Data plane design (see DESIGN.md):
 //   * every rank owns, in NVSwitch peer-mapped ("symmetric") memory,
@@ -172,7 +172,7 @@ __device__ __forceinline__ float4 ld_stream_f4(const float4* p) {
 }
 // local streaming loads with an L2 evict-first policy: data consumed exactly
 // once (z, g, m, residual) must not push the freshly published outbox -- which
-// phase 2 re-reads -- out of the 126 MB L2.  (On sm_100a the `.L2::evict_first`
+// phase 2 re-reads -- out of the 50 MB L2.  (The `.L2::evict_first`
 // qualifier is only legal on 32-byte loads, so 16-byte loads carry the policy
 // as an explicit cache hint.)
 __device__ __forceinline__ uint64_t l2_evict_first_policy() {
@@ -278,4 +278,5 @@ cudaError_t sgp_launch_barrier(SgpSignalPad* const* pads, SgpState* st, int rank
 cudaError_t sgp_launch_allreduce_sgd(const SgpArgs* args, void* const* grad_peers, int grid,
                                      cudaStream_t stream);
 int sgp_max_resident_ctas(int device);
+cudaError_t sgp_preload_kernels();
 }

@@ -1,4 +1,4 @@
-// sm_100a gossip kernels: fused SGD + push-sum mix over NVSwitch peer memory.
+// sm_90a gossip kernels: fused SGD + push-sum mix over NVSwitch peer memory.
 //
 // Replaces, in ONE launch per training step, the reference's K1-K9 elementwise
 // swarm (ps_numerator / unbias / residual add / pre-scale / flatten / scale /
@@ -560,8 +560,7 @@ sgp_gather_tma_kernel(const SgpArgs a, const int pub_grid)
 //
 // sgp_step_kernel pulls the peers' outboxes with register-staged 16-byte loads: every
 // consumer thread has 4 x 16 B in flight and the CTA alternates between an HBM-bound phase 1
-// and an NVLink-bound phase 2 (0.257 ms at ResNet-50 size on 2 GPUs = 52 % of the NVLink
-// roofline, profiles/README.md).  Here the two phases run on different warps of the same CTA:
+// and an NVLink-bound phase 2, so its time is close to the sum of the two.  Here the two phases run on different warps of the same CTA:
 //
 //   warps 0-7 (consumers)  for seg = 0..K:   phase 1 of segment `seg`   (SGD + publish, HBM)
 //                                            phase 2 of segment `seg-1` (mix + de-bias)
@@ -597,8 +596,7 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 
 // 9 warps x 2 CTAs per SM: the register file is split over 4 sub-partitions (16 K registers
 // each), so 18 warps only fit at <= 102 registers per thread -- __launch_bounds__(288, 2) makes
-// ptxas pick 96.  (At 112 registers ncu showed launch__occupancy_limit_registers = 1 block and
-// the kernel ran one CTA per SM, profiles/step_pipe_2gpu_nvlink_ncu_r2_v1.csv.)
+// ptxas pick 96.  (At 112 registers the kernel runs one CTA per SM.)
 __global__ void __launch_bounds__(PIPE_THREADS, 2)
 sgp_step_pipe_kernel(const SgpArgs a)
 {
@@ -882,9 +880,8 @@ __global__ void sgp_probe_kernel(const SgpArgs a, const int pub_grid, uint32_t* 
 // ---------------------------------------------------------------------------
 // Overlap-SGP gather on the COPY ENGINES (one in-neighbour per step).  A gather kernel on the side
 // stream -- even the 32-CTA TMA one -- holds SMs while the forward pass starts: persistent
-// one-CTA-per-SM kernels (the tcgen05 GEMMs) and 2-CTA/SM tile loops then wait for "their" SM, and
-// the overlap costs more than it hides (bench: OSGP +0.41 ms vs SGP +0.22 ms per step at 2 GPUs,
-// profiles/bench_r2_n2_*).  With a single in-neighbour the residual is just a copy of the peer's
+// one-CTA-per-SM kernels (the wgmma GEMMs) and 2-CTA/SM tile loops then wait for "their" SM, and
+// the overlap costs more than it hides.  With a single in-neighbour the residual is just a copy of the peer's
 // outbox, so:
 //     sgp_gather_wait_kernel   ONE CTA: wait for the in-neighbour's publish flags of this step
 //     cudaMemcpyAsync          peer outbox -> residual, 100 MB over NVLink on a DMA engine: zero SMs
@@ -1307,7 +1304,7 @@ cudaError_t sgp_launch_peer_reduce(float* dst, const float* const* srcs, int nsr
     for (int k = 0; k < nsrc; ++k) l.p[k] = srcs[k];
     const long long n4 = n / 4;
     int grid = (int)((n4 + SGP_THREADS - 1) / SGP_THREADS);
-    if (grid > 148 * 8) grid = 148 * 8;
+    if (grid > 132 * 8) grid = 132 * 8;
     if (grid < 1) grid = 1;
     sgp_peer_reduce_kernel<<<grid, SGP_THREADS, 0, stream>>>(dst, l, n4, scale);
     return cudaGetLastError();
@@ -1317,7 +1314,7 @@ cudaError_t sgp_launch_zero(void* p, long long bytes, cudaStream_t stream)
 {
     const long long n16 = bytes / 16;
     int grid = (int)((n16 + SGP_THREADS - 1) / SGP_THREADS);
-    if (grid > 148 * 8) grid = 148 * 8;
+    if (grid > 132 * 8) grid = 132 * 8;
     if (grid < 1) grid = 1;
     sgp_zero_kernel<<<grid, SGP_THREADS, 0, stream>>>(reinterpret_cast<float4*>(p), n16);
     return cudaGetLastError();
@@ -1335,10 +1332,30 @@ cudaError_t sgp_launch_scale(float* x, long long n, const float* scalar, int inv
 {
     long long n4 = n / 4;
     int grid = (int)((n4 + SGP_THREADS - 1) / SGP_THREADS);
-    if (grid > 148 * 8) grid = 148 * 8;
+    if (grid > 132 * 8) grid = 132 * 8;
     if (grid < 1) grid = 1;
     sgp_scale_kernel<<<grid, SGP_THREADS, 0, stream>>>(x, n, scalar, invert, shadow);
     return cudaGetLastError();
+}
+
+// Load every gossip kernel into the current device's context now.  Under lazy module loading a
+// kernel is loaded at its first launch, and loading can wait for the whole device.  A process that
+// drives several ranks (one GPU each, or virtual ranks sharing one GPU) would then wait for one
+// rank's spinning gossip kernel whose in-neighbour's publish it has not launched yet.
+cudaError_t sgp_preload_kernels()
+{
+    const void* kernels[] = {
+        (const void*)sgp_step_kernel, (const void*)sgp_gather_kernel, (const void*)sgp_gather_tma_kernel,
+        (const void*)sgp_step_pipe_kernel, (const void*)sgp_probe_kernel, (const void*)sgp_gather_wait_kernel,
+        (const void*)sgp_gather_ack_kernel, (const void*)sgp_bilat_decide_kernel, (const void*)sgp_bilat_ctl_kernel,
+        (const void*)sgp_allreduce_sgd_kernel, (const void*)sgp_zero_kernel, (const void*)sgp_barrier_kernel,
+        (const void*)sgp_scale_kernel, (const void*)sgp_peer_reduce_kernel};
+    for (const void* k : kernels) {
+        cudaFuncAttributes attr;
+        const cudaError_t e = cudaFuncGetAttributes(&attr, k);
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
 }
 
 int sgp_max_resident_ctas(int device)

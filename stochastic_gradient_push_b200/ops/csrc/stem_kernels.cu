@@ -4,7 +4,7 @@
 // Why a dedicated kernel: with 3 input channels the library falls back to generic
 // kernels (ncu launch list, batch 256: fprop 1.48 ms, wgrad 0.77 ms per step) although
 // the layer only moves ~0.5 GB (ideal ~0.1 ms).  K = 7*7*3 = 147 is too short for the
-// big tcgen05 tiles to matter -- the op is bandwidth/issue bound -- so this uses warp-
+// big wgmma tiles to matter -- the op is bandwidth/issue bound -- so this uses warp-
 // level mma.sync.m16n8k16 (bf16 in, fp32 accumulate) with the im2col gather done on the
 // fly from a shared-memory copy of the input patch:
 //
@@ -297,8 +297,7 @@ stem_wgrad_kernel(const uint16_t* __restrict__ x, const uint16_t* __restrict__ d
 // ===========================================================================
 // fp32 activations / weights, TF32 tensor-core math (mma.sync.m16n8k8.tf32): the
 // precision-matched flagship path (the reference's cuDNN runs this layer in TF32 too, with
-// generic kernels: 2.60 ms forward + 2.58 ms wgrad at batch 256 in
-// profiles/launches_r2_fp32_bs256_before_tf32_gemm_summary.json).
+// generic kernels).
 // Same tiling as the bf16 kernels; fp32 words in shared memory, so no pair-packing tricks:
 //   fprop : Y[128 x 64] = A[128 x 152] * W^T[152 x 64]      (K 147 -> 152 = 19 k-steps of 8)
 //   wgrad : dW[64 x 152] += dY^T[64 x 128] * A[128 x 152]   (K = the tile's 128 pixels)
@@ -537,7 +536,7 @@ cudaError_t stem_launch_fwd_f32(const void* x, const void* w, void* y, int N, in
                                 cudaStream_t st)
 {
     const long long tiles = (long long)N * ((OH + ST_TH - 1) / ST_TH) * ((OW + ST_TW - 1) / ST_TW);
-    int grid = 148 * 2;
+    int grid = 132 * 2;
     if (tiles < grid) grid = (int)tiles;
     static bool configured[64] = {};
     int dev = 0;
@@ -557,7 +556,7 @@ cudaError_t stem_launch_wgrad_f32(const void* x, const void* dy, float* dw_acc, 
                                   int OH, int OW, cudaStream_t st)
 {
     const long long tiles = (long long)N * ((OH + ST_TH - 1) / ST_TH) * ((OW + ST_TW - 1) / ST_TW);
-    int grid = 148 * 2;
+    int grid = 132 * 2;
     if (tiles < grid) grid = (int)tiles;
     stem_wgrad_tf32_kernel<<<grid, ST_THREADS, 0, st>>>((const float*)x, (const float*)dy, dw_acc, N, H, W, OH, OW);
     return cudaGetLastError();
@@ -567,7 +566,7 @@ cudaError_t stem_launch_fwd(const void* x, const void* w, void* y, int N, int H,
                             cudaStream_t st)
 {
     const long long tiles = (long long)N * ((OH + ST_TH - 1) / ST_TH) * ((OW + ST_TW - 1) / ST_TW);
-    int grid = 148 * 2;
+    int grid = 132 * 2;
     if (tiles < grid) grid = (int)tiles;
     stem_fwd_kernel<<<grid, ST_THREADS, 0, st>>>((const uint16_t*)x, (const uint16_t*)w, (uint16_t*)y,
                                                  N, H, W, OH, OW);
@@ -578,7 +577,7 @@ cudaError_t stem_launch_wgrad(const void* x, const void* dy, float* dw_acc, int 
                               int OH, int OW, cudaStream_t st)
 {
     const long long tiles = (long long)N * ((OH + ST_TH - 1) / ST_TH) * ((OW + ST_TW - 1) / ST_TW);
-    int grid = 148 * 2;
+    int grid = 132 * 2;
     if (tiles < grid) grid = (int)tiles;
     stem_wgrad_kernel<<<grid, ST_THREADS, 0, st>>>((const uint16_t*)x, (const uint16_t*)dy, dw_acc,
                                                    N, H, W, OH, OW);

@@ -6,7 +6,7 @@
 //   every rank   cuMemCreate (POSIX-fd exportable physical memory on its GPU), map it
 //   exchange     the POSIX fds are passed between the ranks' processes over abstract unix-domain
 //                sockets (SCM_RIGHTS; `FdChannel` below -- pidfd_getfd is refused with EPERM inside
-//                the GPU containers, profiles/gputest_multigpu_n2_r2_nvls_attempt1.log), then
+//                containers), then
 //                cuMemImportFromShareableHandle'd; no fabric handles / IMEX daemon needed
 //   unicast      every peer's allocation is mapped (cuMemAddressReserve / cuMemMap / cuMemSetAccess):
 //                plain P2P loads / stores / cp.async.bulk over NVLink work as before

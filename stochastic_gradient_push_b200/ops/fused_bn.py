@@ -1,9 +1,9 @@
 """
 FusedBatchNormAct2d: BatchNorm2d (+ residual add) (+ ReLU) as ONE op, backed by
-the sm_100a NHWC kernels in ``csrc/bn_kernels.cu``.
+the sm_90a NHWC kernels in ``csrc/bn_kernels.cu``.
 
-Why it exists: an ncu launch list of the ResNet-50 training step at batch 256
-(``profiles/launches_r1_bs256_before_fused_bn.csv``) attributes ~59 % of the
+Why it exists: in the ResNet-50 training step at batch 256 the launch list
+attributes most of the
 GPU time to the framework's channels-last BatchNorm kernels and ~13 % to
 stand-alone ReLU / add / cast kernels, versus ~15 % for the tensor-core
 convolutions.  All of that work is memory-bound, so it is rewritten as the
@@ -18,8 +18,8 @@ runs the reference composition ``relu(batch_norm(x) + residual)``, which is
 also the oracle in the numerics tests.
 
 ``conv_bn_act`` / ``conv_bn_act_split`` go one step further for 1x1 / stride-1
-convolutions: the convolution itself runs as the hand-written tcgen05 GEMM of
-``csrc/conv1x1_kernels.cu`` (TMA operand ring, TMEM accumulators), whose
+convolutions: the convolution itself runs as the hand-written wgmma GEMM of
+``csrc/conv1x1_kernels.cu`` (TMA operand ring, register accumulators), whose
 epilogue produces the BatchNorm statistics (no separate statistics pass) and,
 in backward, adds the skip-branch gradient of a residual block inside the
 dgrad GEMM (no autograd accumulation pass).  Also here: the NHWC max-pool and
@@ -39,7 +39,7 @@ from . import native
 
 FORCE_REFERENCE = False      # debugging / A-B switch: route everything to the PyTorch composition
 
-# 1x1 convolutions feeding a training-mode BatchNorm run as the tcgen05 GEMM with the
+# 1x1 convolutions feeding a training-mode BatchNorm run as the wgmma GEMM with the
 # statistics fused into its epilogue (csrc/conv1x1_kernels.cu).  SGP_B200_CONV1X1=0 routes
 # them back to the library convolution + stand-alone statistics pass.
 USE_TCGEN05_CONV1X1 = os.environ.get('SGP_B200_CONV1X1', '1') != '0'
@@ -134,7 +134,7 @@ class FusedBatchNormAct2d(nn.BatchNorm2d):
 # 1x1 convolution + BatchNorm (+ residual) (+ ReLU)
 # --------------------------------------------------------------------------- #
 class _Conv1x1BNAct(torch.autograd.Function):
-    """``act(bn(conv1x1(x, w)) [+ residual])`` in training mode.  Forward: tcgen05 GEMM
+    """``act(bn(conv1x1(x, w)) [+ residual])`` in training mode.  Forward: wgmma GEMM
     whose epilogue also produces the BatchNorm statistics, finalize, apply.  Backward: the
     fused BN backward, then the library's dgrad / wgrad for the convolution."""
 
@@ -216,7 +216,7 @@ class _Conv1x1BNActSplit(torch.autograd.Function):
 
 
 def _conv1x1_operands(conv, bn, x, residual, relu):
-    """(x, fusable): x possibly cast the way autocast would; fusable says whether the tcgen05
+    """(x, fusable): x possibly cast the way autocast would; fusable says whether the wgmma
     conv + BN path covers this call."""
     if not (USE_TCGEN05_CONV1X1 and not FORCE_REFERENCE and bn.training and bn.track_running_stats
             and x.is_cuda and native.available() and x.dim() == 4
@@ -243,7 +243,7 @@ def _conv1x1_operands(conv, bn, x, residual, relu):
 
 def conv_bn_act(conv: nn.Conv2d, bn: 'FusedBatchNormAct2d', x, residual=None, relu=False):
     """``bn(conv(x), residual=residual, relu=relu)``; 1x1 / stride-1 convolutions of NHWC bf16
-    activations in training mode take the fused tcgen05 path."""
+    activations in training mode take the fused wgmma path."""
     xk, ok = _conv1x1_operands(conv, bn, x, residual, relu)
     if ok:
         momentum = 0.1 if bn.momentum is None else bn.momentum
@@ -287,7 +287,7 @@ class _MaxPoolNHWC(torch.autograd.Function):
 
 
 class MaxPool2dNHWC(nn.MaxPool2d):
-    """``nn.MaxPool2d`` whose channels-last CUDA path is the sm_100a gather
+    """``nn.MaxPool2d`` whose channels-last CUDA path is the sm_90a gather
     kernel pair in ``csrc/pool_kernels.cu`` (1-byte argmax codes instead of
     int64 indices, atomic-free backward).  Other inputs use the stock op."""
 

@@ -4,7 +4,7 @@ FusedCrossEntropyWithAccuracy: softmax cross-entropy + prec@1 / prec@5 in ONE la
 The reference computes ``nn.CrossEntropyLoss`` and then, every iteration,
 ``accuracy(output, target, topk=(1, 5))`` followed by three ``.item()`` host
 synchronisations (``/root/reference/gossip_sgd.py:372-373, 394-399, 192-198``).
-Here one sm_100a kernel (``csrc/loss_kernels.cu``) emits the mean loss and both
+Here one sm_90a kernel (``csrc/loss_kernels.cu``) emits the mean loss and both
 accuracies into a 3-float device tensor and keeps the per-row log-sum-exp for
 the backward kernel; the training step copies those 12 bytes into a pinned ring
 without ever blocking the host (``parallel/trainer.py``).

@@ -1,5 +1,5 @@
 """
-Loader for the in-tree sm_100a extension (``stochastic_gradient_push_b200/_C*.so``).
+Loader for the in-tree sm_90a extension (``stochastic_gradient_push_b200/_C*.so``).
 
 The extension is never silently replaced by a PyTorch fallback: on a machine
 with a CUDA device ``load()`` either returns the native module or raises.  If

@@ -1,5 +1,5 @@
 """
-GossipEngine: drives the sm_100a gossip kernels for ONE rank.
+GossipEngine: drives the sm_90a gossip kernels for ONE rank.
 
 It owns the peer-visible signal pad + double-buffered outbox (symmetric
 memory), the device-side schedule tables emitted from a ``GraphManager`` /

@@ -9,7 +9,7 @@ API parity with ``gossip/ad_psgd.py:36-418``: same constructor arguments,
 The reference forks a separate gossip *process* that owns a second
 ``torch.distributed`` world, a shared-memory (CUDA-IPC / pinned) copy of the
 model + gradients and its own ``torch.optim.SGD``, and loops forever
-{apply new gradients; bilateral average with the next peer}.  On B200 none of
+{apply new gradients; bilateral average with the next peer}.  On H100 none of
 that needs a process:
 
 * the "gossip copy" is a second flat arena on the same GPU; gradients reach it

@@ -9,7 +9,7 @@ attributes ``ps_weight``, ``is_ps_numerator``, ``gossip_enable``,
 ``gossiping``, ``params_mixed``, ``overlap``, ``synch_freq``, ``asynch``,
 ``lazy_mixing``, ``num_updates``, ``dist_config``, ``gossip_stream``).
 
-What is different underneath (B200-first):
+What is different underneath (H100-first):
 
 * parameters are re-homed into ONE flat, 256-byte aligned arena at wrap time
   (``utils/arena.py``); there is no per-step flatten / unflatten / per-tensor
@@ -59,7 +59,7 @@ HEARTBEAT_TIMEOUT = 300  # seconds a rank waits for its in-neighbours (reference
 # backends
 # --------------------------------------------------------------------------- #
 class _KernelBackend(object):
-    """sm_100a data plane: GossipEngine over symmetric memory."""
+    """sm_90a data plane: GossipEngine over symmetric memory."""
 
     name = 'nvlink'
 
@@ -371,7 +371,7 @@ class GossipDataParallel(Module):
         if use_kernels and not (on_cuda and all_fp32):
             raise RuntimeError('nvlink transport needs fp32 CUDA parameters')
         if use_kernels and not _native_ok():
-            raise RuntimeError('nvlink transport requested but the sm_100a extension is '
+            raise RuntimeError('nvlink transport requested but the sm_90a extension is '
                                'not available (python -m stochastic_gradient_push_b200.ops.build)')
 
         # push-sum weight (host mirror; the kernel transport keeps the truth on device)

@@ -13,7 +13,7 @@ Differences from the reference that are deliberate:
   ``Edge.process_group`` is ``None`` unless :meth:`materialize_process_groups`
   is called (collective; only useful for reference-style broadcast transports).
 * **The graph emits a device table** (:meth:`device_table`): per phase the in-
-  and out-neighbours of this rank as an int32 tensor that the sm_100a kernels
+  and out-neighbours of this rank as an int32 tensor that the sm_90a kernels
   index with ``step % period`` -- the per-step neighbour list never touches
   Python on the hot path.
 * ``world_size == 1`` is a valid (peer-less) graph instead of a math domain

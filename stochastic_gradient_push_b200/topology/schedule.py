@@ -6,7 +6,7 @@ topology is a *phone book* -- for every rank the ordered list of ranks it may
 push to -- plus a window of ``peers_per_itr`` consecutive phone-book slots that
 is active in a given iteration and slides by ``peers_per_itr`` every time the
 graph is rotated.  Everything the transports need (the c10d fallback, the
-device-side neighbour table indexed by the sm_100a mix kernels) is derived from
+device-side neighbour table indexed by the sm_90a mix kernels) is derived from
 this one structure.
 
 Parity notes (reference = facebookresearch/stochastic_gradient_push):

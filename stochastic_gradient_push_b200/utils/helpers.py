@@ -4,7 +4,7 @@ Tensor / logging / process-group helpers.
 API parity with ``gossip/utils/helpers.py`` (flatten_tensors :21-36,
 unflatten_tensors :39-57, group_by_dtype :60-70, communicate :73-88,
 make_logger :91-114, is_power_of :117-128, create_process_group :131-146).
-On the B200 hot path none of the flatten helpers run: parameters live in a
+On the H100 hot path none of the flatten helpers run: parameters live in a
 flat arena (``utils/arena.py``) and "flatten" is the identity.
 """
 

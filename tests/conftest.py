@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on B200 via gpurun)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100)')
     config.addinivalue_line('markers', 'multigpu: needs >= 2 CUDA devices')
 
 

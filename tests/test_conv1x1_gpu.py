@@ -1,4 +1,4 @@
-"""tcgen05 1x1-convolution GEMM with fused BatchNorm statistics (csrc/conv1x1_kernels.cu)
+"""wgmma 1x1-convolution GEMM with fused BatchNorm statistics (csrc/conv1x1_kernels.cu)
 vs plain PyTorch fp32 references of the same ops."""
 import pytest
 import torch
@@ -220,7 +220,7 @@ def test_unsupported_inputs_fall_back(monkeypatch):
 @pytest.mark.parametrize('cin,width,hw', [(256, 64, 14), (512, 128, 7)])
 def test_fp32_bottleneck_matches_library_path(monkeypatch, cin, width, hw):
     """fp32 activations / weights (the precision-matched flagship path): a bottleneck through the
-    TF32 tcgen05 GEMMs (statistics + skip gradient fused) and through library TF32 convolutions +
+    TF32 wgmma GEMMs (statistics + skip gradient fused) and through library TF32 convolutions +
     the stand-alone fused BN, both measured against the SAME block evaluated in fp64.  TF32
     rounding flips ReLU masks of near-zero activations, so two TF32 paths differ element-wise;
     what must hold is that ours is as close to the fp64 truth as the library path is."""

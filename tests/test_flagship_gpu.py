@@ -34,7 +34,7 @@ def test_trainer_resnet50_loss_decreases_world1():
 
 
 def test_trainer_fp32_tf32_path_matches_library_path(monkeypatch):
-    """The precision-matched flagship step (fp32 activations / weights, TF32 tcgen05 1x1 GEMMs with
+    """The precision-matched flagship step (fp32 activations / weights, TF32 wgmma 1x1 GEMMs with
     fused statistics + skip gradient, TF32 stem kernels, fused loss + accuracy) against the same
     step with every convolution on the library (cuDNN TF32): same losses within TF32 noise, both
     memorise a fixed batch, metrics ring carries [loss, prec@1, prec@5]."""

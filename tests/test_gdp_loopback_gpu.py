@@ -3,6 +3,9 @@ ONE process on ONE GPU (``LocalWorld`` loop-back): the same world-simulation ora
 multi-process tests (tests/test_multigpu.py), but runnable on a single-GPU box -- SGP, D-PSGD,
 Overlap-SGP, the peers_per_itr schedule swap and the graph-captured trainer all exercise the
 flag / ack protocol between kernels that are co-resident on the same device."""
+import functools
+import threading
+
 import pytest
 import torch
 
@@ -37,24 +40,49 @@ def _world(n, graph_name, ppi, overlap, fused, nesterov):
     return ranks
 
 
+def _in_threads(fns):
+    """Run one callable per virtual rank, each on its own host thread, as every rank has its own
+    process in a real run.  A host call of one rank may wait for the whole device (the first launch
+    of a library kernel can), and a gossip kernel of that rank spins until its in-neighbour's
+    publish is launched: that launch must not queue behind the waiting call on a shared thread."""
+    errors = []
+
+    def run(fn):
+        try:
+            fn()
+        except BaseException as e:          # re-raised on the test's thread
+            errors.append(e)
+    threads = [threading.Thread(target=run, args=(fn,)) for fn in fns]
+    for t in threads:
+        t.start()
+    for t in threads:
+        t.join()
+    if errors:
+        raise errors[0]
+
+
 def _run(n, graph_name, ppi, steps, overlap, fused, nesterov, ppi_switch=None):
     dev = torch.device('cuda', 0)
     ranks = _world(n, graph_name, ppi, overlap, fused, nesterov)
+
+    def rank_step(r, step):
+        model, opt, s = ranks[r]
+        with torch.cuda.stream(s):
+            x, y = sim._batch(r, step)
+            loss = ((model(x.to(dev)) - y.to(dev)) ** 2).mean()
+            loss.backward()
+            opt.step()
+            opt.zero_grad()
+            if not overlap:
+                model.transfer_params()          # launches the fused kernel; peers follow on their streams
+
     for step in range(steps):
         if ppi_switch is not None and step == ppi_switch[0]:
             torch.cuda.synchronize()
             for model, _, s in ranks:
                 with torch.cuda.stream(s):
                     model.update_gossiper('peers_per_itr', ppi_switch[1])
-        for r, (model, opt, s) in enumerate(ranks):
-            with torch.cuda.stream(s):
-                x, y = sim._batch(r, step)
-                loss = ((model(x.to(dev)) - y.to(dev)) ** 2).mean()
-                loss.backward()
-                opt.step()
-                opt.zero_grad()
-                if not overlap:
-                    model.transfer_params()          # launches the fused kernel; peers follow on their streams
+        _in_threads([functools.partial(rank_step, r, step) for r in range(n)])
     for model, _, s in ranks:
         with torch.cuda.stream(s):
             model.sync_comms()
@@ -136,10 +164,12 @@ def test_loopback_graphed_trainer_equals_eager(algo):
                 for tr in trainers:
                     with torch.cuda.stream(tr.stream):
                         tr._capture()
-            for r, tr in enumerate(trainers):
+
+            def rank_step(r):
                 x = torch.randn(8, 3, 32, 32, generator=gens[r]).pin_memory()
                 y = torch.randint(0, 10, (8,), generator=gens[r]).pin_memory()
-                tr.step(x, y)
+                trainers[r].step(x, y)
+            _in_threads([functools.partial(rank_step, r) for r in range(n)])
             torch.cuda.synchronize()
         for tr in trainers:
             tr.finish()

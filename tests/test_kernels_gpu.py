@@ -1,4 +1,4 @@
-"""sm_100a kernels vs plain PyTorch fp32/fp64 oracles.
+"""sm_90a kernels vs plain PyTorch fp32/fp64 oracles.
 
 Loop-back layout: N virtual ranks on ONE GPU (``LocalWorld``), each with its
 own stream and a small grid so that all kernels are co-resident and really spin

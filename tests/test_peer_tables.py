@@ -1,4 +1,4 @@
-"""Device schedule tables (ops/peer_mix.build_tables): the receiver-side edge weights the sm_100a
+"""Device schedule tables (ops/peer_mix.build_tables): the receiver-side edge weights the sm_90a
 gossip kernel multiplies its P2P loads with.  Host logic only -- no GPU.
 
 Push-sum needs a COLUMN-stochastic mixing matrix every step: whatever rank j keeps for itself plus

@@ -100,7 +100,7 @@ def main():
     print('ResNet-50 fwd 1x1 conv+BN total: library %.3f ms, wgmma %.3f ms' % (tot_lib, tot_tc))
 
     # backward of the first 1x1 convolution of every bottleneck: dX = dY . W (+ skip gradient)
-    drows, d_lib, d_tc = [], 0.0, 0.0
+    drows, d_lib, d_tc, d_m2, d_m3 = [], 0.0, 0.0, 0.0, 0.0
     for hw, width, cin, mult in DGRAD_LAYERS:
         dy = torch.randn(args.batch, width, hw, hw, device='cuda').to(DT) \
             .contiguous(memory_format=torch.channels_last)
@@ -119,21 +119,45 @@ def main():
             wt = w.reshape(width, cin).t().contiguous()
             return C.conv1x1_forward(dy, wt, False, skip)
 
+        # the previous block's bn3 backward reduction: stand-alone (MODE 2 dgrad + mode-2 reduce
+        # pass over dy / yraw3 / out3) vs folded into the dgrad epilogue (MODE 3)
+        yraw3 = torch.randn_like(skip)
+        out3 = torch.relu(yraw3)
+        mask = torch.randint(0, 256, (skip.numel() // cin, cin // 8), dtype=torch.uint8, device='cuda')
+        coef = torch.stack([yraw3.float().mean((0, 2, 3)), torch.ones(cin, device='cuda'),
+                            torch.ones(cin, device='cuda'), torch.zeros(cin, device='cuda')])
+        wt_ = w.reshape(width, cin).t().contiguous()
+
+        def mode2_reduce():
+            return C.bn_backward(C.conv1x1_forward(dy, wt_, False, skip), yraw3, out3, coef, True, True)
+
+        def mode3():
+            dz, partial = C.conv1x1_dgrad_bn_reduce(dy, wt_, skip, yraw3, coef, mask)
+            return C.bn_backward_from_partials(dz, yraw3, coef, partial)
+
         with torch.no_grad():
             for _ in range(3):
-                lib(); fused()
+                lib(); fused(); mode2_reduce(); mode3()
             t_lib, t_tc = timed(lib, args.iters, flush), timed(fused, args.iters, flush)
-        drows.append(dict(hw=hw, width=width, cin=cin, mult=mult, library=t_lib, wgmma=t_tc))
+            t_m2, t_m3 = timed(mode2_reduce, args.iters, flush), timed(mode3, args.iters, flush)
+        drows.append(dict(hw=hw, width=width, cin=cin, mult=mult, library=t_lib, wgmma=t_tc,
+                          mode2_plus_bn_bwd=t_m2, mode3_plus_bn_bwd=t_m3))
         d_lib += mult * t_lib
         d_tc += mult * t_tc
-        print('dgrad %3dx%-3d %4d->%-4d x%d | lib dgrad + add %.3f ms | wgmma dgrad(+skip) %.3f ms' % (
-            hw, hw, width, cin, mult, t_lib, t_tc), flush=True)
+        d_m2 += mult * t_m2
+        d_m3 += mult * t_m3
+        print('dgrad %3dx%-3d %4d->%-4d x%d | lib dgrad + add %.3f ms | wgmma dgrad(+skip) %.3f ms | '
+              'bn3 bwd + dgrad: MODE 2 + reduce %.3f ms, MODE 3 %.3f ms' % (
+                  hw, hw, width, cin, mult, t_lib, t_tc, t_m2, t_m3), flush=True)
     print('ResNet-50 conv1 dgrad + skip-gradient accumulation total: library %.3f ms, wgmma %.3f ms' % (d_lib, d_tc))
+    print('with the previous bn3 backward (reduce + finalize + dx): MODE 2 + reduce %.3f ms, MODE 3 %.3f ms' % (
+        d_m2, d_m3))
     if args.out:
         os.makedirs(os.path.dirname(args.out) or '.', exist_ok=True)
         with open(args.out, 'w') as f:
             json.dump(dict(batch=args.batch, dtype=args.dtype, total_library_ms=tot_lib, total_wgmma_ms=tot_tc, layers=rows,
-                           dgrad_library_ms=d_lib, dgrad_wgmma_ms=d_tc, dgrad_layers=drows), f, indent=1)
+                           dgrad_library_ms=d_lib, dgrad_wgmma_ms=d_tc, dgrad_mode2_reduce_ms=d_m2,
+                           dgrad_mode3_ms=d_m3, dgrad_layers=drows), f, indent=1)
 
 
 if __name__ == '__main__':

@@ -24,7 +24,8 @@ cudaError_t bn_launch_stats_finalize(const float* partial, int G, long long M, i
 cudaError_t bn_launch_eval_coeff(int C, const float* gamma, const float* beta, const float* rmean,
                                  const float* rvar, float eps, float* scale, float* shift, cudaStream_t st);
 cudaError_t bn_launch_apply(int dtype, int relu, int add, const void* x, const void* res,
-                            const float* scale, const float* shift, void* y, long long M, int C, cudaStream_t st);
+                            const float* scale, const float* shift, void* y, uint8_t* mask, long long M, int C,
+                            cudaStream_t st);
 cudaError_t bn_launch_bwd_reduce(int dtype, int mode, const void* dy, const void* x, const void* y,
                                  const float* scale, const float* shift, const float* mean,
                                  const float* invstd, float* partial, void* dz, long long M, int C,
@@ -122,7 +123,7 @@ static std::vector<torch::Tensor> bn_forward(torch::Tensor x, c10::optional<torc
                                       (float)eps, scale, shift, st));
     }
     BN_CHECK(bn_launch_apply(dt, relu ? 1 : 0, has_res ? 1 : 0, x.data_ptr(),
-                             has_res ? residual->data_ptr() : nullptr, scale, shift, y.data_ptr(),
+                             has_res ? residual->data_ptr() : nullptr, scale, shift, y.data_ptr(), nullptr,
                              M, C, st));
     return {y, coef};
 }
@@ -163,6 +164,31 @@ static std::vector<torch::Tensor> bn_backward(torch::Tensor dy, torch::Tensor x,
                               x.data_ptr(), scale, shift, gg + 2 * C, gg + 3 * C, dx.data_ptr(),
                               M, C, st));
     return {dx, dz, grads.select(0, 0), grads.select(0, 1)};
+}
+
+// bn_backward's finalize + dx passes for a dz whose reduction partial[G][2][C] (sum dz, sum dz * xhat)
+// was produced elsewhere (the MODE 3 dgrad epilogue); returns (dx, grad_gamma, grad_beta)
+static std::vector<torch::Tensor> bn_backward_from_partials(torch::Tensor dz, torch::Tensor x, torch::Tensor coef,
+                                                            torch::Tensor partial)
+{
+    long long M; int C;
+    nhwc_dims(x, M, C);
+    const int dt = dtype_code(x);
+    TORCH_CHECK(dz.scalar_type() == x.scalar_type() && dz.sizes() == x.sizes() && dz.strides() == x.strides());
+    TORCH_CHECK(partial.scalar_type() == torch::kFloat32 && partial.is_contiguous() && partial.dim() == 3 &&
+                partial.size(1) == 2 && partial.size(2) == C);
+    c10::cuda::CUDAGuard guard(x.get_device());
+    auto st = at::cuda::getCurrentCUDAStream();
+    const float* mean = coef.data_ptr<float>();
+    const float* invstd = mean + C; const float* scale = mean + 2 * C; const float* shift = mean + 3 * C;
+    auto grads = torch::empty({4, C}, torch::TensorOptions().dtype(torch::kFloat32).device(x.device()));
+    float* gg = grads.data_ptr<float>();
+    BN_CHECK(bn_launch_bwd_finalize(partial.data_ptr<float>(), (int)partial.size(0), M, C, scale, mean, invstd,
+                                    gg, gg + C, gg + 2 * C, gg + 3 * C, st));
+    auto dx = torch::empty_like(x);
+    BN_CHECK(bn_launch_bwd_dx(dt, 0, dz.data_ptr(), x.data_ptr(), scale, shift, gg + 2 * C, gg + 3 * C,
+                              dx.data_ptr(), M, C, st));
+    return {dx, grads.select(0, 0), grads.select(0, 1)};
 }
 
 // ---------------------------------------------------------------------------
@@ -274,10 +300,11 @@ static torch::Tensor stem_wgrad(torch::Tensor x, torch::Tensor dy)
 // ---------------------------------------------------------------------------
 extern "C" {
 int c1_supported(long long M, int N, int K, int f32);
-int c1_partial_rows(long long M, int N, int K, int num_sms, int f32);
-void c1_describe_plan(long long M, int N, int K, int num_sms, int residual, int f32, int* out);
+int c1_partial_rows(long long M, int N, int K, int num_sms, int bn_reduce, int f32);
+void c1_describe_plan(long long M, int N, int K, int num_sms, int residual, int bn_reduce, int f32, int* out);
 cudaError_t c1_launch_gemm(const void* x, const void* w, void* y, long long M, int N, int K, float* partial,
-                           const void* residual, int num_sms, int f32, cudaStream_t st);
+                           const void* residual, const void* bn_x, const float* coef, const uint8_t* mask,
+                           int num_sms, int f32, cudaStream_t st);
 cudaError_t c1_launch_stats_finalize(const float* partial, int R, int C, const float* gamma, const float* beta,
                                      float* rmean, float* rvar, long long* nbt, float momentum, float eps,
                                      float* mean, float* invstd, float* scale, float* shift, cudaStream_t st);
@@ -309,15 +336,16 @@ static torch::Tensor conv1x1_alloc_out(const torch::Tensor& x, int N)
 }
 
 // host-side launch plan of the GEMM for a shape (no GPU needed)
-static py::dict conv1x1_plan(long long M, int N, int K, int num_sms, bool residual, bool f32)
+// (bn_reduce: the MODE 3 dgrad + BatchNorm backward reduction, which implies a residual)
+static py::dict conv1x1_plan(long long M, int N, int K, int num_sms, bool residual, bool f32, bool bn_reduce)
 {
     TORCH_CHECK(c1_supported(M, N, K, f32), "unsupported GEMM shape");
     int v[7];
-    c1_describe_plan(M, N, K, num_sms, residual ? 1 : 0, f32 ? 1 : 0, v);
+    c1_describe_plan(M, N, K, num_sms, residual ? 1 : 0, bn_reduce ? 1 : 0, f32 ? 1 : 0, v);
     py::dict d;
     d["block_n"] = v[0]; d["grid"] = v[1]; d["ctas_per_n"] = v[2]; d["stages"] = v[3];
     d["resident_w"] = v[4] != 0; d["store_slabs"] = v[5]; d["smem_bytes"] = v[6];
-    d["partial_rows"] = c1_partial_rows(M, N, K, num_sms, f32 ? 1 : 0);
+    d["partial_rows"] = c1_partial_rows(M, N, K, num_sms, bn_reduce ? 1 : 0, f32 ? 1 : 0);
     return d;
 }
 
@@ -343,23 +371,54 @@ static torch::Tensor conv1x1_forward(torch::Tensor x, torch::Tensor w, bool with
                     "conv1x1_forward: residual must match the output's shape and layout");
     torch::Tensor partial;
     if (with_stats)
-        partial = torch::empty({c1_partial_rows(M, N, K, sm_count(), f32), 3, N},
+        partial = torch::empty({c1_partial_rows(M, N, K, sm_count(), 0, f32), 3, N},
                                torch::TensorOptions().dtype(torch::kFloat32).device(x.device()));
     BN_CHECK(c1_launch_gemm(x.data_ptr(), w.data_ptr(), y.data_ptr(), M, N, K,
                             with_stats ? partial.data_ptr<float>() : nullptr,
-                            has_res ? residual->data_ptr() : nullptr, sm_count(), f32,
+                            has_res ? residual->data_ptr() : nullptr, nullptr, nullptr, nullptr, sm_count(), f32,
                             at::cuda::getCurrentCUDAStream()));
     return y;
 }
 
-// training-mode  out = act(bn(conv1x1(x, w)) [+ residual]);  returns (conv output, out, coef)
+// MODE 3: dz = mask ? x . w^T + residual : 0 and the backward reduction of the BatchNorm (+ residual
+// + ReLU) whose input was bn_x, output mask `mask` ([M, N/8] uint8) and coefficients `coef` ([4, N]:
+// mean, invstd, scale, shift).  Returns (dz, partial[R][2][N]) for bn_backward_from_partials.
+static std::vector<torch::Tensor> conv1x1_dgrad_bn_reduce(torch::Tensor x, torch::Tensor w, torch::Tensor residual,
+                                                          torch::Tensor bn_x, torch::Tensor coef, torch::Tensor mask)
+{
+    TORCH_CHECK(conv1x1_can_fuse(x, w), "conv1x1_dgrad_bn_reduce: unsupported tensors");
+    const int K = (int)x.size(1), N = (int)w.size(0);
+    const long long M = x.numel() / K;
+    c10::cuda::CUDAGuard guard(x.get_device());
+    auto y = conv1x1_alloc_out(x, N);
+    for (const torch::Tensor* t : {&residual, &bn_x})
+        TORCH_CHECK(t->is_cuda() && t->scalar_type() == x.scalar_type() && t->sizes() == y.sizes() &&
+                    t->strides() == y.strides() && (reinterpret_cast<uintptr_t>(t->data_ptr()) & 15) == 0,
+                    "conv1x1_dgrad_bn_reduce: residual / bn_x must match the output's shape and layout");
+    TORCH_CHECK(coef.is_cuda() && coef.scalar_type() == torch::kFloat32 && coef.is_contiguous() &&
+                coef.dim() == 2 && coef.size(1) == N && coef.size(0) >= 2);
+    TORCH_CHECK(mask.is_cuda() && mask.scalar_type() == torch::kUInt8 && mask.is_contiguous() &&
+                mask.numel() == M * (N / 8) && (reinterpret_cast<uintptr_t>(mask.data_ptr()) & 15) == 0,
+                "conv1x1_dgrad_bn_reduce: mask must be [M, N/8] uint8");
+    const int f32 = x.scalar_type() == torch::kFloat32 ? 1 : 0;
+    auto partial = torch::empty({c1_partial_rows(M, N, K, sm_count(), 1, f32), 2, N},
+                                torch::TensorOptions().dtype(torch::kFloat32).device(x.device()));
+    BN_CHECK(c1_launch_gemm(x.data_ptr(), w.data_ptr(), y.data_ptr(), M, N, K, partial.data_ptr<float>(),
+                            residual.data_ptr(), bn_x.data_ptr(), coef.data_ptr<float>(), mask.data_ptr<uint8_t>(),
+                            sm_count(), f32, at::cuda::getCurrentCUDAStream()));
+    return {y, partial};
+}
+
+// training-mode  out = act(bn(conv1x1(x, w)) [+ residual]);  returns (conv output, out, coef).
+// mask (optional, residual + relu only): filled with out's 1-bit ReLU mask, [M, N/8] uint8
 static std::vector<torch::Tensor> conv1x1_bn_forward(torch::Tensor x, torch::Tensor w,
                                                      c10::optional<torch::Tensor> residual,
                                                      torch::Tensor gamma, torch::Tensor beta,
                                                      c10::optional<torch::Tensor> running_mean,
                                                      c10::optional<torch::Tensor> running_var,
                                                      c10::optional<torch::Tensor> num_batches_tracked,
-                                                     double momentum, double eps, bool relu)
+                                                     double momentum, double eps, bool relu,
+                                                     c10::optional<torch::Tensor> mask)
 {
     TORCH_CHECK(conv1x1_can_fuse(x, w), "conv1x1_bn_forward: unsupported tensors");
     const int K = (int)x.size(1), N = (int)w.size(0);
@@ -375,10 +434,15 @@ static std::vector<torch::Tensor> conv1x1_bn_forward(torch::Tensor x, torch::Ten
                              && residual->strides() == yraw.strides());
     const int sms = sm_count();
     const int f32 = x.scalar_type() == torch::kFloat32 ? 1 : 0;
-    const int R = c1_partial_rows(M, N, K, sms, f32);
+    const bool has_mask = mask.has_value() && mask->defined();
+    if (has_mask)
+        TORCH_CHECK(has_res && relu && mask->is_cuda() && mask->scalar_type() == torch::kUInt8 &&
+                    mask->is_contiguous() && mask->numel() == M * (N / 8),
+                    "conv1x1_bn_forward: mask must be [M, N/8] uint8 (residual + relu only)");
+    const int R = c1_partial_rows(M, N, K, sms, 0, f32);
     auto partial = torch::empty({R, 3, N}, fopt);
     BN_CHECK(c1_launch_gemm(x.data_ptr(), w.data_ptr(), yraw.data_ptr(), M, N, K, partial.data_ptr<float>(),
-                            nullptr, sms, f32, st));
+                            nullptr, nullptr, nullptr, nullptr, sms, f32, st));
     auto coef = torch::empty({4, N}, fopt);      // mean, invstd, scale, shift
     float* mean = coef.data_ptr<float>();
     float* rm = nullptr; float* rv = nullptr; long long* nbt = nullptr;
@@ -394,7 +458,7 @@ static std::vector<torch::Tensor> conv1x1_bn_forward(torch::Tensor x, torch::Ten
     auto out = torch::empty_like(yraw);
     BN_CHECK(bn_launch_apply(f32, relu ? 1 : 0, has_res ? 1 : 0, yraw.data_ptr(),
                              has_res ? residual->data_ptr() : nullptr, mean + 2 * N, mean + 3 * N,
-                             out.data_ptr(), M, N, st));
+                             out.data_ptr(), has_mask ? mask->data_ptr<uint8_t>() : nullptr, M, N, st));
     return {yraw, out, coef};
 }
 
@@ -454,10 +518,14 @@ void bind_bn(py::module& mod)
     mod.def("xent_backward", &xent_backward);
     mod.def("conv1x1_can_fuse", &conv1x1_can_fuse);
     mod.def("conv1x1_plan", &conv1x1_plan, py::arg("M"), py::arg("N"), py::arg("K"), py::arg("num_sms") = 132,
-            py::arg("residual") = false, py::arg("f32") = false);
+            py::arg("residual") = false, py::arg("f32") = false, py::arg("bn_reduce") = false);
     mod.def("conv1x1_forward", &conv1x1_forward, py::arg("x"), py::arg("w"), py::arg("with_stats") = false,
             py::arg("residual") = py::none());
-    mod.def("conv1x1_bn_forward", &conv1x1_bn_forward);
+    mod.def("conv1x1_bn_forward", &conv1x1_bn_forward, py::arg("x"), py::arg("w"), py::arg("residual"),
+            py::arg("gamma"), py::arg("beta"), py::arg("running_mean"), py::arg("running_var"),
+            py::arg("num_batches_tracked"), py::arg("momentum"), py::arg("eps"), py::arg("relu"),
+            py::arg("mask") = py::none());
+    mod.def("conv1x1_dgrad_bn_reduce", &conv1x1_dgrad_bn_reduce);
     mod.def("stem_can_fuse", &stem_can_fuse);
     mod.def("stem_forward", &stem_forward);
     mod.def("stem_wgrad", &stem_wgrad);
@@ -467,4 +535,5 @@ void bind_bn(py::module& mod)
     mod.def("bn_can_fuse", &bn_can_fuse);
     mod.def("bn_forward", &bn_forward);
     mod.def("bn_backward", &bn_backward);
+    mod.def("bn_backward_from_partials", &bn_backward_from_partials);
 }

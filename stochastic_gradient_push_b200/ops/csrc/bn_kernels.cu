@@ -222,11 +222,13 @@ __global__ void bn_eval_coeff_kernel(int C, const float* __restrict__ gamma, con
 
 // ---------------------------------------------------------------------------
 // forward: apply   y = act(x*scale + shift [+ res])
+// MASK: also mask[M, C/8], bit i of byte j = (y[row, 8j+i] > 0) -- the ReLU mask of a residual block's
+// output for the next block's conv1 dgrad (MODE 3 of conv1x1_kernels.cu), 1/32 of y's fp32 bytes
 // ---------------------------------------------------------------------------
-template <typename T, bool RELU, bool ADD>
+template <typename T, bool RELU, bool ADD, bool MASK = false>
 __global__ void __launch_bounds__(BN_THREADS, (sizeof(T) == 4 && ADD) ? 3 : 4)     // fp32 + residual: 80 registers
 bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, const float* __restrict__ scale,
-                const float* __restrict__ shift, T* __restrict__ y, long long M, int C)
+                const float* __restrict__ shift, T* __restrict__ y, uint8_t* __restrict__ mask, long long M, int C)
 {
     const Map mp(C);
     if (!mp.active) return;
@@ -253,14 +255,20 @@ bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, const float*
                 F8 a;
                 if (ADD) a = Io<T>::decode(ar[u]);
                 F8 o;
+                uint32_t bits = 0;
 #pragma unroll
                 for (int i = 0; i < 8; ++i) {
                     float v = fmaf(d.v[i], sc.v[i], sh.v[i]);
                     if (ADD) v += a.v[i];
                     if (RELU) v = fmaxf(v, 0.f);
                     o.v[i] = v;
+                    if (MASK) {     // the sign of y as stored (bf16 rounds the tiniest positives to 0)
+                        const float vs = sizeof(T) == 2 ? __bfloat162float(__float2bfloat16_rn(v)) : v;
+                        bits |= (vs > 0.f ? 1u : 0u) << i;
+                    }
                 }
                 Io<T>::store(y + rr * C + off, o);
+                if (MASK) mask[rr * (C / BN_VEC) + mp.cv] = (uint8_t)bits;
             }
         }
     }
@@ -447,13 +455,22 @@ cudaError_t bn_launch_eval_coeff(int C, const float* gamma, const float* beta, c
 }
 
 #define BN_APPLY(T, R, A) bn_apply_kernel<T, R, A><<<G, BN_THREADS, 0, st>>>( \
-    (const T*)x, (const T*)res, scale, shift, (T*)y, M, C)
+    (const T*)x, (const T*)res, scale, shift, (T*)y, nullptr, M, C)
 
+// mask (nullable; relu && add only): the 1-bit ReLU mask [M, C/8] of y
 cudaError_t bn_launch_apply(int dtype, int relu, int add, const void* x, const void* res,
-                            const float* scale, const float* shift, void* y, long long M, int C,
+                            const float* scale, const float* shift, void* y, uint8_t* mask, long long M, int C,
                             cudaStream_t st)
 {
     const int G = bn_grid(M, C, (dtype == 1 && add) ? 6 : 8);   // fp32 + residual holds 3 CTAs/SM: 2 waves
+    if (mask != nullptr) {
+        if (!(relu && add)) return cudaErrorInvalidValue;
+        if (dtype == 0) bn_apply_kernel<__nv_bfloat16, true, true, true><<<G, BN_THREADS, 0, st>>>(
+            (const __nv_bfloat16*)x, (const __nv_bfloat16*)res, scale, shift, (__nv_bfloat16*)y, mask, M, C);
+        else bn_apply_kernel<float, true, true, true><<<G, BN_THREADS, 0, st>>>(
+            (const float*)x, (const float*)res, scale, shift, (float*)y, mask, M, C);
+        return cudaGetLastError();
+    }
     if (dtype == 0) {
         if (relu && add) BN_APPLY(__nv_bfloat16, true, true);
         else if (relu)   BN_APPLY(__nv_bfloat16, true, false);

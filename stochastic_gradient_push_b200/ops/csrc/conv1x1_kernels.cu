@@ -39,6 +39,13 @@
 //           slab), summed in fp32 before the single bf16 rounding.  Used as the dgrad of the first
 //           convolution of a residual block with R = the skip-branch gradient, which replaces
 //           autograd's read-read-write accumulation pass over the block's widest tensor.
+//   MODE 3  MODE 2 + the backward reduction of the BatchNorm (+ residual + ReLU) that produced this
+//           dgrad's input X' in the previous block:  dz = mask ? X.W^T + R : 0 is stored, and per
+//           channel sum(dz) and sum(dz * (x' - mean) * invstd) are accumulated, x' being the BN's
+//           input (a second TMA slab stream shaped like R), mean / invstd from its coefficients and
+//           mask its 1-bit ReLU mask [M, N/8] (plain loads).  The statistics are read back from the
+//           stored (rounded) slab like MODE 1's and merged into partial[ctas_per_n][2][N], the layout
+//           bn_bwd_finalize_kernel consumes; the stand-alone reduce pass over dy / x' / out is gone.
 //
 // Timing: benchmarks/conv1x1_bench.py.
 //
@@ -327,14 +334,17 @@ struct C1Plan {            // host-computed shared-memory plan (bytes are multip
 };
 
 // MODE 0: Y = X.W^T          MODE 1: + BatchNorm statistics of Y          MODE 2: Y = X.W^T + R
+// MODE 3: dz = mask ? X.W^T + R : 0, + BatchNorm backward reduction against bn_x (tm_b), coef, mask
 template <int BN, int MODE, bool F32>
 __global__ void __launch_bounds__(kThreads, 1)
 c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w,
-               const __grid_constant__ CUtensorMap tm_y, const __grid_constant__ CUtensorMap tm_r, int M, int N,
-               int K, float* __restrict__ partial, const C1Plan plan)
+               const __grid_constant__ CUtensorMap tm_y, const __grid_constant__ CUtensorMap tm_r,
+               const __grid_constant__ CUtensorMap tm_b, int M, int N, int K, float* __restrict__ partial,
+               const float* __restrict__ coef, const uint8_t* __restrict__ mask, const C1Plan plan)
 {
     constexpr bool STATS = MODE == 1;
-    constexpr bool RES = MODE == 2;
+    constexpr bool RES = MODE >= 2;
+    constexpr bool BNR = MODE == 3;
     constexpr int BK = Elt<F32>::BK;
     constexpr int MMA_K = Elt<F32>::MMA_K;
     constexpr int COLS = Elt<F32>::COLS;
@@ -356,12 +366,14 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
     const bool resident = plan.resident != 0;
     const int nbuf = plan.nbuf;
 
-    // [ resident W : k_blocks x B_BYTES ][ ring : stages x (X tile [+ W tile]) ][ store slabs ][ barriers ]
+    // [ resident W : k_blocks x B_BYTES ][ ring : stages x (X tile [+ W tile]) ][ store slabs ]
+    // [ MODE 3: bn_x slabs, 8 warps x 2 ][ barriers ]
     uint8_t* sW = smem;
     uint8_t* ring = sW + (resident ? k_blocks * B_BYTES : 0);
     const int stage_bytes = A_BYTES + (resident ? 0 : B_BYTES);
     uint8_t* sO = ring + stages * stage_bytes;
-    uint64_t* full = reinterpret_cast<uint64_t*>(sO + 8 * nbuf * SLAB_BYTES);
+    uint8_t* sB = sO + 8 * nbuf * SLAB_BYTES;
+    uint64_t* full = reinterpret_cast<uint64_t*>(sB + (BNR ? 16 * SLAB_BYTES : 0));
     uint64_t* empty = full + MAX_STAGES;
     uint64_t* wfull = empty + MAX_STAGES;    // resident W landed
     uint64_t* rbar0 = wfull + 1;             // MODE 2: residual slab landed, [8 warps][2 slots]
@@ -373,6 +385,7 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         for (int i = 0; i < stages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], kMmaWarps); }
         mbar_init(wfull, 1);
         if (RES) { tma_prefetch_desc(&tm_r); for (int i = 0; i < 16; ++i) mbar_init(&rbar0[i], 1); }
+        if (BNR) tma_prefetch_desc(&tm_b);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -430,12 +443,16 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         const uint32_t rbar = smem_u32(rbar0 + e * 2);
         uint32_t rphase = 0;                                     // bit b: parity of slab b's barrier
         const int tile_step = ctas_per_n;
+        // MODE 3: the bn_x slab of the same rows / columns lands on the residual slab's barrier
+        const uint32_t bslab0 = smem_u32(sB) + (uint32_t)(e * 2 * SLAB_BYTES);
+        constexpr uint32_t R_TX = (BNR ? 2 : 1) * SLAB_BYTES;
         if (RES && lane == 0) {
             const int mt0 = j;
             if (mt0 < m_tiles && M - mt0 * BM - row0 > 0) {
-                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(rbar), "r"(SLAB_BYTES)
+                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(rbar), "r"(R_TX)
                              : "memory");
                 tma_load_2d_s(&tm_r, rbar, slab0, nb * BN, mt0 * BM + row0, L2_EVICT_FIRST);
+                if (BNR) tma_load_2d_s(&tm_b, rbar, bslab0, nb * BN, mt0 * BM + row0, L2_EVICT_FIRST);
             }
         }
         if (resident) mbar_wait(wfull, 0);
@@ -479,6 +496,24 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
                     }
                     __syncwarp();
                 }
+                // MODE 3: this lane's mask bits of rows r0 and r0 + 8, one byte per 8-column group c:
+                // bit 2*(lane%4) + i%2 of byte c is element d[4c + i].  Issued before the slab wait.
+                uint32_t mk[2][2] = {{0u, 0u}, {0u, 0u}};     // [row r0 / r0 + 8][bytes 0-3 / 4-7]
+                if (BNR && nrows > 0) {
+                    const size_t pitch = (size_t)(N / 8);
+                    const uint8_t* mp = mask + (size_t)(mt * BM + row0 + r0) * pitch + (nb * BN + s * COLS) / 8;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        if (r0 + 8 * h < nrows) {
+                            if (F32) {
+                                mk[h][0] = __ldg(reinterpret_cast<const unsigned int*>(mp + 8 * h * pitch));
+                            } else {
+                                const uint2 v = __ldg(reinterpret_cast<const uint2*>(mp + 8 * h * pitch));
+                                mk[h][0] = v.x; mk[h][1] = v.y;
+                            }
+                        }
+                    }
+                }
                 if (RES && nrows > 0) {
                     const uint32_t bar = rbar + (uint32_t)(slot * 8);
                     const uint32_t par = (rphase >> slot) & 1u;
@@ -502,6 +537,9 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
                         const uint32_t chunk = F32 ? (uint32_t)(2 * c + ((lane & 3) >> 1)) : (uint32_t)c;
                         const uint32_t addr = slab + wr_off + ((chunk ^ (uint32_t)(r0 & 7)) << 4) +
                                               (F32 ? (uint32_t)((lane & 1) * 8) : rd_off);
+                        // MODE 3 keep bits of d[0..3] (c is a compile-time index)
+                        const uint32_t msh = (uint32_t)(8 * (c & 3) + 2 * (lane & 3));
+                        const uint32_t mlo = mk[0][c >> 2] >> msh, mhi = mk[1][c >> 2] >> msh;
                         if (F32) {
                             float v0 = d[0], v1 = d[1], v2 = d[2], v3 = d[3];
                             if (RES) {
@@ -510,6 +548,10 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
                                 asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(a2), "=f"(a3) : "r"(addr + 1024u)
                                              : "memory");
                                 v0 += a0; v1 += a1; v2 += a2; v3 += a3;
+                            }
+                            if (BNR) {
+                                v0 = (mlo & 1u) ? v0 : 0.f; v1 = (mlo & 2u) ? v1 : 0.f;
+                                v2 = (mhi & 1u) ? v2 : 0.f; v3 = (mhi & 2u) ? v3 : 0.f;
                             }
                             asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v0), "f"(v1) : "memory");
                             asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr + 1024u), "f"(v2), "f"(v3)
@@ -522,6 +564,10 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
                                 asm volatile("ld.shared.b32 %0, [%1];" : "=r"(b) : "r"(addr + 1024u) : "memory");
                                 v0 += __uint_as_float(a << 16); v1 += __uint_as_float(a & 0xFFFF0000u);
                                 v2 += __uint_as_float(b << 16); v3 += __uint_as_float(b & 0xFFFF0000u);
+                            }
+                            if (BNR) {
+                                v0 = (mlo & 1u) ? v0 : 0.f; v1 = (mlo & 2u) ? v1 : 0.f;
+                                v2 = (mhi & 1u) ? v2 : 0.f; v3 = (mhi & 2u) ? v3 : 0.f;
                             }
                             asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr),
                                          "r"(pack_bf16(__float_as_uint(v0), __float_as_uint(v1))) : "memory");
@@ -542,11 +588,44 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
                             asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");   // other slab is free
                             const uint32_t nbar = rbar + (uint32_t)((slot ^ 1) * 8);
                             asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(nbar),
-                                         "r"(SLAB_BYTES)
+                                         "r"(R_TX)
                                          : "memory");
                             tma_load_2d_s(&tm_r, nbar, slab0 + (uint32_t)((slot ^ 1) * SLAB_BYTES), nb * BN + ns * COLS,
                                           nmt * BM + row0, L2_EVICT_FIRST);
+                            // (its previous contents were read back by every lane before the __syncwarp above)
+                            if (BNR)
+                                tma_load_2d_s(&tm_b, nbar, bslab0 + (uint32_t)((slot ^ 1) * SLAB_BYTES),
+                                              nb * BN + ns * COLS, nmt * BM + row0, L2_EVICT_FIRST);
                         }
+                    }
+                }
+                if (BNR && nrows > 0) {
+                    // lane = channel (fp32) / channel pair (bf16), as in MODE 1: dz from the stored slab,
+                    // x' from the bn_x slab at the same swizzled offset
+                    const uint32_t rd = slab + rd_off;
+                    const uint32_t rb = bslab0 + (uint32_t)(slot * SLAB_BYTES) + rd_off;
+                    const int ch = nb * BN + s * COLS + (F32 ? lane : 2 * lane);
+                    const float mu0 = __ldg(coef + ch), is0 = __ldg(coef + N + ch);
+                    const float mu1 = F32 ? 0.f : __ldg(coef + ch + 1), is1 = F32 ? 0.f : __ldg(coef + N + ch + 1);
+                    auto acc_row = [&](int r) {
+                        const uint32_t o = (uint32_t)(r * 128 + ((rd_chunk ^ (r & 7)) << 4));
+                        uint32_t u, b;
+                        asm volatile("ld.shared.b32 %0, [%1];" : "=r"(u) : "r"(rd + o));
+                        asm volatile("ld.shared.b32 %0, [%1];" : "=r"(b) : "r"(rb + o));
+                        const float g0 = F32 ? __uint_as_float(u) : __uint_as_float(u << 16);
+                        const float x0 = F32 ? __uint_as_float(b) : __uint_as_float(b << 16);
+                        s0[s] += g0; q0[s] = fmaf(g0, (x0 - mu0) * is0, q0[s]);
+                        if (!F32) {
+                            const float g1 = __uint_as_float(u & 0xFFFF0000u);
+                            const float x1 = __uint_as_float(b & 0xFFFF0000u);
+                            s1[s] += g1; q1[s] = fmaf(g1, (x1 - mu1) * is1, q1[s]);
+                        }
+                    };
+                    if (nrows == 16) {
+#pragma unroll
+                        for (int r = 0; r < 16; ++r) acc_row(r);
+                    } else {
+                        for (int r = 0; r < nrows; ++r) acc_row(r);
                     }
                 }
                 if (STATS && nrows > 0) {
@@ -634,6 +713,30 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
                 p[0] = n_tot;
                 p[N] = mu;
                 p[2 * (size_t)N] = m2;
+            }
+        }
+        if (BNR) {
+            // the eight warps' (sum dz, sum dz*xhat) merged into partial[j][2][N] (ring as scratch, as above)
+            asm volatile("bar.sync 1, %0;" ::"n"(kMmaWarps * 32) : "memory");
+            float2* sc = reinterpret_cast<float2*>(ring);
+#pragma unroll
+            for (int s = 0; s < NS; ++s) {
+                if (F32) {
+                    sc[e * BN + s * COLS + lane] = make_float2(s0[s], q0[s]);
+                } else {
+                    sc[e * BN + s * COLS + 2 * lane] = make_float2(s0[s], q0[s]);
+                    sc[e * BN + s * COLS + 2 * lane + 1] = make_float2(s1[s], q1[s]);
+                }
+            }
+            asm volatile("bar.sync 1, %0;" ::"n"(kMmaWarps * 32) : "memory");
+            const int t = (int)threadIdx.x;
+            if (t < BN) {
+                float a = 0.f, b = 0.f;
+#pragma unroll
+                for (int i = 0; i < 8; ++i) { const float2 v = sc[i * BN + t]; a += v.x; b += v.y; }
+                float* p = partial + (size_t)j * 2 * N + nb * BN + t;
+                p[0] = a;
+                p[N] = b;
             }
         }
         if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
@@ -798,18 +901,21 @@ bool fits_resident(int bn, int K, bool f32)
     return SMEM_LIMIT - SMEM_FIXED - 8 * SLAB_BYTES - k_blocks * bn * ROW_BYTES >= 3 * A_BYTES;
 }
 
-int pick_bn(long long M, int N, int K, int num_sms, bool f32)
+// MODE 3 (bn_reduce) runs at most 128 wide: at 256 its 128 accumulators per thread plus the reduction
+// state exceed the 168 registers a 288-thread CTA gets, and the kernel spills.
+int pick_bn(long long M, int N, int K, int num_sms, bool f32, bool bn_reduce)
 {
     const long long m_tiles = (M + BM - 1) / BM;
     int best = 0;
     long long best_cost = 0;
+    const int cap = bn_reduce ? 128 : 256;
     const int force = bn_override();
-    if (force >= 64 && force <= 256 && N % force == 0) return force;
+    if (force >= 64 && force <= cap && N % force == 0) return force;
     // fp32 operands are twice as wide: prefer the widest tile whose W block stays resident (a
     // non-resident 256-wide tile re-streams 3x the bytes of X per row tile through L2)
-    int bn_max = 256;
+    int bn_max = cap;
     if (f32 && c1_f32_prefer_resident())
-        for (int bn = 256; bn >= 128; bn >>= 1)      // (a 64-wide tile re-reads X once per 64 channels)
+        for (int bn = cap; bn >= 128; bn >>= 1)      // (a 64-wide tile re-reads X once per 64 channels)
             if (N % bn == 0 && fits_resident(bn, K, true)) { bn_max = bn; break; }
     for (int bn = bn_max; bn >= 64; bn >>= 1) {
         if (N % bn) continue;
@@ -821,9 +927,10 @@ int pick_bn(long long M, int N, int K, int num_sms, bool f32)
     return best;
 }
 
-void grid_shape(long long M, int N, int K, int num_sms, bool f32, int& bn, int& ctas_per_n, int& grid)
+void grid_shape(long long M, int N, int K, int num_sms, bool f32, bool bn_reduce, int& bn, int& ctas_per_n,
+                int& grid)
 {
-    bn = pick_bn(M, N, K, num_sms, f32);
+    bn = pick_bn(M, N, K, num_sms, f32, bn_reduce);
     const int n_blocks = N / bn;
     const long long m_tiles = (M + BM - 1) / BM;
     long long per = num_sms / n_blocks;
@@ -835,36 +942,42 @@ void grid_shape(long long M, int N, int K, int num_sms, bool f32, int& bn, int& 
 
 // Shared-memory plan.  W stays resident when the CTA's [BN, K] block plus a >= 3-deep X ring
 // fits (then every row tile costs one 16 KB X load instead of X + W); the store slabs shrink
-// from 2 to 1 per warp if that is what makes it fit.
-C1Plan make_plan(int bn, int K, int n_blocks, bool residual, bool f32, int& smem_bytes)
+// from 2 to 1 per warp if that is what makes it fit.  MODE 3 adds 8 x 2 bn_x slabs.
+C1Plan make_plan(int bn, int K, int n_blocks, bool residual, bool bn_reduce, bool f32, int& smem_bytes)
 {
     const int bk = f32 ? Elt<true>::BK : Elt<false>::BK;
     const int k_blocks = (K + bk - 1) / bk;
     const int b_bytes = bn * ROW_BYTES;
+    const int extra = bn_reduce ? 16 * SLAB_BYTES : 0;
+    residual = residual || bn_reduce;
     C1Plan p;
     p.x_hint_first = n_blocks == 1;
     p.resident = 0;
     p.nbuf = 2;
-    for (int nbuf = 2; nbuf >= (residual ? 2 : 1) && !p.resident; --nbuf) {   // MODE 2 double-buffers its slabs
-        const int ring = SMEM_LIMIT - SMEM_FIXED - 8 * nbuf * SLAB_BYTES - k_blocks * b_bytes;
+    for (int nbuf = 2; nbuf >= (residual ? 2 : 1) && !p.resident; --nbuf) {   // MODE 2/3 double-buffer their slabs
+        const int ring = SMEM_LIMIT - SMEM_FIXED - extra - 8 * nbuf * SLAB_BYTES - k_blocks * b_bytes;
         if (ring >= 3 * A_BYTES) { p.resident = 1; p.nbuf = nbuf; }
     }
     const int stage_bytes = A_BYTES + (p.resident ? 0 : b_bytes);
-    const int ring = SMEM_LIMIT - SMEM_FIXED - 8 * p.nbuf * SLAB_BYTES - (p.resident ? k_blocks * b_bytes : 0);
+    const int ring = SMEM_LIMIT - SMEM_FIXED - extra - 8 * p.nbuf * SLAB_BYTES - (p.resident ? k_blocks * b_bytes : 0);
     p.stages = ring / stage_bytes;
     if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
     smem_bytes = SMEM_FIXED + (p.resident ? k_blocks * b_bytes : 0) + p.stages * stage_bytes +
-                 8 * p.nbuf * SLAB_BYTES;
+                 8 * p.nbuf * SLAB_BYTES + extra;
     return p;
 }
 
 template <int BN, bool F32>
 cudaError_t launch(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap& ty, const CUtensorMap& tr,
-                   int M, int N, int K, float* partial, int mode, int grid, cudaStream_t st)
+                   const CUtensorMap& tb, int M, int N, int K, float* partial, const float* coef,
+                   const uint8_t* mask, int mode, int grid, cudaStream_t st)
 {
+    constexpr int M3 = BN <= 128 ? 3 : 0;           // (no 256-wide MODE 3: see pick_bn)
+    if (mode == 3 && M3 != 3) return cudaErrorInvalidValue;
     auto kern = mode == 1 ? c1_gemm_kernel<BN, 1, F32>
-                          : (mode == 2 ? c1_gemm_kernel<BN, 2, F32> : c1_gemm_kernel<BN, 0, F32>);
-    static bool configured[3][64] = {};            // function attributes are per device (and per instantiation)
+              : mode == 2 ? c1_gemm_kernel<BN, 2, F32>
+              : mode == 3 ? c1_gemm_kernel<BN, M3, F32> : c1_gemm_kernel<BN, 0, F32>;
+    static bool configured[4][64] = {};            // function attributes are per device (and per instantiation)
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64 || !configured[mode][dev]) {
@@ -873,9 +986,9 @@ cudaError_t launch(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorM
         if (dev >= 0 && dev < 64) configured[mode][dev] = true;
     }
     int smem = 0;
-    const C1Plan plan = make_plan(BN, K, N / BN, mode == 2, F32, smem);
+    const C1Plan plan = make_plan(BN, K, N / BN, mode == 2, mode == 3, F32, smem);
     if (plan.stages < 2) return cudaErrorInvalidValue;
-    kern<<<grid, kThreads, smem, st>>>(tx, tw, ty, tr, M, N, K, partial, plan);
+    kern<<<grid, kThreads, smem, st>>>(tx, tw, ty, tr, tb, M, N, K, partial, coef, mask, plan);
     return cudaGetLastError();
 }
 
@@ -893,49 +1006,54 @@ int c1_supported(long long M, int N, int K, int f32)
 
 // launch plan for a shape (host logic only; exercised by the CPU tests):
 // out = {BLOCK_N, grid, ctas_per_n, stages, resident, nbuf, dynamic smem bytes}
-void c1_describe_plan(long long M, int N, int K, int num_sms, int residual, int f32, int* out)
+void c1_describe_plan(long long M, int N, int K, int num_sms, int residual, int bn_reduce, int f32, int* out)
 {
     int bn, per, grid, smem = 0;
-    grid_shape(M, N, K, num_sms, f32 != 0, bn, per, grid);
-    const C1Plan p = make_plan(bn, K, N / bn, residual != 0, f32 != 0, smem);
+    grid_shape(M, N, K, num_sms, f32 != 0, bn_reduce != 0, bn, per, grid);
+    const C1Plan p = make_plan(bn, K, N / bn, residual != 0, bn_reduce != 0, f32 != 0, smem);
     out[0] = bn; out[1] = grid; out[2] = per; out[3] = p.stages; out[4] = p.resident; out[5] = p.nbuf;
     out[6] = smem;
 }
 
-// number of partial-statistics rows c1_launch_gemm writes for this shape
-int c1_partial_rows(long long M, int N, int K, int num_sms, int f32)
+// number of partial-statistics rows c1_launch_gemm writes for this shape (bn_reduce: in MODE 3)
+int c1_partial_rows(long long M, int N, int K, int num_sms, int bn_reduce, int f32)
 {
     int bn, per, grid;
-    grid_shape(M, N, K, num_sms, f32 != 0, bn, per, grid);
+    grid_shape(M, N, K, num_sms, f32 != 0, bn_reduce != 0, bn, per, grid);
     return per;              // one merged partial row per CTA
 }
 
 // y[M,N] = x[M,K] . w[N,K]^T [+ residual[M,N]]; all operands bf16 (f32 == 0) or all fp32 with TF32
 // tensor-core math (f32 != 0); partial (nullable) = [c1_partial_rows][3][N] fp32 statistics of y.
-// partial and residual are mutually exclusive.
+// partial and residual are mutually exclusive, except in MODE 3 (mask != nullptr): then residual,
+// bn_x ([M, N], y's dtype), coef (mean [N], invstd [N]) and mask ([M, N/8] bytes) are all given,
+// y = dz and partial = [c1_partial_rows][2][N] (sum dz, sum dz * xhat).
 cudaError_t c1_launch_gemm(const void* x, const void* w, void* y, long long M, int N, int K, float* partial,
-                           const void* residual, int num_sms, int f32, cudaStream_t st)
+                           const void* residual, const void* bn_x, const float* coef, const uint8_t* mask,
+                           int num_sms, int f32, cudaStream_t st)
 {
-    if (!c1_supported(M, N, K, f32) || (partial && residual)) return cudaErrorInvalidValue;
-    const int mode = partial ? 1 : (residual ? 2 : 0);
+    if (!c1_supported(M, N, K, f32)) return cudaErrorInvalidValue;
+    if (mask ? !(partial && residual && bn_x && coef) : (partial && residual)) return cudaErrorInvalidValue;
+    const int mode = mask ? 3 : partial ? 1 : (residual ? 2 : 0);
     const bool f = f32 != 0;
     int bn, per, grid;
-    grid_shape(M, N, K, num_sms, f, bn, per, grid);
-    CUtensorMap tx, tw, ty, tr;
+    grid_shape(M, N, K, num_sms, f, mode == 3, bn, per, grid);
+    CUtensorMap tx, tw, ty, tr, tb;
     if (!make_map(&tx, x, M, K, BM, true, f) || !make_map(&tw, w, N, K, bn, true, f) ||
-        !make_map(&ty, y, M, N, 16, false, f) || !make_map(&tr, residual ? residual : y, M, N, 16, false, f))
+        !make_map(&ty, y, M, N, 16, false, f) || !make_map(&tr, residual ? residual : y, M, N, 16, false, f) ||
+        !make_map(&tb, bn_x ? bn_x : y, M, N, 16, false, f))
         return cudaErrorInvalidValue;
     if (f) {
         switch (bn) {
-        case 256: return launch<256, true>(tx, tw, ty, tr, (int)M, N, K, partial, mode, grid, st);
-        case 128: return launch<128, true>(tx, tw, ty, tr, (int)M, N, K, partial, mode, grid, st);
-        default: return launch<64, true>(tx, tw, ty, tr, (int)M, N, K, partial, mode, grid, st);
+        case 256: return launch<256, true>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st);
+        case 128: return launch<128, true>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st);
+        default: return launch<64, true>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st);
         }
     }
     switch (bn) {
-    case 256: return launch<256, false>(tx, tw, ty, tr, (int)M, N, K, partial, mode, grid, st);
-    case 128: return launch<128, false>(tx, tw, ty, tr, (int)M, N, K, partial, mode, grid, st);
-    default: return launch<64, false>(tx, tw, ty, tr, (int)M, N, K, partial, mode, grid, st);
+    case 256: return launch<256, false>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st);
+    case 128: return launch<128, false>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st);
+    default: return launch<64, false>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st);
     }
 }
 

@@ -48,6 +48,10 @@ USE_TCGEN05_CONV1X1 = os.environ.get('SGP_B200_CONV1X1', '1') != '0'
 # the tensor-core stem kernels (csrc/stem_kernels.cu); SGP_B200_STEM=0 -> library convolution
 USE_STEM_KERNELS = os.environ.get('SGP_B200_STEM', '1') != '0'
 
+# A residual block's last BN backward reduction runs inside the next block's conv1 dgrad GEMM
+# (MODE 3 of csrc/conv1x1_kernels.cu); SGP_B200_BN_BWD_FUSE=0 keeps the stand-alone reduce pass.
+USE_BN_BWD_FUSE = os.environ.get('SGP_B200_BN_BWD_FUSE', '1') != '0'
+
 
 def _can_fuse(x: torch.Tensor) -> bool:
     if FORCE_REFERENCE or not x.is_cuda or not native.available():
@@ -133,6 +137,20 @@ class FusedBatchNormAct2d(nn.BatchNorm2d):
 # --------------------------------------------------------------------------- #
 # 1x1 convolution + BatchNorm (+ residual) (+ ReLU)
 # --------------------------------------------------------------------------- #
+class _BNBackwardHandoff:
+    """What a residual block's last BN (``_Conv1x1BNAct`` with a residual) leaves on its output
+    so that the next block's conv1 dgrad (``_Conv1x1BNActSplit``) can do that BN's backward
+    reduction in its epilogue: the BN input ``yraw``, its ``coef`` and the output's 1-bit ReLU
+    ``mask``.  The dgrad records which tensor it produced (``dz_key``: data pointer and version)
+    and the reduction ``partial``; the BN backward uses them only if its incoming gradient is
+    that very tensor, unmodified."""
+    __slots__ = ('yraw', 'coef', 'mask', 'dz_key', 'partial')
+
+    def __init__(self, yraw, coef, mask):
+        self.yraw, self.coef, self.mask = yraw, coef, mask
+        self.dz_key = self.partial = None
+
+
 class _Conv1x1BNAct(torch.autograd.Function):
     """``act(bn(conv1x1(x, w)) [+ residual])`` in training mode.  Forward: wgmma GEMM
     whose epilogue also produces the BatchNorm statistics, finalize, apply.  Backward: the
@@ -142,11 +160,18 @@ class _Conv1x1BNAct(torch.autograd.Function):
     def forward(ctx, x, w, residual, gamma, beta, running_mean, running_var, nbt, momentum, eps, relu):
         C = native.load()
         w16 = w if w.dtype == x.dtype else w.detach().to(x.dtype)      # compute-dtype weights
+        mask = None
+        if residual is not None and relu and USE_BN_BWD_FUSE:
+            M, N = x.numel() // x.shape[1], w.shape[0]
+            mask = torch.empty((M, N // 8), dtype=torch.uint8, device=x.device)
         yraw, out, coef = C.conv1x1_bn_forward(x, w16, residual, gamma, beta, running_mean, running_var,
-                                               nbt, momentum, eps, relu)
+                                               nbt, momentum, eps, relu, mask)
         ctx.relu = relu
         ctx.add = residual is not None
         ctx.w_dtype = w.dtype
+        ctx.handoff = None
+        if mask is not None:
+            ctx.handoff = out._sgp_bn_handoff = _BNBackwardHandoff(yraw, coef, mask)
         if ctx.add:
             ctx.save_for_backward(x, w16, yraw, coef, out)
         else:
@@ -158,7 +183,16 @@ class _Conv1x1BNAct(torch.autograd.Function):
         C = native.load()
         x, w16, yraw, coef = ctx.saved_tensors[:4]
         out = ctx.saved_tensors[4] if ctx.add else None
-        dyraw, dz, ggamma, gbeta = C.bn_backward(dy, yraw, out, coef, ctx.relu, ctx.add)
+        h = ctx.handoff
+        if h is not None and h.dz_key == (dy.data_ptr(), dy._version) and dy.stride() == yraw.stride():
+            # dy is the next block's MODE 3 dgrad output: already masked (it is this BN's dz and the
+            # residual branch's gradient), its reduction already done
+            dyraw, ggamma, gbeta = C.bn_backward_from_partials(dy, yraw, coef, h.partial)
+            dz = dy
+        else:
+            dyraw, dz, ggamma, gbeta = C.bn_backward(dy, yraw, out, coef, ctx.relu, ctx.add)
+        if h is not None:
+            h.dz_key = h.partial = None
         dx, dw, _ = torch.ops.aten.convolution_backward(
             dyraw, x, w16, None, [1, 1], [0, 0], [1, 1], False, [0, 0], 1,
             [ctx.needs_input_grad[0], ctx.needs_input_grad[1], False])
@@ -174,13 +208,14 @@ class _Conv1x1BNActSplit(torch.autograd.Function):
     separate read-read-write accumulation pass over the widest activation of the block."""
 
     @staticmethod
-    def forward(ctx, x, w, gamma, beta, running_mean, running_var, nbt, momentum, eps, relu):
+    def forward(ctx, x, w, gamma, beta, running_mean, running_var, nbt, momentum, eps, relu, handoff):
         C = native.load()
         w16 = w if w.dtype == x.dtype else w.detach().to(x.dtype)
         yraw, out, coef = C.conv1x1_bn_forward(x, w16, None, gamma, beta, running_mean, running_var,
                                                nbt, momentum, eps, relu)
         ctx.relu = relu
         ctx.w_dtype = w.dtype
+        ctx.handoff = handoff
         ctx.save_for_backward(x, w16, yraw, coef)
         ctx.set_materialize_grads(False)
         return out, x.view_as(x)
@@ -200,7 +235,13 @@ class _Conv1x1BNActSplit(torch.autograd.Function):
             if res is not None and (res.dtype != dyraw.dtype
                                     or not res.is_contiguous(memory_format=torch.channels_last)):
                 res = res.to(dyraw.dtype).contiguous(memory_format=torch.channels_last)
-            if C.conv1x1_can_fuse(dyraw, wt):
+            h = ctx.handoff
+            if (h is not None and res is not None and h.yraw.dtype == dyraw.dtype
+                    and h.yraw.stride() == res.stride() and C.conv1x1_can_fuse(dyraw, wt)):
+                # + the previous block's last BN backward reduction (MODE 3): dx is that BN's dz
+                dx, h.partial = C.conv1x1_dgrad_bn_reduce(dyraw, wt, res, h.yraw, h.coef, h.mask)
+                h.dz_key = (dx.data_ptr(), dx._version)
+            elif C.conv1x1_can_fuse(dyraw, wt):
                 dx = C.conv1x1_forward(dyraw, wt, False, res)
             else:
                 dx = torch.ops.aten.convolution_backward(
@@ -212,7 +253,7 @@ class _Conv1x1BNActSplit(torch.autograd.Function):
                 dyraw, x, w16, None, [1, 1], [0, 0], [1, 1], False, [0, 0], 1, [False, True, False])[1]
             if dw.dtype != ctx.w_dtype:
                 dw = dw.to(ctx.w_dtype)
-        return dx, dw, ggamma, gbeta, None, None, None, None, None, None
+        return dx, dw, ggamma, gbeta, None, None, None, None, None, None, None
 
 
 def _conv1x1_operands(conv, bn, x, residual, relu):
@@ -255,13 +296,22 @@ def conv_bn_act(conv: nn.Conv2d, bn: 'FusedBatchNormAct2d', x, residual=None, re
 def conv_bn_act_split(conv: nn.Conv2d, bn: 'FusedBatchNormAct2d', x, relu=False):
     """``(bn(conv(x), relu=relu), x)`` for an ``x`` that is also consumed by a skip connection:
     use the returned ``x`` for the skip branch and its gradient is added inside the dgrad GEMM
-    of ``conv`` (see :class:`_Conv1x1BNActSplit`).  Falls back to ``(conv_bn_act(...), x)``."""
+    of ``conv`` (see :class:`_Conv1x1BNActSplit`).  Falls back to ``(conv_bn_act(...), x)``.
+
+    When ``x`` is the output of the previous block's fused last BN, that BN's backward reduction
+    also moves into the dgrad; the gradient ``x`` then receives is the post-ReLU-mask one, so this
+    is skipped when anyone can observe it (a hook on ``x`` or ``x.retain_grad()``)."""
     if x.requires_grad and torch.is_grad_enabled():
         xk, ok = _conv1x1_operands(conv, bn, x, None, relu)
         if ok and xk is x:
             momentum = 0.1 if bn.momentum is None else bn.momentum
+            handoff = getattr(x, '_sgp_bn_handoff', None)
+            if handoff is not None and (not USE_BN_BWD_FUSE or x._backward_hooks or x.retains_grad
+                                        or handoff.yraw.shape != x.shape):
+                handoff = None
             return _Conv1x1BNActSplit.apply(x, conv.weight, bn.weight, bn.bias, bn.running_mean,
-                                            bn.running_var, bn.num_batches_tracked, momentum, bn.eps, relu)
+                                            bn.running_var, bn.num_batches_tracked, momentum, bn.eps, relu,
+                                            handoff)
     return conv_bn_act(conv, bn, x, relu=relu), x
 
 

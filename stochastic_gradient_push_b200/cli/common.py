@@ -103,6 +103,10 @@ def build_parser(adpsgd: bool = False) -> argparse.ArgumentParser:
     p.add_argument('--amp', default=True, **B, help='bf16 autocast for forward/backward')
     p.add_argument('--channels_last', default=True, **B)
     p.add_argument('--transport', default='auto', choices=['auto', 'nvlink', 'c10d'])
+    p.add_argument('--gossip_dtype', default='fp32', choices=['fp32', 'bf16'],
+                   help='precision of the gossip messages (GossipDataParallel(gossip_dtype=...)): bf16 '
+                        'halves the bytes sent per in-neighbour and conserves push-sum mass exactly; '
+                        'parameters stay fp32.  Synchronous SGP and D-PSGD only')
     p.add_argument('--nprocs_per_node', default=1, type=int,
                    help='hierarchical mode (GossipDataParallel(nprocs_per_node=K), reference '
                         'gossip/distributed.py:62-80; it has no flag for it): K consecutive ranks form a '
@@ -185,6 +189,13 @@ def finalize_args(args, adpsgd=False):
     assert 0 in args.ppi_schedule, 'peers_per_itr_schedule must define epoch 0'
     if args.all_reduce:
         assert args.graph_type == -1, '--all_reduce needs --graph_type -1'
+    if args.gossip_dtype == 'bf16':
+        unsupported = ('AD-PSGD' if adpsgd else '--all_reduce' if args.all_reduce else
+                       '--overlap (OSGP)' if getattr(args, 'overlap', False) else
+                       '--nprocs_per_node > 1' if getattr(args, 'nprocs_per_node', 1) > 1 else None)
+        if unsupported:
+            raise ValueError('--gossip_dtype bf16 is not supported with %s; bf16 messages are '
+                             'implemented for synchronous SGP and D-PSGD' % unsupported)
 
     if args.backend == 'gloo' and args.network_interface_type == 'ethernet':
         try:

@@ -64,6 +64,7 @@ def build_model_and_optimizer(args, log):
         push_sum=args.push_sum, overlap=args.overlap, synch_freq=args.synch_freq,
         verbose=args.verbose, use_streams=not args.no_cuda_streams, rank=args.rank,
         world_size=args.world_size, transport=args.transport, nprocs_per_node=args.nprocs_per_node,
+        gossip_dtype=torch.bfloat16 if args.gossip_dtype == 'bf16' else None,
         # the captured fast path trains through the bf16 shadow-weight twin (no autocast casts)
         compute_dtype=(torch.bfloat16 if (args.cuda_graph and args.amp and args.fused
                                           and args.device == 'cuda' and args.transport != 'c10d')

@@ -38,6 +38,32 @@ from .mixing_manager import MixingManager, UniformMixing
 
 
 # --------------------------------------------------------------------------- #
+# bf16 message wire format (GossipDataParallel(gossip_dtype=torch.bfloat16), c10d plane)
+# --------------------------------------------------------------------------- #
+def bf16_message_numel(n: int) -> int:
+    """bf16 elements of one message carrying ``n`` values: the payload, padded to an even
+    length, then two slots holding the bit pattern of the fp32 push-sum weight (which must not
+    be rounded)."""
+    return n + (n & 1) + 2
+
+
+def pack_bf16_message(msg: torch.Tensor, x: torch.Tensor, scale: float, weight: float) -> torch.Tensor:
+    """Write Q(scale * x) and the fp32 ``weight`` into the bf16 buffer ``msg``.  Returns
+    Q(scale * x) on ``x``'s device, which the sender subtracts from its own numerator: it loses
+    exactly what the receiver gets, so push-sum mass is conserved."""
+    n = x.numel()
+    q = (x * scale).to(torch.bfloat16)
+    msg[:n].copy_(q, non_blocking=True)
+    msg[n:].zero_()
+    msg[n + (n & 1):].view(torch.float32).fill_(weight)
+    return q
+
+
+def bf16_message_weight(msg: torch.Tensor, n: int) -> float:
+    return float(msg[n + (n & 1):].view(torch.float32)[0])
+
+
+# --------------------------------------------------------------------------- #
 # transports
 # --------------------------------------------------------------------------- #
 class C10dTransport(object):

@@ -121,7 +121,8 @@ public:
                   c10::optional<torch::Tensor> shadow, c10::optional<torch::Tensor> residual,
                   torch::Tensor pad_ptrs, c10::optional<torch::Tensor> outbox_ptrs,
                   torch::Tensor table, torch::Tensor wtable, int rank, int world,
-                  torch::Tensor state, torch::Tensor hyper, double timeout_s)
+                  torch::Tensor state, torch::Tensor hyper, double timeout_s, bool msg_bf16,
+                  int64_t outbox_bytes)
     {
         TORCH_CHECK(z.is_cuda() && z.scalar_type() == torch::kFloat32 && z.is_contiguous(),
                     "z must be a contiguous fp32 CUDA tensor");
@@ -162,8 +163,13 @@ public:
         }
         args_.pads = reinterpret_cast<SgpSignalPad* const*>(pad_ptrs.data_ptr<int64_t>());
         keep_.push_back(pad_ptrs);
+        msg_bf16_ = msg_bf16;
         if (outbox_ptrs.has_value() && outbox_ptrs->defined()) {
             TORCH_CHECK(outbox_ptrs->scalar_type() == torch::kInt64 && outbox_ptrs->numel() == world);
+            // (every rank's outbox has the size of ours: symmetric allocations are equal)
+            const int64_t need = 2 * z.numel() * (msg_bf16 ? 2 : 4);
+            TORCH_CHECK(outbox_bytes < 0 || outbox_bytes >= need, "outbox of ", outbox_bytes,
+                        " bytes is too small for 2 x ", z.numel(), msg_bf16 ? " bf16" : " fp32", " messages");
             args_.outboxes = reinterpret_cast<float* const*>(outbox_ptrs->data_ptr<int64_t>());
             keep_.push_back(*outbox_ptrs);
         }
@@ -232,6 +238,13 @@ public:
     {
         check_grid(grid);
         SgpArgs a = prepare(flags);
+        if (msg_bf16_ && (a.flags & SGP_F_PUBLISH)) {     // (a local, unpublished update sends nothing)
+            const unsigned int full_step = SGP_F_PHASE1 | SGP_F_PUBLISH | SGP_F_PHASE2;
+            TORCH_CHECK((a.flags & full_step) == full_step &&
+                        (a.flags & (SGP_F_FOLD_RES | SGP_F_NO_ROTATE | SGP_F_KEEP_Z | SGP_F_SELF_FROM_Z)) == 0,
+                        "bf16 gossip messages support only the full synchronous step (SGP / D-PSGD)");
+            a.flags |= SGP_F_MSG_BF16;
+        }
         if (a.flags & SGP_F_SGD) TORCH_CHECK(a.g && a.m, "SGD needs grad + momentum buffers");
         if (a.flags & SGP_F_FOLD_RES) TORCH_CHECK(a.residual, "fold needs a residual buffer");
         if (a.flags & SGP_F_PUBLISH) TORCH_CHECK(a.outboxes, "publish needs outboxes");
@@ -248,6 +261,7 @@ public:
     // ---- AD-PSGD building blocks (all stream-ordered, no host decisions) ----
     void bilat_decide(int pub_grid, bool passive, double max_wait_us, c10::optional<torch::Tensor> host_fb)
     {
+        check_fp32_messages();
         SgpArgs a = prepare(0);
         uint32_t* fb = nullptr;
         if (host_fb.has_value() && host_fb->defined()) {
@@ -262,6 +276,7 @@ public:
     }
     void bilat_work(int grid)
     {
+        check_fp32_messages();
         check_grid(grid);
         SgpArgs a = prepare(SGP_F_FROM_STATE | (args_.shadow ? SGP_F_SHADOW : 0u));
         c10::cuda::CUDAGuard guard(device_);
@@ -275,12 +290,14 @@ public:
     // raw access for the native gossip daemon
     SgpArgs raw_args(unsigned int flags) const { return prepare(flags); }
     int device() const { return device_; }
+    bool msg_bf16() const { return msg_bf16_; }
 
     void set_pipe(bool on) { use_pipe_ = on; }
     bool pipe() const { return use_pipe_; }
 
     void gather(int grid, int pub_grid, bool tma)
     {
+        check_fp32_messages();
         check_grid(grid);
         SgpArgs a = prepare(0);
         TORCH_CHECK(a.residual && a.outboxes);
@@ -295,6 +312,7 @@ public:
     // residual) -> ack (1 thread).  `src_ptr`: address of the in-neighbour's outbox half of this step.
     void gather_dma(int pub_grid, int64_t src_ptr)
     {
+        check_fp32_messages();
         SgpArgs a = prepare(0);
         TORCH_CHECK(a.residual && a.outboxes && src_ptr != 0);
         c10::cuda::CUDAGuard guard(device_);
@@ -307,6 +325,7 @@ public:
 
     void probe(int pub_grid, c10::optional<torch::Tensor> host_flag)
     {
+        check_fp32_messages();
         SgpArgs a = prepare(0);
         uint32_t* hf = nullptr;
         if (host_flag.has_value() && host_flag->defined()) {
@@ -320,6 +339,7 @@ public:
 
     void allreduce_sgd(torch::Tensor grad_ptrs, unsigned int flags, int grid)
     {
+        check_fp32_messages();
         check_grid(grid);
         SgpArgs a = prepare(flags);
         TORCH_CHECK(a.m, "allreduce_sgd needs a momentum buffer");
@@ -350,6 +370,11 @@ private:
         if (!a.shadow) a.flags &= ~SGP_F_SHADOW;
         return a;
     }
+    void check_fp32_messages() const
+    {
+        TORCH_CHECK(!msg_bf16_, "this gossip operation is not implemented for bf16 messages "
+                    "(only the full synchronous SGP / D-PSGD step is)");
+    }
     void check_grid(int grid) const
     {
         TORCH_CHECK(grid >= 1 && grid <= SGP_MAX_CTAS, "grid out of range");
@@ -362,6 +387,7 @@ private:
     int device_ = 0;
     int max_grid_ = 0;
     bool grad_bf16_ = false;
+    bool msg_bf16_ = false;
     bool use_pipe_ = true;
     std::vector<torch::Tensor> keep_;
     std::vector<torch::Tensor> sched_keep_;
@@ -390,6 +416,7 @@ public:
         : ctx_(std::move(ctx)), grid_(grid), passive_(passive), max_wait_us_(max_wait_us),
           depth_(depth < 1 ? 1 : (depth > 8 ? 8 : depth)), idle_sleep_us_(idle_sleep_us)
     {
+        TORCH_CHECK(!ctx_->msg_bf16(), "the AD-PSGD gossip daemon does not support bf16 messages");
         device_ = ctx_->device();
         c10::cuda::CUDAGuard guard(device_);
         int lo = 0, hi = 0;
@@ -656,6 +683,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, mod)
     mod.attr("F_IN_NUMER") = (unsigned)SGP_F_IN_NUMER;
     mod.attr("F_KEEP_Z") = (unsigned)SGP_F_KEEP_Z;
     mod.attr("F_SELF_FROM_Z") = (unsigned)SGP_F_SELF_FROM_Z;
+    mod.attr("F_MSG_BF16") = (unsigned)SGP_F_MSG_BF16;
 
     py::class_<BilatDaemon>(mod, "BilatDaemon")
         .def(py::init<std::shared_ptr<GossipContext>, int, bool, double, int, double>(), py::arg("ctx"),
@@ -684,11 +712,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, mod)
         .def(py::init<torch::Tensor, c10::optional<torch::Tensor>, c10::optional<torch::Tensor>,
                       c10::optional<torch::Tensor>, c10::optional<torch::Tensor>, torch::Tensor,
                       c10::optional<torch::Tensor>, torch::Tensor, torch::Tensor, int, int,
-                      torch::Tensor, torch::Tensor, double>(),
+                      torch::Tensor, torch::Tensor, double, bool, int64_t>(),
              py::arg("z"), py::arg("g"), py::arg("m"), py::arg("shadow"), py::arg("residual"),
              py::arg("pad_ptrs"), py::arg("outbox_ptrs"), py::arg("table"), py::arg("wtable"),
              py::arg("rank"), py::arg("world"), py::arg("state"), py::arg("hyper"),
-             py::arg("timeout_s") = 30.0)
+             py::arg("timeout_s") = 30.0, py::arg("msg_bf16") = false, py::arg("outbox_bytes") = -1)
         .def("set_schedule", &GossipContext::set_schedule)
         .def("set_grad", &GossipContext::set_grad)
         .def("set_sgd_buffers", &GossipContext::set_sgd_buffers)

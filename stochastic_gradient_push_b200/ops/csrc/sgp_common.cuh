@@ -3,7 +3,8 @@
 // Data plane design (see DESIGN.md):
 //   * every rank owns, in NVSwitch peer-mapped ("symmetric") memory,
 //       - a signal pad  (SgpSignalPad): sequence flags + push-sum weight
-//       - an outbox     (2 x n floats, double buffered by step parity)
+//       - an outbox     (2 x n floats, double buffered by step parity; 2 x n bf16 with
+//                        SGP_F_MSG_BF16)
 //   * a gossip step is a PULL: the producer writes its outbox and releases a
 //     per-CTA sequence flag; consumers acquire the flag over NVLink and read
 //     the outbox with 16-byte P2P loads, applying the edge weight while they
@@ -104,6 +105,10 @@ struct SgpHyper {
 #define SGP_F_KEEP_Z     (1u << 10)  // phase 1 publishes a snapshot but leaves z untouched
 #define SGP_F_SELF_FROM_Z (1u << 11) // phase 2 mixes the CURRENT z (not the published snapshot)
 #define SGP_F_FROM_STATE (1u << 12)  // take the mode bits from SgpState::bilat_cmd (set by the decide kernel)
+// bf16 gossip messages (full synchronous step only): the outbox holds Q(x) = bf16(x), the sender
+// keeps c = x - (1 - self_w) * Q(x) in z, and phase 2 mixes c + sum_k in_w[k] * Q(x_k), so the
+// network's push-sum mass sum_i x_i is conserved exactly (up to fp32 rounding)
+#define SGP_F_MSG_BF16   (1u << 13)
 
 struct SgpArgs {
     // local buffers (length n, n % SGP_CHUNK == 0)
@@ -117,7 +122,7 @@ struct SgpArgs {
     float*               residual;   // overlap residual or null
     // symmetric memory: device arrays of per-rank base pointers
     SgpSignalPad* const* pads;       // [world]
-    float* const*        outboxes;   // [world], each 2*n floats
+    float* const*        outboxes;   // [world], each 2*n floats (2*n bf16 with SGP_F_MSG_BF16)
     // schedule
     const int*           table;      // [period][SGP_TABLE_ROW]
     const float*         wtable;     // [period][SGP_WTABLE_ROW]
@@ -200,6 +205,15 @@ __device__ __forceinline__ uint2 ld_once_u2(const uint2* p, uint64_t pol) {
 __device__ __forceinline__ void st_hint_f4(float4* p, float4 v, uint64_t pol) {
     asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1,%2,%3,%4}, %5;"
                  :: "l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(pol) : "memory");
+}
+__device__ __forceinline__ uint2 ld_stream_u2(const uint2* p) {
+    uint2 v;
+    asm volatile("ld.global.L1::no_allocate.v2.u32 {%0,%1}, [%2];" : "=r"(v.x), "=r"(v.y) : "l"(p));
+    return v;
+}
+__device__ __forceinline__ void st_hint_u2(uint2* p, uint2 v, uint64_t pol) {
+    asm volatile("st.global.L2::cache_hint.v2.u32 [%0], {%1,%2}, %3;"
+                 :: "l"(p), "r"(v.x), "r"(v.y), "l"(pol) : "memory");
 }
 __device__ __forceinline__ void st_f4(float4* p, float4 v) {
     asm volatile("st.global.v4.f32 [%0], {%1,%2,%3,%4};"

@@ -15,6 +15,8 @@
 //   sgp_scale_kernel   flat x *= w  /  x /= w  (ps_numerator / unbias API parity)
 #include "sgp_common.cuh"
 
+#include <type_traits>
+
 namespace {
 
 struct RowInfo {
@@ -72,11 +74,15 @@ __device__ __forceinline__ bool cta_done_is_last(SgpState* st) {
 }  // namespace
 
 // ---------------------------------------------------------------------------
-// Fused step kernel
+// Fused step kernel.  MSG_BF16 (SGP_F_MSG_BF16): bf16 messages, full synchronous step only
+// (PHASE1 | PUBLISH | PHASE2; the launcher rejects every other mode): phase 1 publishes Q(x) and
+// keeps c = x - (1 - self_w) Q(x) in z, phase 2 mixes c + sum_k in_w[k] Q(x_k).
 // ---------------------------------------------------------------------------
+template <bool MSG_BF16>
 __global__ void __launch_bounds__(SGP_THREADS, 2)
 sgp_step_kernel(const SgpArgs a)
 {
+    using Msg = typename std::conditional<MSG_BF16, __nv_bfloat16, float>::type;
     __shared__ float s_wn;        // new push-sum weight
     __shared__ int   s_ok;
 
@@ -104,7 +110,7 @@ sgp_step_kernel(const SgpArgs a)
     const float w1 = w0 + wres;                    // weight of the published numerator
 
     SgpSignalPad* mypad = a.pads[a.rank];
-    float* my_out = a.outboxes ? (a.outboxes[a.rank] + (size_t)parity * a.n) : nullptr;
+    Msg* my_out = a.outboxes ? (reinterpret_cast<Msg*>(a.outboxes[a.rank]) + (size_t)parity * a.n) : nullptr;
 
     const SgpHyper hp = *a.hyper;
     const uint64_t pol_first = l2_evict_first_policy();
@@ -149,11 +155,11 @@ sgp_step_kernel(const SgpArgs a)
     float w_next = ((flags & SGP_F_PUBLISH) && !(flags & SGP_F_KEEP_Z)) ? row.self_w * w1 : w1;
     float inv_wn = 1.f;
     bool pull_ok = true;
-    const float* peer_out[SGP_MAX_PEERS];
+    const Msg* peer_out[SGP_MAX_PEERS];
 #pragma unroll
     for (int k = 0; k < SGP_MAX_PEERS; ++k)
         peer_out[k] = ((flags & SGP_F_PHASE2) && k < row.n_in && row.in[k] >= 0)
-                          ? a.outboxes[row.in[k]] + (size_t)parity * a.n : nullptr;
+                          ? reinterpret_cast<const Msg*>(a.outboxes[row.in[k]]) + (size_t)parity * a.n : nullptr;
 
     for (int seg = 0; seg < K; ++seg) {
         const long long it_lo = my_chunks * seg / K;
@@ -212,8 +218,15 @@ sgp_step_kernel(const SgpArgs a)
                         xv.x = fmaf(r[u].x, rscale, xv.x); xv.y = fmaf(r[u].y, rscale, xv.y);
                         xv.z = fmaf(r[u].z, rscale, xv.z); xv.w = fmaf(r[u].w, rscale, xv.w);
                     }
-                    if (flags & SGP_F_PUBLISH)   // keep the outbox in L2 for phase 2 / peers
+                    if constexpr (MSG_BF16) {
+                        // publish Q(x); z keeps what was not sent: c = x - (1 - self_w) Q(x)
+                        const uint2 q = f4_to_bf16x4(xv);
+                        st_hint_u2(reinterpret_cast<uint2*>(my_out + i), q, pol_last);
+                        st_hint_f4(reinterpret_cast<float4*>(a.z + i),
+                                   fma4(bf16x4_to_f4(q), row.self_w - 1.f, xv), pol_last);
+                    } else if (flags & SGP_F_PUBLISH) {   // keep the outbox in L2 for phase 2 / peers
                         st_hint_f4(reinterpret_cast<float4*>(my_out + i), xv, pol_last);
+                    }
                     if (write_z) {
                         const float4 zv = mul4(xv, inv_w1);
                         st_f4(reinterpret_cast<float4*>(a.z + i), zv);
@@ -263,21 +276,29 @@ sgp_step_kernel(const SgpArgs a)
 #pragma unroll
                     for (int u = 0; u < SGP_UNROLL; ++u) {
                         const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
-                        // own term: the snapshot this CTA just published (L2-resident),
-                        // or (AD-PSGD) the live parameters, which may already carry
-                        // newer local SGD updates
-                        const float* own = (flags & SGP_F_SELF_FROM_Z) ? a.z : my_out;
-                        acc[u] = mul4(ld_once_f4(reinterpret_cast<const float4*>(own + i), pol_first),
-                                      (flags & SGP_F_SELF_FROM_Z) ? row.self_w * w0 : row.self_w);
+                        if constexpr (MSG_BF16) {
+                            // own term: c, kept in z by phase 1 (already carries the self weight)
+                            acc[u] = ld_once_f4(reinterpret_cast<const float4*>(a.z + i), pol_first);
+                        } else {
+                            // own term: the snapshot this CTA just published (L2-resident),
+                            // or (AD-PSGD) the live parameters, which may already carry
+                            // newer local SGD updates
+                            const float* own = (flags & SGP_F_SELF_FROM_Z) ? a.z : my_out;
+                            acc[u] = mul4(ld_once_f4(reinterpret_cast<const float4*>(own + i), pol_first),
+                                          (flags & SGP_F_SELF_FROM_Z) ? row.self_w * w0 : row.self_w);
+                        }
                     }
                     // peer loads: all UNROLL requests of one peer in flight together
                     for (int k = 0; k < row.n_in; ++k) {
-                        const float* po = peer_out[k];
+                        const Msg* po = peer_out[k];
                         if (po == nullptr) continue;
 #pragma unroll
                         for (int u = 0; u < SGP_UNROLL; ++u) {
                             const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
-                            pv[u] = ld_stream_f4(reinterpret_cast<const float4*>(po + i));
+                            if constexpr (MSG_BF16)
+                                pv[u] = bf16x4_to_f4(ld_stream_u2(reinterpret_cast<const uint2*>(po + i)));
+                            else
+                                pv[u] = ld_stream_f4(reinterpret_cast<const float4*>(po + i));
                         }
                         const float wk = row.in_w[k];
 #pragma unroll
@@ -296,15 +317,19 @@ sgp_step_kernel(const SgpArgs a)
             else if (!(flags & SGP_F_SELF_FROM_Z) && (flags & SGP_F_PHASE1)) {
                 // an in-neighbour timed out: "every in-message of this round was lost" -- de-bias the
                 // numerator this CTA published (a valid push-sum state) instead of leaving the
-                // pre-SGD parameters behind; the sticky status word makes the host raise
-                const float inv_own = 1.f / w1;
+                // pre-SGD parameters behind; the sticky status word makes the host raise.  With bf16
+                // messages the numerator this rank still holds is c (it sent the rest), carrying the
+                // weight self_w * w1 -- see sgp_step_pipe_kernel
+                const float inv_own = MSG_BF16 ? 1.f / (row.self_w * w1) : 1.f / w1;
+                const float* own;
+                if constexpr (MSG_BF16) own = a.z; else own = my_out;
                 for (long long it = it_lo; it < it_hi; ++it) {
                     const long long c = b + it * gridDim.x;
                     const long long base = c * SGP_CHUNK + (long long)tid * SGP_VEC;
 #pragma unroll
                     for (int u = 0; u < SGP_UNROLL; ++u) {
                         const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
-                        const float4 zv = mul4(ld_once_f4(reinterpret_cast<const float4*>(my_out + i), pol_first),
+                        const float4 zv = mul4(ld_once_f4(reinterpret_cast<const float4*>(own + i), pol_first),
                                                inv_own);
                         st_f4(reinterpret_cast<float4*>(a.z + i), zv);
                         if (flags & SGP_F_SHADOW)
@@ -584,6 +609,14 @@ sgp_gather_tma_kernel(const SgpArgs a, const int pub_grid)
 // failed, completes its barriers without data, and the consumers de-bias their own published
 // numerator instead (z = x_own / w1, i.e. "every in-message of this round was lost" -- a valid
 // push-sum state); the sticky status word makes the host raise at its next poll.
+//
+// MSG_BF16 (SGP_F_MSG_BF16): the outbox holds Q(x) = bf16(x) and each ring stage one 8 KB bf16
+// chunk.  Phase 1 keeps c = x - (1 - self_w) Q(x) in z (overwritten by phase 2 anyway) and phase 2
+// computes c + sum_k in_w[k] Q(x_k): the sender loses exactly what its out-neighbours receive, so
+// sum_i x_i is conserved for any column-stochastic schedule.  On a timed-out in-neighbour the
+// consumers de-bias c over self_w * w1 (the weight the rank keeps when every in-message is lost):
+// c is what this rank still holds after sending, so the fallback stays a valid push-sum state.
+// That needs self_w > 0, which every mixing of this project has (1 / (peers + 1) for uniform).
 // ---------------------------------------------------------------------------
 #define PIPE_STAGES    4
 #define PIPE_CONSUMERS SGP_THREADS                 // 256: the chunk decomposition of sgp_step_kernel
@@ -597,11 +630,14 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 // 9 warps x 2 CTAs per SM: the register file is split over 4 sub-partitions (16 K registers
 // each), so 18 warps only fit at <= 102 registers per thread -- __launch_bounds__(288, 2) makes
 // ptxas pick 96.  (At 112 registers the kernel runs one CTA per SM.)
+template <bool MSG_BF16>
 __global__ void __launch_bounds__(PIPE_THREADS, 2)
 sgp_step_pipe_kernel(const SgpArgs a)
 {
+    using Msg = typename std::conditional<MSG_BF16, __nv_bfloat16, float>::type;
+    constexpr uint32_t MSG_BYTES = SGP_CHUNK * sizeof(Msg);                    // one chunk per stage
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    float* ring = reinterpret_cast<float*>(smem_raw);                          // [STAGES][CHUNK]
+    unsigned char* ring = smem_raw;                                            // [STAGES][MSG_BYTES]
     uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + PIPE_STAGES * SGP_TMA_BYTES);
     uint64_t* empty = full + PIPE_STAGES;
     uint64_t* wbar = empty + PIPE_STAGES;            // new push-sum weight is known
@@ -626,7 +662,7 @@ sgp_step_pipe_kernel(const SgpArgs a)
     const float w1 = w0;                              // (no residual fold in the synchronous step)
 
     SgpSignalPad* mypad = a.pads[a.rank];
-    float* my_out = a.outboxes[a.rank] + (size_t)parity * a.n;
+    Msg* my_out = reinterpret_cast<Msg*>(a.outboxes[a.rank]) + (size_t)parity * a.n;
 
     const long long my_chunks = (nchunks > b) ? (nchunks - 1 - b) / gridDim.x + 1 : 0;
     int K = a.segments < 1 ? 1 : a.segments;
@@ -676,9 +712,10 @@ sgp_step_pipe_kernel(const SgpArgs a)
                     for (int k = 0; k < n_in; ++k) {
                         mbar_wait(&empty[stage], phase ^ 1u);
                         if (ok) {
-                            const float* src = a.outboxes[in_rank[k]] + (size_t)parity * a.n + c * SGP_CHUNK;
-                            mbar_expect_tx(&full[stage], SGP_TMA_BYTES);
-                            tma_load_1d(ring + (size_t)stage * SGP_CHUNK, src, SGP_TMA_BYTES, &full[stage]);
+                            const Msg* src = reinterpret_cast<const Msg*>(a.outboxes[in_rank[k]]) +
+                                             (size_t)parity * a.n + c * SGP_CHUNK;
+                            mbar_expect_tx(&full[stage], MSG_BYTES);
+                            tma_load_1d(ring + (size_t)stage * MSG_BYTES, src, MSG_BYTES, &full[stage]);
                         } else {
                             mbar_arrive(&full[stage]);           // nothing will land: release the consumers
                         }
@@ -766,7 +803,15 @@ sgp_step_pipe_kernel(const SgpArgs a)
                                     st_f4(reinterpret_cast<float4*>(a.g2 + i), make_float4(0.f, 0.f, 0.f, 0.f));
                             }
                         }
-                        st_hint_f4(reinterpret_cast<float4*>(my_out + i), xv, pol_last);
+                        if constexpr (MSG_BF16) {
+                            // publish Q(x); z keeps what was not sent: c = x - (1 - self_w) Q(x)
+                            const uint2 q = f4_to_bf16x4(xv);
+                            st_hint_u2(reinterpret_cast<uint2*>(my_out + i), q, pol_last);
+                            st_hint_f4(reinterpret_cast<float4*>(a.z + i),
+                                       fma4(bf16x4_to_f4(q), row.self_w - 1.f, xv), pol_last);
+                        } else {
+                            st_hint_f4(reinterpret_cast<float4*>(my_out + i), xv, pol_last);
+                        }
                     }
                 }
                 asm volatile("bar.sync 1, %0;" :: "n"(PIPE_CONSUMERS) : "memory");
@@ -791,15 +836,25 @@ sgp_step_pipe_kernel(const SgpArgs a)
 #pragma unroll
                     for (int u = 0; u < SGP_UNROLL; ++u) {
                         const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
-                        acc[u] = mul4(ld_once_f4(reinterpret_cast<const float4*>(my_out + i), pol_first),   // L2 hit
-                                      row.self_w);
+                        if constexpr (MSG_BF16)      // c already carries the self weight
+                            acc[u] = ld_once_f4(reinterpret_cast<const float4*>(a.z + i), pol_first);   // L2 hit
+                        else
+                            acc[u] = mul4(ld_once_f4(reinterpret_cast<const float4*>(my_out + i), pol_first),   // L2 hit
+                                          row.self_w);
                     }
                     for (int k = 0; k < n_in; ++k) {
                         mbar_wait(&full[cstage], cphase);
-                        const float4* src = reinterpret_cast<const float4*>(ring + (size_t)cstage * SGP_CHUNK);
+                        const unsigned char* stage_p = ring + (size_t)cstage * MSG_BYTES;
                         const float wk = in_w[k];
 #pragma unroll
-                        for (int u = 0; u < SGP_UNROLL; ++u) acc[u] = fma4(src[tid + u * SGP_THREADS], wk, acc[u]);
+                        for (int u = 0; u < SGP_UNROLL; ++u) {
+                            float4 v;
+                            if constexpr (MSG_BF16)
+                                v = bf16x4_to_f4(reinterpret_cast<const uint2*>(stage_p)[tid + u * SGP_THREADS]);
+                            else
+                                v = reinterpret_cast<const float4*>(stage_p)[tid + u * SGP_THREADS];
+                            acc[u] = fma4(v, wk, acc[u]);
+                        }
                         __syncwarp();
                         if (lane == 0) mbar_arrive(&empty[cstage]);     // this warp is done with the stage
                         if (++cstage == PIPE_STAGES) { cstage = 0; cphase ^= 1u; }
@@ -808,9 +863,15 @@ sgp_step_pipe_kernel(const SgpArgs a)
 #pragma unroll
                     for (int u = 0; u < SGP_UNROLL; ++u) {
                         const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
-                        const float4 zv = failed
-                            ? mul4(ld_once_f4(reinterpret_cast<const float4*>(my_out + i), pol_first), inv_w1)
-                            : mul4(acc[u], inv_wn);
+                        float4 zv;
+                        if constexpr (MSG_BF16)    // own numerator c (still in z) over the weight kept
+                            zv = failed ? mul4(ld_once_f4(reinterpret_cast<const float4*>(a.z + i), pol_first),
+                                               inv_w1 / row.self_w)
+                                        : mul4(acc[u], inv_wn);
+                        else
+                            zv = failed
+                                ? mul4(ld_once_f4(reinterpret_cast<const float4*>(my_out + i), pol_first), inv_w1)
+                                : mul4(acc[u], inv_wn);
                         st_f4(reinterpret_cast<float4*>(a.z + i), zv);
                         if (flags & SGP_F_SHADOW)
                             st_u2(reinterpret_cast<uint2*>(a.shadow + i), f4_to_bf16x4(zv));
@@ -1195,31 +1256,58 @@ sgp_peer_reduce_kernel(float* __restrict__ dst, const SgpPtrList srcs, long long
 // ---------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------
+// bf16 messages are implemented for the full synchronous step only
+static bool msg_bf16_mode_ok(unsigned int flags)
+{
+    if (!(flags & SGP_F_MSG_BF16)) return true;
+    const unsigned int full = SGP_F_PHASE1 | SGP_F_PUBLISH | SGP_F_PHASE2;
+    const unsigned int partial = SGP_F_FOLD_RES | SGP_F_NO_ROTATE | SGP_F_KEEP_Z | SGP_F_SELF_FROM_Z |
+                                 SGP_F_FROM_STATE;
+    return (flags & full) == full && (flags & partial) == 0u;
+}
+
+template <bool MSG_BF16>
+static cudaError_t configure_step_pipe()
+{
+    cudaError_t e = cudaFuncSetAttribute(sgp_step_pipe_kernel<MSG_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         PIPE_SMEM);
+    if (e != cudaSuccess) return e;
+    // two CTAs x 64 KB per SM: ask for the large shared-memory carve-out (the default one fits
+    // a single CTA: launch__occupancy_limit_shared_mem = 1 in the first ncu capture)
+    return cudaFuncSetAttribute(sgp_step_pipe_kernel<MSG_BF16>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                cudaSharedmemCarveoutMaxShared);
+}
+
 extern "C" {
 
 cudaError_t sgp_launch_step(const SgpArgs* args, int grid, cudaStream_t stream)
 {
-    sgp_step_kernel<<<grid, SGP_THREADS, 0, stream>>>(*args);
+    if (!msg_bf16_mode_ok(args->flags)) return cudaErrorInvalidValue;
+    if (args->flags & SGP_F_MSG_BF16)
+        sgp_step_kernel<true><<<grid, SGP_THREADS, 0, stream>>>(*args);
+    else
+        sgp_step_kernel<false><<<grid, SGP_THREADS, 0, stream>>>(*args);
     return cudaGetLastError();
 }
 
 cudaError_t sgp_launch_step_pipe(const SgpArgs* args, int grid, cudaStream_t stream)
 {
+    if (!msg_bf16_mode_ok(args->flags)) return cudaErrorInvalidValue;
     static bool configured[64] = {};
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64 || !configured[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(sgp_step_pipe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             PIPE_SMEM);
-        if (e != cudaSuccess) return e;
-        // two CTAs x 64 KB per SM: ask for the large shared-memory carve-out (the default one fits
-        // a single CTA: launch__occupancy_limit_shared_mem = 1 in the first ncu capture)
-        e = cudaFuncSetAttribute(sgp_step_pipe_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                 cudaSharedmemCarveoutMaxShared);
+        cudaError_t e = configure_step_pipe<false>();
+        if (e == cudaSuccess) e = configure_step_pipe<true>();
         if (e != cudaSuccess) return e;
         if (dev >= 0 && dev < 64) configured[dev] = true;
     }
-    sgp_step_pipe_kernel<<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
+    // (the bf16 ring uses half of each stage: the occupancy, and so the grid every rank shares,
+    // stays that of the fp32 kernel)
+    if (args->flags & SGP_F_MSG_BF16)
+        sgp_step_pipe_kernel<true><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
+    else
+        sgp_step_pipe_kernel<false><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
     return cudaGetLastError();
 }
 
@@ -1228,22 +1316,27 @@ int sgp_max_resident_ctas_pipe(int device)
 {
     int sms = 0, per_sm = 0;
     if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) return 0;
-    cudaFuncSetAttribute(sgp_step_pipe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PIPE_SMEM);
-    cudaFuncSetAttribute(sgp_step_pipe_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
-                         cudaSharedmemCarveoutMaxShared);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sgp_step_pipe_kernel, PIPE_THREADS, PIPE_SMEM)
+    configure_step_pipe<false>();
+    configure_step_pipe<true>();
+    int per_sm_bf16 = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sgp_step_pipe_kernel<false>, PIPE_THREADS, PIPE_SMEM)
         != cudaSuccess) return 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_bf16, sgp_step_pipe_kernel<true>, PIPE_THREADS,
+                                                      PIPE_SMEM) != cudaSuccess) return 0;
+    if (per_sm_bf16 < per_sm) per_sm = per_sm_bf16;
     return sms * per_sm;
 }
 
 cudaError_t sgp_launch_gather(const SgpArgs* args, int grid, int pub_grid, cudaStream_t stream)
 {
+    if (args->flags & SGP_F_MSG_BF16) return cudaErrorInvalidValue;
     sgp_gather_kernel<<<grid, SGP_THREADS, 0, stream>>>(*args, pub_grid);
     return cudaGetLastError();
 }
 
 cudaError_t sgp_launch_gather_tma(const SgpArgs* args, int grid, int pub_grid, cudaStream_t stream)
 {
+    if (args->flags & SGP_F_MSG_BF16) return cudaErrorInvalidValue;
     const int smem = SGP_TMA_STAGES * SGP_TMA_BYTES + SGP_TMA_STAGES * 8 + 64;
     static bool configured = false;
     if (!configured) {
@@ -1345,8 +1438,9 @@ cudaError_t sgp_launch_scale(float* x, long long n, const float* scalar, int inv
 cudaError_t sgp_preload_kernels()
 {
     const void* kernels[] = {
-        (const void*)sgp_step_kernel, (const void*)sgp_gather_kernel, (const void*)sgp_gather_tma_kernel,
-        (const void*)sgp_step_pipe_kernel, (const void*)sgp_probe_kernel, (const void*)sgp_gather_wait_kernel,
+        (const void*)sgp_step_kernel<false>, (const void*)sgp_step_kernel<true>, (const void*)sgp_gather_kernel,
+        (const void*)sgp_gather_tma_kernel, (const void*)sgp_step_pipe_kernel<false>,
+        (const void*)sgp_step_pipe_kernel<true>, (const void*)sgp_probe_kernel, (const void*)sgp_gather_wait_kernel,
         (const void*)sgp_gather_ack_kernel, (const void*)sgp_bilat_decide_kernel, (const void*)sgp_bilat_ctl_kernel,
         (const void*)sgp_allreduce_sgd_kernel, (const void*)sgp_zero_kernel, (const void*)sgp_barrier_kernel,
         (const void*)sgp_scale_kernel, (const void*)sgp_peer_reduce_kernel};
@@ -1362,7 +1456,7 @@ int sgp_max_resident_ctas(int device)
 {
     int sms = 0, per_sm = 0;
     if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) return 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sgp_step_kernel, SGP_THREADS, 0)
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sgp_step_kernel<false>, SGP_THREADS, 0)
         != cudaSuccess) return 0;
     return sms * per_sm;
 }

@@ -11,6 +11,11 @@ and exposes the four launches the algorithms are built from:
     gather()            Overlap-SGP, side stream: residual = sum of P2P loads
     local(sgd, fold)    no communication: [SGD] / fold only (flush, world==1)
 
+``msg_dtype=torch.bfloat16`` sends bf16 messages (half the bytes per in-neighbour) with exact
+push-sum mass conservation: the outbox holds Q(x) = bf16(x), the sender keeps
+x - (1 - self_w) Q(x), and the receivers add in_w * Q(x_j).  Only :meth:`mix` (SGP / D-PSGD)
+supports it.
+
 All launches go to the *current* CUDA stream and are CUDA-graph capturable:
 nothing that changes per step (phase, parity, lr, push-sum weight) is a kernel
 argument -- it all lives in device memory.
@@ -67,8 +72,12 @@ class GossipEngine(object):
                  grid: Optional[int] = None, gather_grid: Optional[int] = None,
                  timeout_s: float = 30.0, name: str = 'sgp', segments: int = 4,
                  gather_tma: bool = True, soft_timeout_s: Optional[float] = None,
-                 gather_dma: Optional[bool] = None):
+                 gather_dma: Optional[bool] = None, msg_dtype: Optional[torch.dtype] = None):
         C = native.load()
+        if msg_dtype not in (None, torch.float32, torch.bfloat16):
+            raise ValueError('gossip message dtype must be torch.float32 or torch.bfloat16, got %s'
+                             % (msg_dtype,))
+        self.msg_bf16 = msg_dtype == torch.bfloat16
         self.C = C
         self.world = world
         self.rank = world.rank
@@ -89,7 +98,8 @@ class GossipEngine(object):
 
         # symmetric allocations (collective across the world)
         self.pad = world.alloc(name + '.pad', C.PAD_BYTES)
-        self.outbox = world.alloc(name + '.outbox', 2 * self.n * 4)
+        elem = 2 if self.msg_bf16 else 4
+        self.outbox = world.alloc(name + '.outbox', 2 * self.n * elem)
 
         # local kernel state / hyper-parameters
         self.state = torch.zeros(C.STATE_BYTES, dtype=torch.uint8, device=self.device)
@@ -118,7 +128,8 @@ class GossipEngine(object):
             z=self.z, g=grad, m=momentum, shadow=shadow, residual=self.residual,
             pad_ptrs=self.pad.table, outbox_ptrs=self.outbox.table,
             table=table, wtable=wtable, rank=self.rank, world=self.nranks,
-            state=self.state, hyper=self.hyper, timeout_s=float(timeout_s))
+            state=self.state, hyper=self.hyper, timeout_s=float(timeout_s),
+            msg_bf16=self.msg_bf16, outbox_bytes=int(self.outbox.nbytes))
         self.period = table.shape[0]
         # phase-1 / phase-2 interleave granularity; must be identical on all ranks
         self.ctx.set_segments(int(segments))
@@ -202,6 +213,10 @@ class GossipEngine(object):
             f |= C.F_SHADOW
         return f
 
+    def _check_fp32_messages(self, what):
+        if self.msg_bf16:
+            raise RuntimeError('GossipEngine.%s is not implemented for bf16 messages (only mix() is)' % what)
+
     def mix(self, sgd=False, zero_grad=True, in_numerator=False):
         C = self.C
         f = self._common(sgd, zero_grad, in_numerator) | C.F_PHASE1 | C.F_PUBLISH | C.F_PHASE2
@@ -210,6 +225,7 @@ class GossipEngine(object):
 
     def publish(self, sgd=False, fold=False, zero_grad=True, in_numerator=False):
         C = self.C
+        self._check_fp32_messages('publish')
         f = self._common(sgd, zero_grad, in_numerator) | C.F_PHASE1 | C.F_PUBLISH
         if fold:
             f |= C.F_FOLD_RES
@@ -242,6 +258,7 @@ class GossipEngine(object):
         per step (the default schedules) this is a COPY-ENGINE transfer of the peer's outbox bracketed
         by a 1-CTA flag wait and a 1-thread ack kernel -- no SM is taken away from the forward pass;
         otherwise a gather kernel (TMA bulk copies by default, register-staged with ``tma=False``)."""
+        self._check_fp32_messages('gather')
         use_dma = self.gather_dma if dma is None else (bool(dma) and self.gather_dma)
         if use_dma:
             s = self.steps - 1                       # publish() of this step already advanced the mirror
@@ -262,12 +279,14 @@ class GossipEngine(object):
     def publish_only(self):
         """Snapshot z into the outbox and release the flags; nothing else."""
         C = self.C
+        self._check_fp32_messages('publish_only')
         self.ctx.step(C.F_PHASE1 | C.F_PUBLISH | C.F_NO_ROTATE | C.F_KEEP_Z, self.grid)
 
     def pull_only(self):
         """z <- self_w * z_now + sum_k in_w[k] * outbox_k ; ack ; advance the round.
         Call after :meth:`probe` reported the partner's snapshot is visible."""
         C = self.C
+        self._check_fp32_messages('pull_only')
         f = C.F_PHASE2 | C.F_PUBLISH | C.F_SELF_FROM_Z
         if self.shadow is not None:
             f |= C.F_SHADOW
@@ -275,6 +294,7 @@ class GossipEngine(object):
         self.steps += 1
 
     def probe(self, host_flag=None):
+        self._check_fp32_messages('probe')
         self.ctx.probe(self.grid, host_flag)
 
     def barrier(self):

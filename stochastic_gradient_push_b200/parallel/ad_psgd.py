@@ -63,8 +63,11 @@ class BilatGossipDataParallel(Module):
                  network_interface_type=None, tcp_interface_name=None,
                  transport='auto', poll_interval=2e-4, gossip_grid=32,
                  heartbeat_timeout=300.0, max_rounds_per_update=4, daemon_depth=2,
-                 partner_wait_us=50.0, symmetric_world=None):
+                 partner_wait_us=50.0, symmetric_world=None, gossip_dtype=None):
         super(BilatGossipDataParallel, self).__init__()
+        from .distributed import check_gossip_dtype
+        # (bf16 bilateral messages would need their own mass-correction term)
+        check_gossip_dtype(gossip_dtype, 'BilatGossipDataParallel (AD-PSGD)')
         first = next(module.parameters())
         on_cuda = first.is_cuda
         if device_ids is None:

@@ -39,8 +39,10 @@ from .trainer import GossipTrainer
 class AllReduceDataParallel(Module):
 
     def __init__(self, module, rank=None, world_size=None, transport='auto',
-                 grad_dtype=torch.float32, timeout_s=60.0, grid=None):
+                 grad_dtype=torch.float32, timeout_s=60.0, grid=None, gossip_dtype=None):
         super().__init__()
+        from .distributed import check_gossip_dtype
+        check_gossip_dtype(gossip_dtype, 'AllReduceDataParallel')
         self.module = module
         if rank is None or world_size is None:
             if dist.is_initialized():

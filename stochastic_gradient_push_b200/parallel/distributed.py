@@ -45,7 +45,7 @@ import torch.distributed as dist
 from torch.autograd import Variable
 from torch.nn.modules import Module
 
-from ..gossiper import C10dTransport
+from ..gossiper import C10dTransport, bf16_message_numel, bf16_message_weight, pack_bf16_message
 from ..mixing_manager import UniformMixing
 from ..topology.graph_manager import NPeerDynamicDirectedExponentialGraph as NPDDEGraph
 from ..utils import tracing
@@ -64,7 +64,7 @@ class _KernelBackend(object):
     name = 'nvlink'
 
     def __init__(self, owner, arena: FlatArena, graph, mixing, world_view, overlap,
-                 compute_dtype, timeout_s, grid):
+                 compute_dtype, timeout_s, grid, msg_dtype=None):
         from ..ops.peer_mix import GossipEngine
         self.owner = owner
         self.arena = arena
@@ -74,8 +74,8 @@ class _KernelBackend(object):
             self.shadow = arena.new_buffer(dtype=torch.bfloat16)
             self.shadow.copy_(arena.flat)
         self.engine = GossipEngine(world_view, arena.flat, graph, mixing, shadow=self.shadow,
-                                   with_residual=True, timeout_s=timeout_s, grid=grid,
-                                   name=owner._symm_name)
+                                   with_residual=msg_dtype is None, timeout_s=timeout_s, grid=grid,
+                                   name=owner._symm_name, msg_dtype=msg_dtype)
         self.gather_event = None
         self.residual_pending = False       # a gather finished/launched and is not folded yet
         self.sgd_pending = False            # FusedGossipSGD.step() deferred into next launch
@@ -87,13 +87,19 @@ class _KernelBackend(object):
 
 class _C10dBackend(object):
     """Portable data plane: isend/irecv of edge-weighted snapshots (+ the
-    push-sum weight as one extra element), residual folded at the next query."""
+    push-sum weight as one extra element), residual folded at the next query.
+
+    ``msg_bf16``: every message is Q(a_j * x) in bf16 with the fp32 weight in its tail (see
+    ``gossiper.pack_bf16_message``); the sender subtracts what it sends instead of scaling by
+    the self weight, so the local result is x - sum_out m_j + sum_in m_j, accumulated in fp32."""
 
     name = 'c10d'
 
     def __init__(self, owner, arenas: Dict[torch.dtype, FlatArena], graph, mixing,
-                 comm_device, group=None):
+                 comm_device, group=None, msg_bf16=False):
         self.owner = owner
+        self.msg_bf16 = msg_bf16
+        self._sent = []             # bf16: (arena, Q(a_j x)) subtracted by the last start()
         self.arenas = arenas
         self.graph = graph
         self.mixing = mixing
@@ -116,15 +122,23 @@ class _C10dBackend(object):
         Returns the self-loop weight the caller applies locally.  ``mix=False`` (retry of an
         interrupted round): the local numerator already carries the self-loop scaling of the
         failed attempt, so the messages are rebuilt from ``x / self_w`` (== the pre-mix
-        numerator) and the caller must NOT scale again."""
+        numerator) and the caller must NOT scale again.  With bf16 messages the numerator is
+        never scaled by the caller: start() subtracts the messages itself (and a retry first
+        adds back those of the failed attempt); only the weight follows the rule above."""
         out_edges, in_edges = self.graph.get_edges()
         self_w, edge_w = self.mixing.scalar_weights([e.dest for e in out_edges])
         undo = 1.0 if mix else 1.0 / float(self_w)
+        if self.msg_bf16:
+            if not mix:
+                for arena, q in self._sent:
+                    arena.flat.add_(q.to(arena.flat.dtype))
+            self._sent = []
         reqs, recvs, keep, poll = [], [], [], []
         for dtype, arena in self.arenas.items():
-            n = arena.total + 1
+            n = bf16_message_numel(arena.total) if self.msg_bf16 else arena.total + 1
+            msg_dtype = torch.bfloat16 if self.msg_bf16 else dtype
             remote_in = [e for e in in_edges if e.src != e.dest]
-            bufs = [self._buf(self.recv_bufs, (dtype, i), n, dtype) for i in range(len(remote_in))]
+            bufs = [self._buf(self.recv_bufs, (dtype, i), n, msg_dtype) for i in range(len(remote_in))]
             batched = getattr(self.transport, 'batched', False)   # NCCL: receives + sends as ONE grouped launch
             if batched:
                 rr = []
@@ -137,12 +151,19 @@ class _C10dBackend(object):
             local_add = []
             send_edges, send_msgs = [], []
             for i, e in enumerate(out_edges):
-                msg = self._buf(self.send_bufs, (dtype, i), n, dtype)
-                msg[:-1].copy_(arena.flat, non_blocking=True)
-                if self.comm_device.type == 'cpu' and arena.flat.is_cuda:
-                    torch.cuda.current_stream().synchronize()
-                msg[-1] = ps_weight
-                msg.mul_(edge_w[e.dest] * undo)
+                msg = self._buf(self.send_bufs, (dtype, i), n, msg_dtype)
+                if self.msg_bf16:
+                    a = float(edge_w[e.dest])
+                    q = pack_bf16_message(msg, arena.flat, a, float(ps_weight) * a * undo)
+                    self._sent.append((arena, q))
+                    if self.comm_device.type == 'cpu' and arena.flat.is_cuda:
+                        torch.cuda.current_stream().synchronize()
+                else:
+                    msg[:-1].copy_(arena.flat, non_blocking=True)
+                    if self.comm_device.type == 'cpu' and arena.flat.is_cuda:
+                        torch.cuda.current_stream().synchronize()
+                    msg[-1] = ps_weight
+                    msg.mul_(edge_w[e.dest] * undo)
                 if e.dest == e.src:
                     local_add.append(msg)
                 else:
@@ -158,6 +179,8 @@ class _C10dBackend(object):
                 reqs += self.transport.post_sends(send_msgs, send_edges)
             recvs.append((arena, bufs + local_add))
             keep.append(send_msgs)
+        for arena, q in self._sent:             # the sender keeps what it did not send
+            arena.flat.sub_(q.to(arena.flat.dtype))
         self.pending = (reqs, recvs, keep, poll)
         if self.graph.is_dynamic_graph():
             self.graph.get_peers(rotate=True)
@@ -191,9 +214,14 @@ class _C10dBackend(object):
         for arena, bufs in recvs:
             for b in bufs:
                 staged = staged or (b.device != arena.flat.device)
-                arena.flat.add_(b[:-1].to(arena.flat.device, non_blocking=True))
-                if first:
-                    w_res += float(b[-1])
+                if self.msg_bf16:
+                    arena.flat.add_(b[:arena.total].to(arena.flat.device, non_blocking=True).to(arena.flat.dtype))
+                    if first:
+                        w_res += bf16_message_weight(b, arena.total)
+                else:
+                    arena.flat.add_(b[:-1].to(arena.flat.device, non_blocking=True))
+                    if first:
+                        w_res += float(b[-1])
             first = False
         if staged and torch.cuda.is_available():
             # pinned CPU receive buffers -> GPU arena: the async H2D copies read the buffers when
@@ -204,6 +232,7 @@ class _C10dBackend(object):
                 if arena.flat.is_cuda:
                     torch.cuda.current_stream(arena.flat.device).synchronize()
         self.pending = None
+        self._sent = []
         return w_res
 
 
@@ -248,8 +277,14 @@ class GossipDataParallel(Module):
                  overlap=False, synch_freq=0, verbose=False, use_streams=True,
                  nprocs_per_node=1, local_node_group=None,
                  transport='auto', compute_dtype=None, symmetric_world=None,
-                 heartbeat_timeout=HEARTBEAT_TIMEOUT, grid=None, symmetric_name=None):
+                 heartbeat_timeout=HEARTBEAT_TIMEOUT, grid=None, symmetric_name=None,
+                 gossip_dtype=None):
         super(GossipDataParallel, self).__init__()
+        # bf16 gossip messages: half the bytes per in-neighbour, push-sum mass conserved exactly
+        # (the sender keeps what it did not send); parameters and push-sum weights stay fp32
+        self.gossip_dtype = check_gossip_dtype(
+            gossip_dtype, 'overlap=True (OSGP)' if overlap else
+            'nprocs_per_node > 1' if nprocs_per_node > 1 else None)
         _INSTANCES[0] += 1
         self._instance_id = _INSTANCES[0]
         self._timeout_s = float(heartbeat_timeout)
@@ -412,9 +447,10 @@ class GossipDataParallel(Module):
                     symmetric_world = self._make_symmetric_world(world_size, first_param.device)
                 self._kernel = _KernelBackend(
                     self, self._arenas[torch.float32], graph, mixing, symmetric_world,
-                    overlap, compute_dtype, self._timeout_s, grid)
+                    overlap, compute_dtype, self._timeout_s, grid, msg_dtype=self.gossip_dtype)
             else:
-                self._c10d = _C10dBackend(self, self._arenas, graph, mixing, comm_device)
+                self._c10d = _C10dBackend(self, self._arenas, graph, mixing, comm_device,
+                                          msg_bf16=self.gossip_dtype is not None)
         self.transport = 'nvlink' if self._kernel is not None else 'c10d'
         self._twin = []          # [bf16 compute twin] (a list so it is not a registered submodule)
         if self._kernel is not None and self._kernel.shadow is not None:
@@ -517,9 +553,13 @@ class GossipDataParallel(Module):
             self._query_gossip_queue()
             self._flush_pending(drain=True)
         super_dict = super(GossipDataParallel, self).state_dict(*args, **kwargs)
-        return {'state_dict': super_dict,
-                'ps_weight': self.ps_weight.detach().cpu().clone(),
-                'is_ps_numerator': self.is_ps_numerator}
+        out = {'state_dict': super_dict,
+               'ps_weight': self.ps_weight.detach().cpu().clone(),
+               'is_ps_numerator': self.is_ps_numerator}
+        if self.gossip_dtype is not None:
+            # informational: parameters are fp32 either way, so a checkpoint loads across dtypes
+            out['gossip_dtype'] = 'bfloat16'
+        return out
 
     def load_state_dict(self, load_dict, *args, **kwargs):
         state_dict = load_dict['state_dict']
@@ -849,8 +889,9 @@ class GossipDataParallel(Module):
             with tracing.span('gossip.post'):
                 self_w = c.start(self._w, pollable=self.asynch, mix=mix)
             if mix:
-                for arena in self._arenas.values():     # keep the self-loop share
-                    arena.flat.mul_(self_w)
+                if not c.msg_bf16:                      # (bf16: start() subtracted the messages)
+                    for arena in self._arenas.values():     # keep the self-loop share
+                        arena.flat.mul_(self_w)
                 self._w *= self_w
         self.params_mixed = False
         self.gossiping = True
@@ -1000,6 +1041,21 @@ class _LocalNvlsGroup(object):
         self.C.nvls_allreduce(None, None, self.g_mc, None, self.pad.table, self.state, self.hyper,
                               self.world.rank, self.world.world, self.timeout_s,
                               1.0 / self.world.world, False, self.grid)
+
+
+def check_gossip_dtype(gossip_dtype, unsupported=None):
+    """Validate a ``gossip_dtype`` argument -> ``torch.bfloat16`` or None (fp32 messages).
+    ``unsupported``: the configuration bf16 messages would be combined with, if that
+    combination is not implemented (the error names it)."""
+    if gossip_dtype in (None, torch.float32):
+        return None
+    if gossip_dtype != torch.bfloat16:
+        raise ValueError('gossip_dtype must be None, torch.float32 or torch.bfloat16, got %r'
+                         % (gossip_dtype,))
+    if unsupported:
+        raise ValueError('gossip_dtype=torch.bfloat16 is not supported with %s; bf16 messages '
+                         'are implemented for synchronous SGP and D-PSGD' % unsupported)
+    return torch.bfloat16
 
 
 def _native_ok() -> bool:

@@ -107,6 +107,14 @@ def build_parser(adpsgd: bool = False) -> argparse.ArgumentParser:
                    help='precision of the gossip messages (GossipDataParallel(gossip_dtype=...)): bf16 '
                         'halves the bytes sent per in-neighbour and conserves push-sum mass exactly; '
                         'parameters stay fp32.  Synchronous SGP and D-PSGD only')
+    p.add_argument('--consensus_freq', default=0, type=int,
+                   help='every N iterations and at each epoch end, log the consensus distance of the '
+                        'ranks\' models (GossipDataParallel.consensus_distance) to stdout and to '
+                        '<checkpoint_dir><tag>consensus_r<rank>_n<world>.csv; 0 = off.  SGP / OSGP / D-PSGD')
+    p.add_argument('--validate_average', default=False, **B,
+                   help='at each epoch end, also validate the push-sum average model (BatchNorm running '
+                        'statistics averaged over the ranks for the purpose) and log its prec@1 in the '
+                        'consensus CSV.  SGP / OSGP / D-PSGD')
     p.add_argument('--nprocs_per_node', default=1, type=int,
                    help='hierarchical mode (GossipDataParallel(nprocs_per_node=K), reference '
                         'gossip/distributed.py:62-80; it has no flag for it): K consecutive ranks form a '
@@ -196,6 +204,15 @@ def finalize_args(args, adpsgd=False):
         if unsupported:
             raise ValueError('--gossip_dtype bf16 is not supported with %s; bf16 messages are '
                              'implemented for synchronous SGP and D-PSGD' % unsupported)
+    if getattr(args, 'consensus_freq', 0) or getattr(args, 'validate_average', False):
+        unsupported = 'AD-PSGD' if adpsgd else '--all_reduce' if args.all_reduce else None
+        if unsupported:
+            raise ValueError('--consensus_freq / --validate_average are not supported with %s: they '
+                             'measure gossip (SGP, OSGP, D-PSGD)' % unsupported)
+        if args.consensus_freq < 0:
+            raise ValueError('--consensus_freq must be >= 0')
+    args.consensus_fname = '{}{}consensus_r{}_n{}.csv'.format(args.checkpoint_dir, args.tag, args.rank,
+                                                              args.world_size)
 
     if args.backend == 'gloo' and args.network_interface_type == 'ethernet':
         try:
@@ -389,6 +406,25 @@ class CSVLog(object):
     def val_row(self, epoch, bt, nt, dt, prec1):
         with open(self.fname, 'a') as f:
             print('{},-1,{},{},{},-1,-1,-1,-1,-1,-1,{}'.format(epoch, bt, nt, dt, prec1), file=f)
+
+
+class ConsensusLog(object):
+    """``--consensus_freq`` / ``--validate_average``: one row per measurement; ``avg_prec1`` is
+    the prec@1 of the push-sum average model (epoch-end rows with ``--validate_average``)."""
+
+    COLUMNS = 'epoch,itr,distance_sq,average_norm_sq,relative,avg_prec1'
+
+    def __init__(self, fname):
+        self.fname = fname
+        if not os.path.exists(fname):
+            with open(fname, 'w') as f:
+                print(self.COLUMNS, file=f)
+
+    def row(self, epoch, itr, stats, avg_prec1=None):
+        with open(self.fname, 'a') as f:
+            print('{},{},{!r},{!r},{!r},{}'.format(epoch, itr, stats.distance_sq, stats.average_norm_sq,
+                                                    stats.relative, '' if avg_prec1 is None else avg_prec1),
+                  file=f)
 
 
 def update_state(state, update_dict):

@@ -30,11 +30,12 @@ import torch.distributed as dist
 import torch.nn as nn
 
 from . import common
-from .common import (CSVLog, Meter, accuracy, build_parser, finalize_args,
+from .common import (CSVLog, ConsensusLog, Meter, accuracy, build_parser, finalize_args,
                      fresh_state, init_model, make_dataloader, update_learning_rate,
                      update_peers_per_itr, update_state)
 from ..experiment import ClusterManager, make_logger
 from ..utils import tracing
+from ..utils.helpers import communicate
 
 
 def parse_args(argv=None):
@@ -147,6 +148,8 @@ def main(argv=None):
     data_meter = Meter(state['data_meter'])
     nn_meter = Meter(state['nn_meter'])
     csv = CSVLog(args.out_fname, args.world_size, args.num_dataloader_workers, args.batch_size)
+    args._consensus_log = (ConsensusLog(args.consensus_fname)
+                           if args.consensus_freq > 0 or args.validate_average else None)
 
     loader, sampler = make_dataloader(args, train=True)
     val_loader = None if args.train_fast else make_dataloader(args, train=False)
@@ -175,6 +178,9 @@ def main(argv=None):
             if prec1 > best_val_prec1:
                 update_state(state, {'is_best': True, 'best_prec1': prec1})
                 best_val_prec1 = prec1
+        if args._consensus_log is not None:
+            epoch_end_consensus(args, model, criterion, val_loader, epoch, log)
+        if not args.train_fast:
             epoch_id = None if args.overwrite_checkpoints else epoch
             cmanager.save_checkpoint(epoch_id, requeue_on_signal=(epoch != args.num_epochs - 1))
 
@@ -278,6 +284,12 @@ def train(args, model, criterion, optimizer, batch_meter, data_meter, nn_meter, 
                 top5.update(a5, n)
             pending = []
             csv.train_row(epoch, i, batch_meter, nn_meter, data_meter, losses, top1, top5)
+        if getattr(args, '_consensus_log', None) is not None and args.consensus_freq > 0 \
+                and (i + 1) % args.consensus_freq == 0:
+            if trainer is not None:
+                trainer.finish()            # (Overlap-SGP: the trainer holds the pending residual)
+            log_consensus(args, model.consensus_distance(), epoch, i, log)
+            t_batch = time.time()           # (not charged to the next iteration's data time)
         if last:
             break
     if trainer is not None:
@@ -292,6 +304,40 @@ def train(args, model, criterion, optimizer, batch_meter, data_meter, nn_meter, 
             top5.update(a5, n)
     csv.train_row(epoch, i, batch_meter, nn_meter, data_meter, losses, top1, top5)
     return losses.avg
+
+
+def log_consensus(args, stats, epoch, itr, log, avg_prec1=None):
+    log.info('consensus epoch {} itr {}: distance_sq {:.6e} average_norm_sq {:.6e} relative {:.6e}{}'.format(
+        epoch, itr, stats.distance_sq, stats.average_norm_sq, stats.relative,
+        '' if avg_prec1 is None else ' average-model Prec@1 {:.3f}'.format(avg_prec1)))
+    args._consensus_log.row(epoch, itr, stats, avg_prec1)
+
+
+def epoch_end_consensus(args, model, criterion, val_loader, epoch, log):
+    """Consensus distance at the end of an epoch; with ``--validate_average`` also the validation
+    accuracy of the push-sum average model.  BatchNorm running statistics are not gossiped: for
+    that validation they are averaged over the ranks, and restored afterwards."""
+    trainer = getattr(args, '_trainer', None)
+    if trainer is not None:
+        trainer.finish()
+    if not (args.validate_average and val_loader is not None):
+        log_consensus(args, model.consensus_distance(), epoch, -1, log)
+        return
+    bufs = [b for b in model.module.buffers() if b.is_floating_point()]
+    saved = [b.detach().clone() for b in bufs]
+    if args.world_size > 1 and bufs:
+        with torch.no_grad():
+            communicate(bufs, dist.all_reduce)
+            for b in bufs:
+                b.div_(args.world_size)
+    try:
+        with model.averaged() as stats:
+            prec1 = validate(args, val_loader, model, criterion, log)
+    finally:
+        with torch.no_grad():
+            for b, s in zip(bufs, saved):
+                b.copy_(s)
+    log_consensus(args, stats, epoch, -1, log, avg_prec1=prec1)
 
 
 def validate(args, val_loader, model, criterion, log):

@@ -357,6 +357,58 @@ public:
                                           args_.timeout_ns, at::cuda::getCurrentCUDAStream()));
     }
 
+    // consensus collective: `slot_ptrs` [world] int64 base pointers of every rank's symmetric slot
+    // buffer (>= 4 doubles each), `scratch` a local fp64 buffer of MAX_CTAS * 4 + 1 zeroed words,
+    // `result` the fp64 [2 + world] tensor every call writes and returns
+    void set_consensus_buffers(torch::Tensor slot_ptrs, torch::Tensor scratch, torch::Tensor result, int grid)
+    {
+        TORCH_CHECK(slot_ptrs.is_cuda() && slot_ptrs.scalar_type() == torch::kInt64 && slot_ptrs.numel() == args_.world);
+        TORCH_CHECK(scratch.is_cuda() && scratch.scalar_type() == torch::kFloat64 && scratch.is_contiguous() &&
+                    scratch.numel() >= (int64_t)SGP_MAX_CTAS * 4 + 1);
+        TORCH_CHECK(result.is_cuda() && result.scalar_type() == torch::kFloat64 && result.is_contiguous() &&
+                    result.numel() == 2 + args_.world);
+        TORCH_CHECK(grid >= 1 && grid <= SGP_MAX_CTAS, "grid out of range");
+        cons_result_ = result;
+        cons_slots_ = slot_ptrs;
+        cons_scratch_ = scratch;
+        cons_grid_ = grid;
+    }
+
+    // Consensus distance over every rank's de-biased parameters (collective, stream-ordered, no
+    // host synchronisation and without allocating: an allocation may wait for the device, where
+    // another virtual rank of this process can be waiting in a barrier for this one).  Returns the
+    // result tensor (fp64 [2 + world], rewritten by the next call): distance_sq, |zbar|^2, then
+    // |z_r - zbar|^2 per rank (full mode; zeros in slice mode).  full: every rank computes the whole
+    // push-sum average zbar into `out` (fp32, length n).
+    torch::Tensor consensus(c10::optional<torch::Tensor> out, bool full)
+    {
+        TORCH_CHECK(args_.outboxes, "consensus needs outboxes");
+        TORCH_CHECK(cons_slots_.defined(), "consensus buffers are not set (set_consensus_buffers)");
+        float* avg = nullptr;
+        if (full) {
+            TORCH_CHECK(out.has_value() && out->defined(), "full mode needs an output tensor");
+            TORCH_CHECK(out->is_cuda() && out->get_device() == device_ && out->scalar_type() == torch::kFloat32 &&
+                        out->is_contiguous() && out->numel() == args_.n,
+                        "out must be a contiguous fp32 tensor of ", args_.n, " elements on the arena's device");
+            avg = out->data_ptr<float>();
+        }
+        c10::cuda::CUDAGuard guard(device_);
+        torch::Tensor result = cons_result_;
+        SgpArgs a = prepare(0);
+        auto slots = reinterpret_cast<double* const*>(cons_slots_.data_ptr<int64_t>());
+        auto st = at::cuda::getCurrentCUDAStream();
+        // barrier / snapshot / barrier / consensus / barrier / finalize / barrier: see sgp_kernels.cu
+        barrier();
+        SGP_CUDA_CHECK(sgp_launch_snapshot(&a, st));
+        barrier();
+        SGP_CUDA_CHECK(sgp_launch_consensus(&a, slots, cons_scratch_.data_ptr<double>(), avg, full ? 1 : 0,
+                                            cons_grid_, st));
+        barrier();
+        SGP_CUDA_CHECK(sgp_launch_consensus_finalize(&a, slots, result.data_ptr<double>(), full ? 1 : 0, st));
+        barrier();
+        return result;
+    }
+
     void set_timeout(double seconds) { args_.timeout_ns = (unsigned long long)(seconds * 1e9); }
     void set_segments(int k) { TORCH_CHECK(k >= 1 && k < SGP_SEQ_STRIDE); args_.segments = k; }
     int segments() const { return args_.segments; }
@@ -394,6 +446,10 @@ private:
     torch::Tensor grad_keep_;
     torch::Tensor grad2_keep_;
     torch::Tensor mom_keep_;
+    torch::Tensor cons_slots_;
+    torch::Tensor cons_scratch_;
+    torch::Tensor cons_result_;
+    int cons_grid_ = 1;
 };
 
 // ---------------------------------------------------------------------------
@@ -736,5 +792,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, mod)
         .def("gather_dma", &GossipContext::gather_dma, py::arg("pub_grid"), py::arg("src_ptr"))
         .def("probe", &GossipContext::probe, py::arg("pub_grid"), py::arg("host_flag") = py::none())
         .def("allreduce_sgd", &GossipContext::allreduce_sgd)
-        .def("barrier", &GossipContext::barrier);
+        .def("barrier", &GossipContext::barrier)
+        .def("set_consensus_buffers", &GossipContext::set_consensus_buffers, py::arg("slot_ptrs"),
+             py::arg("scratch"), py::arg("result"), py::arg("grid"))
+        .def("consensus", &GossipContext::consensus, py::arg("out") = py::none(), py::arg("full") = false);
 }

@@ -4,7 +4,8 @@
 //   * every rank owns, in NVSwitch peer-mapped ("symmetric") memory,
 //       - a signal pad  (SgpSignalPad): sequence flags + push-sum weight
 //       - an outbox     (2 x n floats, double buffered by step parity; 2 x n bf16 with
-//                        SGP_F_MSG_BF16)
+//                        SGP_F_MSG_BF16; between two barriers the consensus collective
+//                        borrows words [0, n) for an fp32 snapshot of z)
 //   * a gossip step is a PULL: the producer writes its outbox and releases a
 //     per-CTA sequence flag; consumers acquire the flag over NVLink and read
 //     the outbox with 16-byte P2P loads, applying the edge weight while they
@@ -43,7 +44,9 @@ struct __align__(128) SgpSignalPad {
     uint32_t ack_seq[SGP_MAX_RANKS];
     // push-sum weight that belongs to outbox[parity]
     float    psw[2];
-    uint32_t _pad0[30];
+    // consensus: push-sum weight of the fp32 snapshot in outbox words [0, n) (sgp_snapshot_kernel)
+    float    snap_w;
+    uint32_t _pad0[29];
     // device barrier: bar_seq[r] is bumped by rank r
     uint32_t bar_seq[SGP_MAX_RANKS];
     // AD-PSGD bilateral handshake (round counters)
@@ -291,6 +294,12 @@ cudaError_t sgp_launch_barrier(SgpSignalPad* const* pads, SgpState* st, int rank
                                unsigned long long timeout_ns, cudaStream_t stream);
 cudaError_t sgp_launch_allreduce_sgd(const SgpArgs* args, void* const* grad_peers, int grid,
                                      cudaStream_t stream);
+// consensus distance / push-sum average model (see sgp_consensus_kernel)
+cudaError_t sgp_launch_snapshot(const SgpArgs* args, cudaStream_t stream);
+cudaError_t sgp_launch_consensus(const SgpArgs* args, double* const* partials, double* scratch, float* avg_out,
+                                 int full, int grid, cudaStream_t stream);
+cudaError_t sgp_launch_consensus_finalize(const SgpArgs* args, double* const* partials, double* result, int full,
+                                          cudaStream_t stream);
 int sgp_max_resident_ctas(int device);
 cudaError_t sgp_preload_kernels();
 }

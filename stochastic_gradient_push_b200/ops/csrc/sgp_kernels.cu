@@ -1254,6 +1254,218 @@ sgp_peer_reduce_kernel(float* __restrict__ dst, const SgpPtrList srcs, long long
 }
 
 // ---------------------------------------------------------------------------
+// Consensus distance and push-sum average model (a collective of every rank; the launcher
+// brackets each step with sgp_barrier_kernel):
+//
+//   barrier   nobody still reads an outbox
+//   sgp_snapshot_kernel            outbox words [0, n) <- z (fp32), pad.snap_w <- w
+//   barrier
+//   sgp_consensus_kernel<FULL>     per element, over every rank's snapshot (TMA ring, items are
+//                                  (chunk, rank) pairs, rank fastest, so each peer byte crosses
+//                                  NVLink once): weighted running mean zbar and unweighted
+//                                  Welford mean m / M2, then sum_j (z_j - zbar)^2 = M2 + n (m - zbar)^2
+//                                  (one pass; sum z^2 - n zbar^2 would cancel catastrophically
+//                                  exactly when the ranks agree).  Per-thread sums in fp64, CTA
+//                                  and grid reductions in a fixed order; the last CTA stores the
+//                                  rank's partials into its symmetric slot.
+//                                  slice (FULL = false): rank r covers chunks [rC/n, (r+1)C/n)
+//                                  full: every rank covers everything, writes zbar and its own
+//                                  |z_r - zbar|^2
+//   barrier
+//   sgp_consensus_finalize_kernel  sum the ranks' slots in rank order -> result (identical bits
+//                                  on every rank)
+//   barrier   nobody still reads a snapshot / slot when the next step overwrites them
+//
+// zbar is accumulated as the weighted running mean zbar_j = zbar_{j-1} + (w_j / W_j)(z_j - zbar_{j-1})
+// (W_j = w_0 + .. + w_j) rather than as (sum_j w_j z_j) / W: the same quantity up to fp32 rounding,
+// but identical replicas give zbar == z exactly, whatever the weights, so their distance is 0.
+// The snapshot never touches pub_seq / ack_seq / psw: the next gossip step publishes with the
+// sequence numbers it would have used anyway.
+// ---------------------------------------------------------------------------
+#define SGP_CONS_STAGES 6
+#define SGP_CONS_SMEM   (SGP_CONS_STAGES * SGP_TMA_BYTES + SGP_CONS_STAGES * 8 + 64)
+#define SGP_CONS_SLOT   4      // doubles per rank: [sum_j (z_j - zbar)^2, |zbar|^2, |z_rank - zbar|^2, -]
+
+__global__ void __launch_bounds__(SGP_THREADS)
+sgp_snapshot_kernel(const SgpArgs a)
+{
+    float4* dst = reinterpret_cast<float4*>(a.outboxes[a.rank]);
+    const float4* src = reinterpret_cast<const float4*>(a.z);
+    const long long n4 = a.n / 4;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4;
+         i += (long long)gridDim.x * blockDim.x)
+        dst[i] = src[i];
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        const uint32_t step = *((volatile uint32_t*)&a.st->step);
+        *((volatile float*)&a.pads[a.rank]->snap_w) = *((volatile float*)&a.st->ps_weight[step & 1u]);
+    }
+}
+
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+    return v;
+}
+
+template <bool FULL>
+__global__ void __launch_bounds__(SGP_THREADS, 2)
+sgp_consensus_kernel(const SgpArgs a, double* const* partials, double* scratch, float* avg_out)
+{
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    float* ring = reinterpret_cast<float*>(smem_raw);                       // [STAGES][CHUNK]
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + SGP_CONS_STAGES * SGP_TMA_BYTES);
+    __shared__ float  s_f[SGP_MAX_RANKS];              // w_j / W_j   (weighted running mean)
+    __shared__ float  s_inv[SGP_MAX_RANKS];            // 1 / (j + 1) (Welford)
+    __shared__ double s_red[3][SGP_THREADS / 32];
+    __shared__ int    s_last;
+
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int world = a.world;
+    const long long nchunks = a.n / SGP_CHUNK;
+    const long long lo = FULL ? 0 : nchunks * a.rank / world;
+    const long long hi = FULL ? nchunks : nchunks * (a.rank + 1) / world;
+
+    if (tid == 0) {
+        float wsum = 0.f;
+        for (int j = 0; j < world; ++j) {
+            const float wj = ld_relaxed_sys_f32(&a.pads[j]->snap_w);
+            wsum += wj;
+            s_f[j] = wj / wsum;
+            s_inv[j] = 1.f / (float)(j + 1);
+        }
+        for (int i = 0; i < SGP_CONS_STAGES; ++i) mbar_init(&full[i], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    const long long span = hi - lo;
+    const long long my_chunks = (span > blockIdx.x) ? (span - 1 - blockIdx.x) / gridDim.x + 1 : 0;
+    const long long items = my_chunks * world;
+
+    auto issue = [&](long long item) {
+        const long long it = item / world;
+        const int j = (int)(item - it * world);
+        const long long c = lo + blockIdx.x + it * gridDim.x;
+        const int stage = (int)(item % SGP_CONS_STAGES);
+        mbar_expect_tx(&full[stage], SGP_TMA_BYTES);
+        tma_load_1d(ring + (size_t)stage * SGP_CHUNK, a.outboxes[j] + c * SGP_CHUNK, SGP_TMA_BYTES, &full[stage]);
+    };
+    if (tid == 0)
+        for (long long i = 0; i < items && i < SGP_CONS_STAGES; ++i) issue(i);
+
+    float4 zb[SGP_UNROLL], mu[SGP_UNROLL], m2[SGP_UNROLL], own[SGP_UNROLL];
+    double acc_d = 0.0, acc_n = 0.0, acc_o = 0.0;
+    const double nd = (double)world;
+    for (long long item = 0; item < items; ++item) {
+        const long long it = item / world;
+        const int j = (int)(item - it * world);
+        const int stage = (int)(item % SGP_CONS_STAGES);
+        mbar_wait(&full[stage], (uint32_t)((item / SGP_CONS_STAGES) & 1));
+        const float4* src = reinterpret_cast<const float4*>(ring + (size_t)stage * SGP_CHUNK);
+        const float fj = s_f[j], ij = s_inv[j];
+#pragma unroll
+        for (int u = 0; u < SGP_UNROLL; ++u) {
+            const float4 v = src[tid + u * SGP_THREADS];
+            // (full mode needs no Welford terms: its distance is sum_r |z_r - zbar|^2, each rank
+            // contributing its own term)
+            if (j == 0) {
+                zb[u] = v;
+                if (!FULL) { mu[u] = v; m2[u] = make_float4(0.f, 0.f, 0.f, 0.f); }
+            } else {
+#define SGP_CONS_UPD(e)                                              \
+                {                                                    \
+                    zb[u].e = fmaf(fj, v.e - zb[u].e, zb[u].e);      \
+                    if (!FULL) {                                     \
+                        const float d = v.e - mu[u].e;               \
+                        mu[u].e = fmaf(d, ij, mu[u].e);              \
+                        m2[u].e = fmaf(d, v.e - mu[u].e, m2[u].e);   \
+                    }                                                \
+                }
+                SGP_CONS_UPD(x) SGP_CONS_UPD(y) SGP_CONS_UPD(z) SGP_CONS_UPD(w)
+#undef SGP_CONS_UPD
+            }
+            if (FULL && j == a.rank) own[u] = v;
+        }
+        if (j == world - 1) {
+            const long long c = lo + blockIdx.x + it * gridDim.x;
+#pragma unroll
+            for (int u = 0; u < SGP_UNROLL; ++u) {
+#define SGP_CONS_ACC(e)                                                                 \
+                {                                                                       \
+                    acc_n = fma((double)zb[u].e, (double)zb[u].e, acc_n);               \
+                    if (FULL) {                                                         \
+                        const double o = (double)own[u].e - (double)zb[u].e;            \
+                        acc_o = fma(o, o, acc_o);                                       \
+                    } else {                                                            \
+                        const double dm = (double)mu[u].e - (double)zb[u].e;            \
+                        acc_d += fma(nd * dm, dm, (double)m2[u].e);                     \
+                    }                                                                   \
+                }
+                SGP_CONS_ACC(x) SGP_CONS_ACC(y) SGP_CONS_ACC(z) SGP_CONS_ACC(w)
+#undef SGP_CONS_ACC
+                if (FULL)
+                    st_f4(reinterpret_cast<float4*>(avg_out + c * SGP_CHUNK) + tid + u * SGP_THREADS, zb[u]);
+            }
+        }
+        __syncthreads();                         // every thread is done with this stage
+        if (tid == 0 && item + SGP_CONS_STAGES < items) {
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads -> async write
+            issue(item + SGP_CONS_STAGES);
+        }
+    }
+
+    // CTA reduction in a fixed order (shuffle tree, then warps 0..7), then the grid: the last CTA
+    // sums the CTA partials in CTA order
+    acc_d = warp_sum_f64(acc_d);
+    acc_n = warp_sum_f64(acc_n);
+    acc_o = warp_sum_f64(acc_o);
+    if (lane == 0) { s_red[0][warp] = acc_d; s_red[1][warp] = acc_n; s_red[2][warp] = acc_o; }
+    __syncthreads();
+    unsigned int* counter = reinterpret_cast<unsigned int*>(scratch + (size_t)SGP_MAX_CTAS * SGP_CONS_SLOT);
+    if (tid == 0) {
+        double t[3] = {0.0, 0.0, 0.0};
+        for (int q = 0; q < 3; ++q)
+            for (int w = 0; w < SGP_THREADS / 32; ++w) t[q] += s_red[q][w];
+        double* mine = scratch + (size_t)blockIdx.x * SGP_CONS_SLOT;
+        mine[0] = t[0]; mine[1] = t[1]; mine[2] = t[2];
+        __threadfence();
+        s_last = atomicAdd(counter, 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (tid == 0 && s_last) {
+        __threadfence();
+        double t[3] = {0.0, 0.0, 0.0};
+        for (unsigned int b = 0; b < gridDim.x; ++b)
+            for (int q = 0; q < 3; ++q) t[q] += ((volatile double*)scratch)[(size_t)b * SGP_CONS_SLOT + q];
+        volatile double* slot = partials[a.rank];
+        slot[0] = t[0];
+        slot[1] = t[1];
+        slot[2] = t[2];
+        *((volatile unsigned int*)counter) = 0u;
+        __threadfence_system();
+    }
+}
+
+// result[0] = distance_sq, result[1] = |zbar|^2, result[2 + r] = |z_r - zbar|^2 (full mode; 0 in
+// slice mode).  Every rank sums the same slots in the same order.  NaN after a timed-out barrier.
+__global__ void sgp_consensus_finalize_kernel(const SgpArgs a, double* const* partials, double* result, int full)
+{
+    if (threadIdx.x != 0) return;
+    double d = 0.0, nrm = 0.0;
+    for (int r = 0; r < a.world; ++r) {
+        const volatile double* p = partials[r];
+        const double own = p[2];
+        d += full ? own : p[0];
+        if (!full) nrm += p[1];
+        result[2 + r] = full ? own : 0.0;
+    }
+    if (full) nrm = ((const volatile double*)partials[0])[1];
+    const bool ok = *((volatile uint32_t*)&a.st->status) == SGP_OK;
+    result[0] = ok ? d / (double)a.world : __longlong_as_double(0x7ff8000000000000ll);
+    result[1] = ok ? nrm : __longlong_as_double(0x7ff8000000000000ll);
+}
+
+// ---------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------
 // bf16 messages are implemented for the full synchronous step only
@@ -1431,6 +1643,48 @@ cudaError_t sgp_launch_scale(float* x, long long n, const float* scalar, int inv
     return cudaGetLastError();
 }
 
+cudaError_t sgp_launch_snapshot(const SgpArgs* args, cudaStream_t stream)
+{
+    if (!args->outboxes || (args->n & 3)) return cudaErrorInvalidValue;
+    const long long n4 = args->n / 4;
+    int grid = (int)((n4 + SGP_THREADS - 1) / SGP_THREADS);
+    if (grid > 132 * 8) grid = 132 * 8;
+    if (grid < 1) grid = 1;
+    sgp_snapshot_kernel<<<grid, SGP_THREADS, 0, stream>>>(*args);
+    return cudaGetLastError();
+}
+
+// scratch: SGP_MAX_CTAS * SGP_CONS_SLOT doubles of CTA partials + one zeroed 32-bit counter
+cudaError_t sgp_launch_consensus(const SgpArgs* args, double* const* partials, double* scratch, float* avg_out,
+                                 int full, int grid, cudaStream_t stream)
+{
+    if (!args->outboxes || grid < 1 || grid > SGP_MAX_CTAS || (full && !avg_out)) return cudaErrorInvalidValue;
+    static bool configured[64] = {};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev < 0 || dev >= 64 || !configured[dev]) {
+        cudaError_t e = cudaFuncSetAttribute(sgp_consensus_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             SGP_CONS_SMEM);
+        if (e == cudaSuccess)
+            e = cudaFuncSetAttribute(sgp_consensus_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     SGP_CONS_SMEM);
+        if (e != cudaSuccess) return e;
+        if (dev >= 0 && dev < 64) configured[dev] = true;
+    }
+    if (full)
+        sgp_consensus_kernel<true><<<grid, SGP_THREADS, SGP_CONS_SMEM, stream>>>(*args, partials, scratch, avg_out);
+    else
+        sgp_consensus_kernel<false><<<grid, SGP_THREADS, SGP_CONS_SMEM, stream>>>(*args, partials, scratch, avg_out);
+    return cudaGetLastError();
+}
+
+cudaError_t sgp_launch_consensus_finalize(const SgpArgs* args, double* const* partials, double* result, int full,
+                                          cudaStream_t stream)
+{
+    sgp_consensus_finalize_kernel<<<1, 32, 0, stream>>>(*args, partials, result, full);
+    return cudaGetLastError();
+}
+
 // Load every gossip kernel into the current device's context now.  Under lazy module loading a
 // kernel is loaded at its first launch, and loading can wait for the whole device.  A process that
 // drives several ranks (one GPU each, or virtual ranks sharing one GPU) would then wait for one
@@ -1443,7 +1697,9 @@ cudaError_t sgp_preload_kernels()
         (const void*)sgp_step_pipe_kernel<true>, (const void*)sgp_probe_kernel, (const void*)sgp_gather_wait_kernel,
         (const void*)sgp_gather_ack_kernel, (const void*)sgp_bilat_decide_kernel, (const void*)sgp_bilat_ctl_kernel,
         (const void*)sgp_allreduce_sgd_kernel, (const void*)sgp_zero_kernel, (const void*)sgp_barrier_kernel,
-        (const void*)sgp_scale_kernel, (const void*)sgp_peer_reduce_kernel};
+        (const void*)sgp_scale_kernel, (const void*)sgp_peer_reduce_kernel, (const void*)sgp_snapshot_kernel,
+        (const void*)sgp_consensus_kernel<false>, (const void*)sgp_consensus_kernel<true>,
+        (const void*)sgp_consensus_finalize_kernel};
     for (const void* k : kernels) {
         cudaFuncAttributes attr;
         const cudaError_t e = cudaFuncGetAttributes(&attr, k);

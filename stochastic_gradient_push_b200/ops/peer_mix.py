@@ -97,6 +97,7 @@ class GossipEngine(object):
             'graph spans %d ranks, symmetric world has %d' % (graph.world_size, self.nranks)
 
         # symmetric allocations (collective across the world)
+        self._name = name
         self.pad = world.alloc(name + '.pad', C.PAD_BYTES)
         elem = 2 if self.msg_bf16 else 4
         self.outbox = world.alloc(name + '.outbox', 2 * self.n * elem)
@@ -299,6 +300,45 @@ class GossipEngine(object):
 
     def barrier(self):
         self.ctx.barrier()
+
+    def consensus(self, out: Optional[torch.Tensor] = None, full: bool = False) -> torch.Tensor:
+        """Consensus distance of the de-biased parameters z_i over every rank (collective: every
+        rank of the world calls it, between gossip steps).  With the push-sum weights w_i,
+        zbar = sum_i w_i z_i / sum_i w_i; returns an fp64 device tensor ``[2 + world]``:
+        ``[distance_sq = (1/n) sum_i |z_i - zbar|^2, |zbar|^2, |z_0 - zbar|^2, ...]`` (the per-rank
+        terms only with ``full=True``; zeros otherwise), bit-identical on every rank.  The tensor is
+        this engine's result buffer: the next call rewrites it.
+
+        ``full=False``: each rank reduces a 1/world slice of the elements (NVLink ingress about one
+        model per rank).  ``full=True``: every rank computes the whole zbar into ``out`` (fp32,
+        length n, required).
+
+        Stream-ordered on the current stream, without a host synchronisation and without
+        allocating after the first call (loop-back
+        tests enqueue every virtual rank before synchronising).  The outbox is borrowed between
+        device barriers; the gossip sequence numbers are untouched, so the next step runs as if
+        this call had not happened.  A timed-out barrier yields NaN and raises at :meth:`poll`."""
+        if full and out is None:
+            raise ValueError('GossipEngine.consensus(full=True) writes the average model into `out`')
+        self.prepare_consensus()
+        return self.ctx.consensus(out if full else None, bool(full))
+
+    def prepare_consensus(self):
+        """Allocate what :meth:`consensus` needs (collective, once; consensus() calls it on first
+        use).  A process that drives several virtual ranks from several threads calls it on every
+        rank first: an allocation implicitly synchronises the device, which must not happen while
+        another virtual rank's barrier kernel waits for this one."""
+        if getattr(self, '_cons_slots', None) is not None:
+            return
+        C = self.C
+        # 4 doubles per rank, symmetric: every rank reads every rank's partial sums
+        self._cons_slots = self.world.alloc(self._name + '.consensus', 4 * 8)
+        self._cons_scratch = torch.zeros(C.MAX_CTAS * 4 + 1, dtype=torch.float64, device=self.device)
+        self._cons_result = torch.zeros(2 + self.nranks, dtype=torch.float64, device=self.device)
+        sms = torch.cuda.get_device_properties(self.device).multi_processor_count
+        nchunks = self.n // C.CHUNK
+        self.ctx.set_consensus_buffers(self._cons_slots.table, self._cons_scratch, self._cons_result,
+                                       int(max(1, min(2 * sms, nchunks, C.MAX_CTAS))))
 
     # -- host-visible state (each of these synchronises) -------------------- #
     def sync_graph(self):

@@ -51,6 +51,7 @@ from ..ops import oracle
 from ..utils.arena import FlatArena
 from ..utils.helpers import make_logger
 from ..utils.metering import Meter
+from .distributed import consensus_unsupported
 
 
 class BilatGossipDataParallel(Module):
@@ -284,6 +285,9 @@ class BilatGossipDataParallel(Module):
 
     def block(self):
         return          # the reference's barrier is unreachable too (ad_psgd.py:212-215)
+
+    # the ranks never stop at the same point, so a consensus snapshot is not defined
+    consensus_distance = average_model = averaged = consensus_unsupported('BilatGossipDataParallel (AD-PSGD)')
 
     def sync_comms(self):
         self._pull_model()

@@ -33,6 +33,7 @@ from torch.nn.modules import Module
 
 from ..ops import native
 from ..utils.arena import FlatArena
+from .distributed import consensus_unsupported
 from .trainer import GossipTrainer
 
 
@@ -127,6 +128,9 @@ class AllReduceDataParallel(Module):
 
     def forward(self, *a, **kw):
         return self.module(*a, **kw)
+
+    # the replicas are identical by construction: there is no consensus distance to measure
+    consensus_distance = average_model = averaged = consensus_unsupported('AllReduceDataParallel')
 
     def set_hyper(self, lr, momentum, weight_decay, nesterov, grad_scale=1.0):
         key = (float(lr), float(momentum), float(weight_decay), bool(nesterov), float(grad_scale))

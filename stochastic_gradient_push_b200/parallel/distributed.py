@@ -37,7 +37,10 @@ numerator / de-biased alternation.
 
 from __future__ import annotations
 
+import contextlib
+import math
 import time
+from collections import namedtuple
 from typing import Dict
 
 import torch
@@ -53,6 +56,29 @@ from ..utils.arena import FlatArena
 from ..utils.helpers import communicate, create_process_group, group_by_dtype, make_logger
 
 HEARTBEAT_TIMEOUT = 300  # seconds a rank waits for its in-neighbours (reference :36)
+
+
+class ConsensusStats(namedtuple('ConsensusStats', ['distance_sq', 'average_norm_sq', 'rank_distance_sq'])):
+    """Result of :meth:`GossipDataParallel.consensus_distance` / ``average_model``:
+    ``distance_sq = (1/n) sum_i |z_i - zbar|^2``, ``average_norm_sq = |zbar|^2`` and, from
+    ``average_model`` only, ``rank_distance_sq[i] = |z_i - zbar|^2`` (else None)."""
+    __slots__ = ()
+
+    @property
+    def relative(self) -> float:
+        """sqrt(distance_sq / average_norm_sq): the ranks' RMS spread relative to the average"""
+        if self.average_norm_sq > 0:
+            return math.sqrt(self.distance_sq / self.average_norm_sq)
+        return 0.0 if self.distance_sq == 0 else math.inf
+
+
+def consensus_unsupported(kind):
+    """A ``consensus_distance`` / ``average_model`` / ``averaged`` stand-in for wrappers that do
+    not implement them (AD-PSGD, all-reduce): raises ValueError."""
+    def method(self, *args, **kwargs):
+        raise ValueError('consensus_distance(), average_model() and averaged() are implemented by '
+                         'GossipDataParallel (SGP, D-PSGD, Overlap-SGP), not by %s' % kind)
+    return method
 
 
 # --------------------------------------------------------------------------- #
@@ -292,6 +318,8 @@ class GossipDataParallel(Module):
         # (one instance per process: the instance counter; several virtual ranks inside ONE process
         # -- LocalWorld loop-back -- must pass the same explicit name)
         self._symm_name = symmetric_name or ('gdp%d' % self._instance_id)
+        self.last_consensus = None      # ConsensusStats of the last consensus_distance() / average_model()
+        self._gossip_done = None        # consensus: event on gossip_stream (prepare_consensus)
         self.exposed_comm_s = 0.0       # c10d data plane: host seconds blocked waiting for peers
         self.gossip_retries = 0         # interrupted gossip rounds that were re-queued (soft retry)
 
@@ -568,6 +596,136 @@ class GossipDataParallel(Module):
         self.is_ps_numerator = load_dict['is_ps_numerator']
         if self._kernel is not None and self._kernel.shadow is not None:
             self._kernel.shadow.copy_(self.arena.flat)
+
+    # -- consensus: distance and push-sum average model ----------------------- #
+    def consensus_distance(self) -> 'ConsensusStats':
+        """How far the ranks' models are apart.  With z_i the de-biased parameters of rank i and
+        w_i its push-sum weight, zbar = sum_i w_i z_i / sum_i w_i (the point push-sum contracts
+        to) and ``distance_sq = (1/n) sum_i |z_i - zbar|^2``; also ``average_norm_sq = |zbar|^2``
+        and ``.relative = sqrt(distance_sq / average_norm_sq)``.  ``rank_distance_sq`` is None.
+        Identical on every rank.
+
+        Collective: every gossiping rank must call it.  In-flight gossip is drained first (as by
+        :meth:`state_dict`).  With a :class:`GossipTrainer` call ``trainer.finish()`` first: under
+        Overlap-SGP the trainer holds the last residual.  On the NVLink plane each rank reduces a
+        1/n slice of the elements from every rank's snapshot; on the c10d plane it is three
+        all-reduces.  Training continued afterwards is unaffected."""
+        return self._consensus(None, full=False)[1]
+
+    def average_model(self, out=None) -> torch.Tensor:
+        """The push-sum average model zbar as a flat fp32 tensor in the arena's layout
+        (``self.arena.views_of(t)`` gives per-parameter views), written into ``out`` if given.
+        Same collective semantics as :meth:`consensus_distance`; its statistics, with
+        ``rank_distance_sq[i] = |z_i - zbar|^2`` for every rank, are left in
+        :attr:`last_consensus`.  BatchNorm buffers are not gossiped and are not averaged."""
+        return self._consensus(out, full=True)[0]
+
+    @contextlib.contextmanager
+    def averaged(self):
+        """Context manager: the parameters (and the bf16 compute copy, if there is one) hold the
+        push-sum average model inside the block and are restored bit for bit on exit.  Yields
+        the :class:`ConsensusStats` of the average.  Collective (calls :meth:`average_model`);
+        buffers such as BatchNorm running statistics stay local."""
+        avg = self.average_model()
+        flat = self.arena.flat
+        shadow = self.compute_shadow
+        with torch.no_grad():
+            saved = flat.clone()
+            saved_shadow = shadow.clone() if shadow is not None else None
+            flat.copy_(avg)
+            if shadow is not None:
+                shadow.copy_(avg)
+        del avg
+        try:
+            yield self.last_consensus
+        finally:
+            with torch.no_grad():
+                flat.copy_(saved)
+                if shadow is not None:
+                    shadow.copy_(saved_shadow)
+
+    def prepare_consensus(self):
+        """Create what the consensus collectives of the NVLink plane need (they do it on first
+        use; collective).  A process that drives several virtual ranks from several threads calls
+        it on every rank before any of them calls :meth:`consensus_distance`: creating a CUDA
+        event or allocating memory can wait for the shared device, where another virtual rank's
+        barrier kernel waits for this one (see ``GossipEngine.prepare_consensus``)."""
+        if self._kernel is None or self._gossip_done is not None:
+            return
+        self._kernel.engine.prepare_consensus()
+        self._kernel.engine.poll()                  # (allocates its pinned status words)
+        self._gossip_done = torch.cuda.Event()
+        if self.gossip_stream is not None:
+            self._gossip_done.record(self.gossip_stream)     # (creates the event)
+
+    def _consensus(self, out, full):
+        what = 'average_model()' if full else 'consensus_distance()'
+        if self.nprocs_per_node > 1:
+            raise ValueError('%s is not implemented for nprocs_per_node > 1 (hierarchical mode)' % what)
+        if list(self._arenas) != [torch.float32]:
+            raise ValueError('%s needs fp32 parameters' % what)
+        flat = self.arena.flat
+        if full:
+            if out is None:
+                out = torch.empty_like(flat)
+            elif out.dtype != torch.float32 or out.numel() != flat.numel() or out.device != flat.device \
+                    or not out.is_contiguous():
+                raise ValueError('out must be a contiguous fp32 tensor of %d elements on %s'
+                                 % (flat.numel(), flat.device))
+        # drain exactly like state_dict(): every received message folded, every deferred update
+        # applied, parameters de-biased
+        if self.asynch:
+            self._drain_async()
+        self._query_gossip_queue()
+        self._flush_pending(drain=True)
+        self.unbias()
+        world = self.dist_config['world_size']
+        if self._kernel is not None:
+            e = self._kernel.engine
+            self.prepare_consensus()
+            if self.gossip_stream is not None:
+                self._gossip_done.record(self.gossip_stream)
+                torch.cuda.current_stream().wait_event(self._gossip_done)
+            res = e.consensus(out, full).cpu()       # (synchronises)
+            e.poll(blocking=True)
+            vals = [float(v) for v in res]
+            ranks = vals[2:2 + world] if full else None
+            stats = ConsensusStats(vals[0], vals[1], ranks)
+        elif world == 1:
+            with torch.no_grad():
+                if full:
+                    out.copy_(flat)
+                nrm = float(flat.double().pow(2).sum())
+            stats = ConsensusStats(0.0, nrm, [0.0] if full else None)
+        else:
+            stats = self._consensus_c10d(out, full, world)
+        self.last_consensus = stats
+        return out, stats
+
+    def _consensus_c10d(self, out, full, world):
+        """c10d plane: sum w z and sum w (all-reduce), then sum |z - zbar|^2 (all-reduce of a
+        per-rank vector, so that every rank also learns every rank's term), in fp64."""
+        dev = self.dist_config['comm_device']
+        grp = self._masters_group
+        with torch.no_grad():
+            z = self.arena.flat.detach().to(dev, torch.float64)
+            w = float(self._w)
+            s = z * w
+            wsum = torch.tensor([w], dtype=torch.float64, device=dev)
+            dist.all_reduce(s, group=grp)
+            dist.all_reduce(wsum, group=grp)
+            zbar = s.div_(wsum)
+            per_rank = torch.zeros(world, dtype=torch.float64, device=dev)
+            per_rank[self.dist_config['rank']] = (z - zbar).pow_(2).sum()
+            dist.all_reduce(per_rank, group=grp)
+            per_rank = [float(v) for v in per_rank.cpu()]
+            dsq = 0.0
+            for v in per_rank:                  # rank order: the same sum on every rank
+                dsq += v
+            nrm = float(zbar.pow(2).sum())
+            if full:
+                out.copy_(zbar.to(out.device, torch.float32))
+        return ConsensusStats(dsq / world, nrm, per_rank if full else None)
 
     def forward(self, *inputs, **kwargs):
         if self.device_ids:

@@ -20,6 +20,7 @@ Two worlds implement the same small interface (``alloc`` / ``ptr_table``):
 
 from __future__ import annotations
 
+import threading
 from typing import Dict, List, Optional
 
 import torch
@@ -194,6 +195,7 @@ class LocalWorld(object):
                 if d != p and not C.enable_peer_access(d, p):
                     raise RuntimeError('no peer access %d -> %d' % (d, p))
         self.buffers: Dict[str, List[_Buffer]] = {}
+        self.lock = threading.Lock()
 
     def alloc(self, name: str, nbytes: int) -> List[_Buffer]:
         C = self._C
@@ -225,8 +227,9 @@ class _LocalRankView(object):
         self.group = None
 
     def alloc(self, name: str, nbytes: int) -> _Buffer:
-        if name not in self.parent.buffers:
-            self.parent.alloc(name, nbytes)
+        with self.parent.lock:          # virtual ranks may allocate from their own threads
+            if name not in self.parent.buffers:
+                self.parent.alloc(name, nbytes)
         b = self.parent.buffers[name][self.rank]
         assert b.nbytes == nbytes
         return b

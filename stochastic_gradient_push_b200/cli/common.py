@@ -115,6 +115,12 @@ def build_parser(adpsgd: bool = False) -> argparse.ArgumentParser:
                    help='at each epoch end, also validate the push-sum average model (BatchNorm running '
                         'statistics averaged over the ranks for the purpose) and log its prec@1 in the '
                         'consensus CSV.  SGP / OSGP / D-PSGD')
+    p.add_argument('--slowmo_frequency', default=0, type=int,
+                   help='SlowMo (GossipDataParallel(slowmo_frequency=N)): every N iterations, average the '
+                        'ranks\' models exactly and take a slow-momentum step; 0 = off.  SGP / OSGP / '
+                        'D-PSGD with --nprocs_per_node 1')
+    p.add_argument('--slowmo_lr', default=1.0, type=float, help='SlowMo slow learning rate alpha')
+    p.add_argument('--slowmo_momentum', default=0.5, type=float, help='SlowMo slow momentum beta')
     p.add_argument('--nprocs_per_node', default=1, type=int,
                    help='hierarchical mode (GossipDataParallel(nprocs_per_node=K), reference '
                         'gossip/distributed.py:62-80; it has no flag for it): K consecutive ranks form a '
@@ -211,6 +217,14 @@ def finalize_args(args, adpsgd=False):
                              'measure gossip (SGP, OSGP, D-PSGD)' % unsupported)
         if args.consensus_freq < 0:
             raise ValueError('--consensus_freq must be >= 0')
+    if getattr(args, 'slowmo_frequency', 0):
+        unsupported = ('AD-PSGD' if adpsgd else '--all_reduce' if args.all_reduce else
+                       '--nprocs_per_node > 1' if getattr(args, 'nprocs_per_node', 1) > 1 else None)
+        if unsupported:
+            raise ValueError('--slowmo_frequency is not supported with %s: SlowMo is implemented for '
+                             'SGP, OSGP and D-PSGD' % unsupported)
+        from ..parallel.distributed import check_slowmo_args
+        check_slowmo_args(args.slowmo_frequency, args.slowmo_lr, args.slowmo_momentum)
     args.consensus_fname = '{}{}consensus_r{}_n{}.csv'.format(args.checkpoint_dir, args.tag, args.rank,
                                                               args.world_size)
 

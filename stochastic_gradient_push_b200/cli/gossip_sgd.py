@@ -66,6 +66,8 @@ def build_model_and_optimizer(args, log):
         verbose=args.verbose, use_streams=not args.no_cuda_streams, rank=args.rank,
         world_size=args.world_size, transport=args.transport, nprocs_per_node=args.nprocs_per_node,
         gossip_dtype=torch.bfloat16 if args.gossip_dtype == 'bf16' else None,
+        slowmo_frequency=args.slowmo_frequency, slowmo_lr=args.slowmo_lr,
+        slowmo_momentum=args.slowmo_momentum,
         # the captured fast path trains through the bf16 shadow-weight twin (no autocast casts)
         compute_dtype=(torch.bfloat16 if (args.cuda_graph and args.amp and args.fused
                                           and args.device == 'cuda' and args.transport != 'c10d')
@@ -262,6 +264,8 @@ def train(args, model, criterion, optimizer, batch_meter, data_meter, nn_meter, 
                 optimizer.zero_grad()
             if not args.overlap and not args.all_reduce:
                 model.transfer_params()
+            if getattr(args, 'slowmo_frequency', 0):
+                model.perform_slowmo(optimizer)        # (the trainer path runs it inside step())
             with torch.no_grad():
                 p1, p5 = accuracy(output, target, topk=(1, 5))
                 pending.append((torch.stack([loss.detach().float().reshape(()), p1[0], p5[0]]),

@@ -409,6 +409,29 @@ public:
         return result;
     }
 
+    // SlowMo step (collective, stream-ordered, no host synchronisation, no allocation): z, `u` and
+    // `x_prev` (fp32, length n, identical on every rank) from the push-sum average zbar of every
+    // rank's z; both push-sum weights <- 1.  init: x_prev <- zbar, u <- 0.  See sgp_slowmo_kernel.
+    void slowmo(torch::Tensor u, torch::Tensor x_prev, double lr, double alpha, double beta, bool init, int grid)
+    {
+        TORCH_CHECK(args_.outboxes, "slowmo needs outboxes");
+        for (const torch::Tensor* t : {&u, &x_prev})
+            TORCH_CHECK(t->is_cuda() && t->get_device() == device_ && t->scalar_type() == torch::kFloat32 &&
+                        t->is_contiguous() && t->numel() == args_.n,
+                        "u and x_prev must be contiguous fp32 tensors of ", args_.n, " elements on the arena's device");
+        TORCH_CHECK(lr > 0.0, "slowmo: the base learning rate must be > 0");
+        TORCH_CHECK(grid >= 1 && grid <= SGP_MAX_CTAS, "grid out of range");
+        c10::cuda::CUDAGuard guard(device_);
+        SgpArgs a = prepare(0);
+        auto st = at::cuda::getCurrentCUDAStream();
+        barrier();
+        SGP_CUDA_CHECK(sgp_launch_snapshot(&a, st));
+        barrier();
+        SGP_CUDA_CHECK(sgp_launch_slowmo(&a, u.data_ptr<float>(), x_prev.data_ptr<float>(), (float)lr, (float)alpha,
+                                         (float)beta, init ? 1 : 0, grid, st));
+        barrier();
+    }
+
     void set_timeout(double seconds) { args_.timeout_ns = (unsigned long long)(seconds * 1e9); }
     void set_segments(int k) { TORCH_CHECK(k >= 1 && k < SGP_SEQ_STRIDE); args_.segments = k; }
     int segments() const { return args_.segments; }
@@ -795,5 +818,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, mod)
         .def("barrier", &GossipContext::barrier)
         .def("set_consensus_buffers", &GossipContext::set_consensus_buffers, py::arg("slot_ptrs"),
              py::arg("scratch"), py::arg("result"), py::arg("grid"))
-        .def("consensus", &GossipContext::consensus, py::arg("out") = py::none(), py::arg("full") = false);
+        .def("consensus", &GossipContext::consensus, py::arg("out") = py::none(), py::arg("full") = false)
+        .def("slowmo", &GossipContext::slowmo, py::arg("u"), py::arg("x_prev"), py::arg("lr"), py::arg("alpha"),
+             py::arg("beta"), py::arg("init"), py::arg("grid"));
 }

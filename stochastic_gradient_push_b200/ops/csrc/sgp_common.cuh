@@ -300,6 +300,9 @@ cudaError_t sgp_launch_consensus(const SgpArgs* args, double* const* partials, d
                                  int full, int grid, cudaStream_t stream);
 cudaError_t sgp_launch_consensus_finalize(const SgpArgs* args, double* const* partials, double* result, int full,
                                           cudaStream_t stream);
+// SlowMo: exact push-sum average + slow-momentum update (see sgp_slowmo_kernel)
+cudaError_t sgp_launch_slowmo(const SgpArgs* args, float* u, float* x_prev, float lr, float alpha, float beta,
+                              int init, int grid, cudaStream_t stream);
 int sgp_max_resident_ctas(int device);
 cudaError_t sgp_preload_kernels();
 }

@@ -1466,6 +1466,122 @@ __global__ void sgp_consensus_finalize_kernel(const SgpArgs a, double* const* pa
 }
 
 // ---------------------------------------------------------------------------
+// SlowMo (slow momentum over periodic exact averaging; Wang et al., ICLR 2020), a collective of
+// every rank bracketed by device barriers like the consensus collective:
+//
+//   barrier | sgp_snapshot_kernel | barrier | sgp_slowmo_kernel | barrier
+//
+// sgp_slowmo_kernel reads every rank's snapshot through the TMA ring of sgp_consensus_kernel
+// ((chunk, rank) items, rank fastest; every rank covers every chunk) and forms zbar with the same
+// weighted running mean, in the same rank order, so zbar -- and the update -- has the same bits
+// on every rank.  Per element, with gamma = lr:
+//
+//   init:   x_prev <- zbar ; u <- 0 ; z <- zbar
+//   else:   u <- beta u + (x_prev - zbar) / gamma ; x_new <- x_prev - alpha gamma u ;
+//           x_prev <- x_new ; z <- x_new
+//
+// (plus the bf16 shadow of z), then both push-sum weight slots <- 1.  After a timed-out barrier
+// (sticky status != OK) nothing is written: the host raises at poll().  pub_seq / ack_seq / psw
+// and the step counter are not touched, so the next gossip step publishes as it would have; the
+// closing barrier keeps that publish from overwriting a snapshot a slower rank still reads.
+// ---------------------------------------------------------------------------
+__global__ void __launch_bounds__(SGP_THREADS, 2)
+sgp_slowmo_kernel(const SgpArgs a, float* u, float* x_prev, float lr, float alpha, float beta, int init)
+{
+    if (*((volatile uint32_t*)&a.st->status) != SGP_OK) return;
+
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    float* ring = reinterpret_cast<float*>(smem_raw);                       // [STAGES][CHUNK]
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + SGP_CONS_STAGES * SGP_TMA_BYTES);
+    __shared__ float s_f[SGP_MAX_RANKS];              // w_j / W_j   (weighted running mean)
+
+    const int tid = threadIdx.x;
+    const int world = a.world;
+    const long long nchunks = a.n / SGP_CHUNK;
+
+    if (tid == 0) {
+        float wsum = 0.f;
+        for (int j = 0; j < world; ++j) {
+            const float wj = ld_relaxed_sys_f32(&a.pads[j]->snap_w);
+            wsum += wj;
+            s_f[j] = wj / wsum;
+        }
+        for (int i = 0; i < SGP_CONS_STAGES; ++i) mbar_init(&full[i], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        if (blockIdx.x == 0) {
+            *((volatile float*)&a.st->ps_weight[0]) = 1.f;
+            *((volatile float*)&a.st->ps_weight[1]) = 1.f;
+        }
+    }
+    __syncthreads();
+
+    const long long my_chunks = (nchunks > blockIdx.x) ? (nchunks - 1 - blockIdx.x) / gridDim.x + 1 : 0;
+    const long long items = my_chunks * world;
+
+    auto issue = [&](long long item) {
+        const long long it = item / world;
+        const int j = (int)(item - it * world);
+        const long long c = blockIdx.x + it * gridDim.x;
+        const int stage = (int)(item % SGP_CONS_STAGES);
+        mbar_expect_tx(&full[stage], SGP_TMA_BYTES);
+        tma_load_1d(ring + (size_t)stage * SGP_CHUNK, a.outboxes[j] + c * SGP_CHUNK, SGP_TMA_BYTES, &full[stage]);
+    };
+    if (tid == 0)
+        for (long long i = 0; i < items && i < SGP_CONS_STAGES; ++i) issue(i);
+
+    const uint64_t pol_first = l2_evict_first_policy();
+    const float alr = alpha * lr;
+    float4 zb[SGP_UNROLL];
+    for (long long item = 0; item < items; ++item) {
+        const long long it = item / world;
+        const int j = (int)(item - it * world);
+        const int stage = (int)(item % SGP_CONS_STAGES);
+        mbar_wait(&full[stage], (uint32_t)((item / SGP_CONS_STAGES) & 1));
+        const float4* src = reinterpret_cast<const float4*>(ring + (size_t)stage * SGP_CHUNK);
+        const float fj = s_f[j];
+#pragma unroll
+        for (int k = 0; k < SGP_UNROLL; ++k) {
+            const float4 v = src[tid + k * SGP_THREADS];
+            if (j == 0) {
+                zb[k] = v;
+            } else {
+                zb[k].x = fmaf(fj, v.x - zb[k].x, zb[k].x);
+                zb[k].y = fmaf(fj, v.y - zb[k].y, zb[k].y);
+                zb[k].z = fmaf(fj, v.z - zb[k].z, zb[k].z);
+                zb[k].w = fmaf(fj, v.w - zb[k].w, zb[k].w);
+            }
+        }
+        __syncthreads();                         // every thread is done with this stage
+        if (tid == 0 && item + SGP_CONS_STAGES < items) {
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads -> async write
+            issue(item + SGP_CONS_STAGES);
+        }
+        if (j == world - 1) {
+            const long long c = blockIdx.x + it * gridDim.x;
+#pragma unroll
+            for (int k = 0; k < SGP_UNROLL; ++k) {
+                const long long i4 = c * (SGP_CHUNK / 4) + tid + k * SGP_THREADS;
+                float4 xn = zb[k], un = make_float4(0.f, 0.f, 0.f, 0.f);
+                if (!init) {
+                    const float4 up = ld_once_f4(reinterpret_cast<const float4*>(u) + i4, pol_first);
+                    const float4 xp = ld_once_f4(reinterpret_cast<const float4*>(x_prev) + i4, pol_first);
+#define SGP_SLOWMO_UPD(e)                                                   \
+                    un.e = fmaf(beta, up.e, __fdiv_rn(xp.e - zb[k].e, lr)); \
+                    xn.e = fmaf(-alr, un.e, xp.e);
+                    SGP_SLOWMO_UPD(x) SGP_SLOWMO_UPD(y) SGP_SLOWMO_UPD(z) SGP_SLOWMO_UPD(w)
+#undef SGP_SLOWMO_UPD
+                }
+                st_hint_f4(reinterpret_cast<float4*>(u) + i4, un, pol_first);
+                st_hint_f4(reinterpret_cast<float4*>(x_prev) + i4, xn, pol_first);
+                st_f4(reinterpret_cast<float4*>(a.z) + i4, xn);
+                if (a.shadow)
+                    st_u2(reinterpret_cast<uint2*>(a.shadow) + i4, f4_to_bf16x4(xn));
+            }
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------
 // bf16 messages are implemented for the full synchronous step only
@@ -1685,6 +1801,23 @@ cudaError_t sgp_launch_consensus_finalize(const SgpArgs* args, double* const* pa
     return cudaGetLastError();
 }
 
+cudaError_t sgp_launch_slowmo(const SgpArgs* args, float* u, float* x_prev, float lr, float alpha, float beta,
+                              int init, int grid, cudaStream_t stream)
+{
+    if (!args->outboxes || !u || !x_prev || grid < 1 || grid > SGP_MAX_CTAS) return cudaErrorInvalidValue;
+    static bool configured[64] = {};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev < 0 || dev >= 64 || !configured[dev]) {
+        const cudaError_t e = cudaFuncSetAttribute(sgp_slowmo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                   SGP_CONS_SMEM);
+        if (e != cudaSuccess) return e;
+        if (dev >= 0 && dev < 64) configured[dev] = true;
+    }
+    sgp_slowmo_kernel<<<grid, SGP_THREADS, SGP_CONS_SMEM, stream>>>(*args, u, x_prev, lr, alpha, beta, init);
+    return cudaGetLastError();
+}
+
 // Load every gossip kernel into the current device's context now.  Under lazy module loading a
 // kernel is loaded at its first launch, and loading can wait for the whole device.  A process that
 // drives several ranks (one GPU each, or virtual ranks sharing one GPU) would then wait for one
@@ -1699,7 +1832,7 @@ cudaError_t sgp_preload_kernels()
         (const void*)sgp_allreduce_sgd_kernel, (const void*)sgp_zero_kernel, (const void*)sgp_barrier_kernel,
         (const void*)sgp_scale_kernel, (const void*)sgp_peer_reduce_kernel, (const void*)sgp_snapshot_kernel,
         (const void*)sgp_consensus_kernel<false>, (const void*)sgp_consensus_kernel<true>,
-        (const void*)sgp_consensus_finalize_kernel};
+        (const void*)sgp_consensus_finalize_kernel, (const void*)sgp_slowmo_kernel};
     for (const void* k : kernels) {
         cudaFuncAttributes attr;
         const cudaError_t e = cudaFuncGetAttributes(&attr, k);

@@ -340,6 +340,24 @@ class GossipEngine(object):
         self.ctx.set_consensus_buffers(self._cons_slots.table, self._cons_scratch, self._cons_result,
                                        int(max(1, min(2 * sms, nchunks, C.MAX_CTAS))))
 
+    def slowmo(self, u: torch.Tensor, x_prev: torch.Tensor, lr: float, alpha: float, beta: float,
+               init: bool):
+        """SlowMo step (collective: every rank of the world calls it, between gossip steps).  With
+        zbar = sum_i w_i z_i / sum_i w_i, the same bits on every rank:
+
+            init:  x_prev <- zbar ; u <- 0 ; z <- zbar
+            else:  u <- beta u + (x_prev - zbar) / lr ; x_prev <- x_prev - alpha lr u ; z <- x_prev
+
+        ``u`` / ``x_prev`` are fp32 tensors of the arena's length, identical on every rank; the
+        bf16 shadow follows z, and both push-sum weights become 1.  Stream-ordered on the current
+        stream, without a host synchronisation or an allocation; the step counter and the gossip
+        sequence numbers are untouched.  A timed-out barrier leaves z, u, x_prev and the weights as
+        they were and raises at :meth:`poll`."""
+        C = self.C
+        sms = torch.cuda.get_device_properties(self.device).multi_processor_count
+        grid = int(max(1, min(2 * sms, self.n // C.CHUNK, C.MAX_CTAS)))
+        self.ctx.slowmo(u, x_prev, float(lr), float(alpha), float(beta), bool(init), grid)
+
     # -- host-visible state (each of these synchronises) -------------------- #
     def sync_graph(self):
         """Advance the python GraphManager to the device's phase."""

@@ -39,6 +39,7 @@ from __future__ import annotations
 
 import contextlib
 import math
+import numbers
 import time
 from collections import namedtuple
 from typing import Dict
@@ -304,8 +305,15 @@ class GossipDataParallel(Module):
                  nprocs_per_node=1, local_node_group=None,
                  transport='auto', compute_dtype=None, symmetric_world=None,
                  heartbeat_timeout=HEARTBEAT_TIMEOUT, grid=None, symmetric_name=None,
-                 gossip_dtype=None):
+                 gossip_dtype=None, slowmo_frequency=0, slowmo_lr=1.0, slowmo_momentum=0.5):
         super(GossipDataParallel, self).__init__()
+        # SlowMo (perform_slowmo): every slowmo_frequency optimizer steps, exact average + slow
+        # momentum step with learning rate slowmo_lr and momentum slowmo_momentum; 0 = off
+        self.slowmo_frequency, self.slowmo_lr, self.slowmo_momentum = check_slowmo_args(
+            slowmo_frequency, slowmo_lr, slowmo_momentum)
+        if self.slowmo_frequency and nprocs_per_node > 1:
+            raise ValueError('SlowMo (slowmo_frequency > 0) is not implemented for nprocs_per_node > 1 '
+                             '(hierarchical mode)')
         # bf16 gossip messages: half the bytes per in-neighbour, push-sum mass conserved exactly
         # (the sender keeps what it did not send); parameters and push-sum weights stay fp32
         self.gossip_dtype = check_gossip_dtype(
@@ -419,6 +427,17 @@ class GossipDataParallel(Module):
             self._build_local_replicas()
 
         all_fp32 = list(by_dtype.keys()) == [torch.float32]
+        # SlowMo state, fp32, arena-sized and identical on every rank: slow momentum u and the model
+        # at the start of the outer iteration x_prev.  Allocated here because the collective must not
+        # allocate (virtual loop-back ranks run it from threads, see prepare_consensus)
+        self._slowmo_u = self._slowmo_x_prev = None
+        self._slowmo_initialized = False
+        self._slowmo_calls = 0
+        if self.slowmo_frequency:
+            if not all_fp32:
+                raise ValueError('SlowMo (slowmo_frequency > 0) needs fp32 parameters')
+            self._slowmo_u = torch.zeros_like(self._arenas[torch.float32].flat)
+            self._slowmo_x_prev = torch.zeros_like(self._slowmo_u)
         if transport == 'auto':
             use_kernels = on_cuda and not self.__cpu_comm and all_fp32 and _native_ok()
             # the kernel data plane maps every peer's buffers over CUDA IPC / NVSwitch: it needs
@@ -587,6 +606,11 @@ class GossipDataParallel(Module):
         if self.gossip_dtype is not None:
             # informational: parameters are fp32 either way, so a checkpoint loads across dtypes
             out['gossip_dtype'] = 'bfloat16'
+        if self.slowmo_frequency:
+            out['slowmo'] = {'u': self._slowmo_u.detach().cpu().clone(),
+                             'x_prev': self._slowmo_x_prev.detach().cpu().clone(),
+                             'initialized': self._slowmo_initialized,
+                             'calls': self._slowmo_calls}
         return out
 
     def load_state_dict(self, load_dict, *args, **kwargs):
@@ -596,6 +620,99 @@ class GossipDataParallel(Module):
         self.is_ps_numerator = load_dict['is_ps_numerator']
         if self._kernel is not None and self._kernel.shadow is not None:
             self._kernel.shadow.copy_(self.arena.flat)
+        sm = load_dict.get('slowmo')
+        if sm is not None and self.slowmo_frequency:
+            self._slowmo_u.copy_(sm['u'])
+            self._slowmo_x_prev.copy_(sm['x_prev'])
+            self._slowmo_initialized = bool(sm['initialized'])
+            self._slowmo_calls = int(sm['calls'])
+
+    # -- SlowMo: slow momentum over periodic exact averaging ------------------- #
+    def perform_slowmo(self, optimizer) -> bool:
+        """SlowMo (Wang et al., ICLR 2020) on top of gossip.  Call it after every optimizer step
+        (in synchronous mode after ``transfer_params()``).  Every ``slowmo_frequency``-th call it
+        drains in-flight gossip (as :meth:`state_dict` does), takes the push-sum average
+        zbar = sum_i w_i z_i / sum_i w_i of the ranks' de-biased parameters and, with
+        gamma = ``optimizer.param_groups[0]['lr']``, alpha = ``slowmo_lr``, beta = ``slowmo_momentum``:
+
+            u <- beta u + (x_prev - zbar) / gamma ;  x_prev <- x_prev - alpha gamma u ;  z_i <- x_prev
+
+        and resets every push-sum weight to 1.  The first such call only averages (x_prev <- zbar,
+        u <- 0): no collective is needed at construction, at the cost of one period of slow
+        momentum (the paper starts x_prev at the initial point).  Afterwards every rank holds the
+        same parameters, u and x_prev.  The base optimizer's momentum and the BatchNorm buffers are
+        left alone; beta = 0, alpha = 1 is periodic exact averaging.
+
+        Returns True when the step ran (collective on those calls), False otherwise (always with
+        ``slowmo_frequency=0``).  With a :class:`GossipTrainer` do not call it: ``trainer.step()``
+        runs the step itself."""
+        gamma = self._slowmo_tick(optimizer)
+        if gamma is None:
+            return False
+        if self.asynch:
+            self._drain_async()
+        self._query_gossip_queue()
+        self._flush_pending(drain=True)
+        self.unbias()
+        if self._kernel is not None:
+            e = self._kernel.engine
+            self.prepare_consensus()
+            if self.gossip_stream is not None:
+                self._gossip_done.record(self.gossip_stream)
+                torch.cuda.current_stream().wait_event(self._gossip_done)
+            self._slowmo_launch(gamma)
+            e.poll(blocking=True)
+        else:
+            self._slowmo_c10d(gamma)
+        return True
+
+    def _slowmo_tick(self, optimizer):
+        """count one optimizer step: the base learning rate if a SlowMo step is due now, else None"""
+        if not self.slowmo_frequency:
+            return None
+        calls = self._slowmo_calls + 1
+        if calls % self.slowmo_frequency:
+            self._slowmo_calls = calls
+            return None
+        gamma = float(optimizer.param_groups[0]['lr'])
+        if not gamma > 0:
+            raise ValueError('SlowMo needs a positive base learning rate, got %r' % gamma)
+        self._slowmo_calls = calls
+        return gamma
+
+    def _slowmo_launch(self, gamma):
+        """NVLink plane: enqueue the SlowMo collective on the current stream (no host sync)"""
+        self._kernel.engine.slowmo(self._slowmo_u, self._slowmo_x_prev, gamma, self.slowmo_lr,
+                                   self.slowmo_momentum, init=not self._slowmo_initialized)
+        self._slowmo_initialized = True
+
+    def _slowmo_c10d(self, gamma):
+        """c10d plane: zbar from fp64 all-reduces of sum w z and sum w, the update in fp32 (the
+        same operations on identical inputs on every rank)"""
+        world = self.dist_config['world_size']
+        flat = self.arena.flat
+        with torch.no_grad():
+            if world > 1:
+                dev = self.dist_config['comm_device']
+                grp = self._masters_group
+                w = float(self._w)
+                s = flat.detach().to(dev, torch.float64) * w
+                wsum = torch.tensor([w], dtype=torch.float64, device=dev)
+                dist.all_reduce(s, group=grp)
+                dist.all_reduce(wsum, group=grp)
+                zbar = s.div_(wsum).to(flat.device, torch.float32)
+            else:
+                zbar = flat.detach().clone()
+            u, x_prev = self._slowmo_u, self._slowmo_x_prev
+            if self._slowmo_initialized:
+                u.mul_(self.slowmo_momentum).add_(x_prev.sub(zbar).div_(gamma))
+                x_prev.sub_(u, alpha=self.slowmo_lr * gamma)
+            else:
+                u.zero_()
+                x_prev.copy_(zbar)
+            flat.copy_(x_prev)
+        self._slowmo_initialized = True
+        self.ps_weight = 1.0
 
     # -- consensus: distance and push-sum average model ----------------------- #
     def consensus_distance(self) -> 'ConsensusStats':
@@ -645,9 +762,10 @@ class GossipDataParallel(Module):
                     shadow.copy_(saved_shadow)
 
     def prepare_consensus(self):
-        """Create what the consensus collectives of the NVLink plane need (they do it on first
-        use; collective).  A process that drives several virtual ranks from several threads calls
-        it on every rank before any of them calls :meth:`consensus_distance`: creating a CUDA
+        """Create what the consensus collectives and :meth:`perform_slowmo` need on the NVLink
+        plane (they do it on first use; collective).  A process that drives several virtual ranks
+        from several threads calls it on every rank before any of them calls
+        :meth:`consensus_distance` or :meth:`perform_slowmo`: creating a CUDA
         event or allocating memory can wait for the shared device, where another virtual rank's
         barrier kernel waits for this one (see ``GossipEngine.prepare_consensus``)."""
         if self._kernel is None or self._gossip_done is not None:
@@ -1214,6 +1332,17 @@ def check_gossip_dtype(gossip_dtype, unsupported=None):
         raise ValueError('gossip_dtype=torch.bfloat16 is not supported with %s; bf16 messages '
                          'are implemented for synchronous SGP and D-PSGD' % unsupported)
     return torch.bfloat16
+
+
+def check_slowmo_args(frequency, lr, momentum):
+    """Validate the SlowMo arguments -> (int frequency >= 0, float alpha > 0, float 0 <= beta < 1)."""
+    if isinstance(frequency, bool) or not isinstance(frequency, numbers.Integral) or frequency < 0:
+        raise ValueError('slowmo_frequency must be an int >= 0 (0 = off), got %r' % (frequency,))
+    if not (isinstance(lr, numbers.Real) and math.isfinite(lr) and lr > 0):
+        raise ValueError('slowmo_lr must be a finite number > 0, got %r' % (lr,))
+    if not (isinstance(momentum, numbers.Real) and 0 <= momentum < 1):
+        raise ValueError('slowmo_momentum must be in [0, 1), got %r' % (momentum,))
+    return int(frequency), float(lr), float(momentum)
 
 
 def _native_ok() -> bool:

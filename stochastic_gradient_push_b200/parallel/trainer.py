@@ -48,6 +48,7 @@ class GossipTrainer(object):
         self.gossip = model.dist_config['world_size'] > 1
         self._init_runtime(self.engine.device, criterion, amp_dtype, use_cuda_graph, warmup_iters,
                            channels_last)
+        self._slowmo_on = model.slowmo_frequency > 0      # step() runs the SlowMo step itself
 
     def _init_runtime(self, device, criterion, amp_dtype, use_cuda_graph, warmup_iters, channels_last):
         """state shared by every trainer flavour (gossip / all-reduce / bilateral)"""
@@ -83,6 +84,7 @@ class GossipTrainer(object):
         self._loss_ring = None
         self._loss_slot = 0
         self._skip_next_sgd = False
+        self._slowmo_on = False
         # kernels of OUR extension in one training step (counted over the graph capture, or over
         # the last eager step): what bench.py reports as gpu_launches / step
         self.own_launches_per_step = None
@@ -256,6 +258,10 @@ class GossipTrainer(object):
         if next_batch is not None:
             self.prefetch(next_batch, next_target)
         self._run()
+        if self._slowmo_on:
+            gamma = self.model._slowmo_tick(self.opt)
+            if gamma is not None:
+                self._slowmo(gamma)
         slot = self._loss_slot
         if read_loss:
             with torch.cuda.stream(self.stream):
@@ -333,6 +339,21 @@ class GossipTrainer(object):
         # capture does not execute: undo the host-side step mirror advance
         self.engine.steps = steps_before
         torch.cuda.synchronize(self.device)
+
+    def _slowmo(self, gamma):
+        """The SlowMo step of ``model.slowmo_frequency > 0`` (see ``GossipDataParallel.perform_slowmo``,
+        which users of the trainer do not call): enqueued on the trainer's stream after the step,
+        with no host synchronisation; a heartbeat failure surfaces at the next check() / poll().
+        Overlap-SGP first lands the deferred SGD and the gathered residual as finish() does.  The
+        engine's step counter does not advance, so the captured graphs stay valid."""
+        with torch.cuda.stream(self.stream):
+            if self.overlap and self.gossip and self.model.gossip_enable:
+                self.stream.wait_stream(self.model.gossip_stream)
+                self._set_lr()
+                self.engine.local(sgd=True, fold=True)
+                self.engine.residual.zero_()       # already folded: the next publish adds 0
+                self._skip_next_sgd = True
+            self.model._slowmo_launch(gamma)
 
     def finish(self):
         """Drain: apply the last deferred SGD / residual (overlap), sync, and poll the kernels'

@@ -16,6 +16,7 @@ extern "C" {
 int bn_supported(long long M, int C);
 int bn_partial_rows(long long M, int C);
 int bn_partial_rows_bwd(long long M, int C);
+int bn_f32_map(int value);
 cudaError_t bn_launch_stats(int dtype, const void* x, float* partial, long long M, int C, int G, cudaStream_t st);
 cudaError_t bn_launch_stats_finalize(const float* partial, int G, long long M, int C, const float* gamma,
                                      const float* beta, float* rmean, float* rvar, long long* nbt,
@@ -25,7 +26,7 @@ cudaError_t bn_launch_eval_coeff(int C, const float* gamma, const float* beta, c
                                  const float* rvar, float eps, float* scale, float* shift, cudaStream_t st);
 cudaError_t bn_launch_apply(int dtype, int relu, int add, const void* x, const void* res,
                             const float* scale, const float* shift, void* y, uint8_t* mask, long long M, int C,
-                            cudaStream_t st);
+                            int G, cudaStream_t st);
 cudaError_t bn_launch_bwd_reduce(int dtype, int mode, const void* dy, const void* x, const void* y,
                                  const float* scale, const float* shift, const float* mean,
                                  const float* invstd, float* partial, void* dz, long long M, int C,
@@ -35,7 +36,7 @@ cudaError_t bn_launch_bwd_finalize(const float* partial, int G, long long M, int
                                    float* c2, float* c3, cudaStream_t st);
 cudaError_t bn_launch_bwd_dx(int dtype, int mode, const void* dz, const void* x, const float* scale,
                              const float* shift, const float* c2, const float* c3, void* dx,
-                             long long M, int C, cudaStream_t st);
+                             long long M, int C, int G, cudaStream_t st);
 }
 
 extern std::atomic<long long> g_sgp_kernel_launches;       // bindings.cpp
@@ -124,7 +125,7 @@ static std::vector<torch::Tensor> bn_forward(torch::Tensor x, c10::optional<torc
     }
     BN_CHECK(bn_launch_apply(dt, relu ? 1 : 0, has_res ? 1 : 0, x.data_ptr(),
                              has_res ? residual->data_ptr() : nullptr, scale, shift, y.data_ptr(), nullptr,
-                             M, C, st));
+                             M, C, 0, st));
     return {y, coef};
 }
 
@@ -162,7 +163,7 @@ static std::vector<torch::Tensor> bn_backward(torch::Tensor dy, torch::Tensor x,
     auto dx = torch::empty_like(x);
     BN_CHECK(bn_launch_bwd_dx(dt, mode == 1 ? 1 : 0, mode == 2 ? dz.data_ptr() : dy.data_ptr(),
                               x.data_ptr(), scale, shift, gg + 2 * C, gg + 3 * C, dx.data_ptr(),
-                              M, C, st));
+                              M, C, 0, st));
     return {dx, dz, grads.select(0, 0), grads.select(0, 1)};
 }
 
@@ -187,8 +188,101 @@ static std::vector<torch::Tensor> bn_backward_from_partials(torch::Tensor dz, to
                                     gg, gg + C, gg + 2 * C, gg + 3 * C, st));
     auto dx = torch::empty_like(x);
     BN_CHECK(bn_launch_bwd_dx(dt, 0, dz.data_ptr(), x.data_ptr(), scale, shift, gg + 2 * C, gg + 3 * C,
-                              dx.data_ptr(), M, C, st));
+                              dx.data_ptr(), M, C, 0, st));
     return {dx, grads.select(0, 0), grads.select(0, 1)};
+}
+
+// ---------------------------------------------------------------------------
+// The streaming BN kernels one launch at a time (kernel tests and benchmarks/bn_bandwidth.py).
+// coef is bn_forward's [4, C] (mean, invstd, scale, shift), c23 a [2, C] (c2, c3); G <= 0 is the
+// grid bn_forward / bn_backward launch.
+// ---------------------------------------------------------------------------
+static void bn_kernel_args(const torch::Tensor& x, const torch::Tensor& coef, long long& M, int& C)
+{
+    nhwc_dims(x, M, C);
+    TORCH_CHECK(x.is_cuda() && bn_supported(M, C), "unsupported tensor for the BN kernels");
+    TORCH_CHECK(coef.is_cuda() && coef.scalar_type() == torch::kFloat32 && coef.is_contiguous() &&
+                coef.dim() == 2 && coef.size(1) == C);
+}
+
+static void same_layout(const torch::Tensor& t, const torch::Tensor& x)
+{
+    TORCH_CHECK(t.scalar_type() == x.scalar_type() && t.sizes() == x.sizes() && t.strides() == x.strides(),
+                "operands must match x's dtype, shape and layout");
+}
+
+// partial[G + 1][2][C]: per-CTA shifted sums and the shift row
+static torch::Tensor bn_kernel_stats(torch::Tensor x, int G)
+{
+    long long M; int C;
+    nhwc_dims(x, M, C);
+    TORCH_CHECK(x.is_cuda() && bn_supported(M, C), "unsupported tensor for the BN kernels");
+    c10::cuda::CUDAGuard guard(x.get_device());
+    if (G <= 0) G = bn_partial_rows(M, C);
+    auto partial = torch::empty({G + 1, 2, C}, x.options().dtype(torch::kFloat32));
+    BN_CHECK(bn_launch_stats(dtype_code(x), x.data_ptr(), partial.data_ptr<float>(), M, C, G,
+                             at::cuda::getCurrentCUDAStream()));
+    return partial;
+}
+
+static torch::Tensor bn_kernel_apply(torch::Tensor x, c10::optional<torch::Tensor> residual, torch::Tensor coef,
+                                     bool relu, c10::optional<torch::Tensor> mask, int G)
+{
+    long long M; int C;
+    bn_kernel_args(x, coef, M, C);
+    TORCH_CHECK(coef.size(0) >= 4);
+    const bool has_res = residual.has_value() && residual->defined();
+    const bool has_mask = mask.has_value() && mask->defined();
+    if (has_res) same_layout(*residual, x);
+    if (has_mask) TORCH_CHECK(mask->is_cuda() && mask->scalar_type() == torch::kUInt8 && mask->is_contiguous() &&
+                              mask->numel() == M * (C / 8), "mask must be [M, C/8] uint8");
+    c10::cuda::CUDAGuard guard(x.get_device());
+    auto y = torch::empty_like(x);
+    const float* cf = coef.data_ptr<float>();
+    BN_CHECK(bn_launch_apply(dtype_code(x), relu ? 1 : 0, has_res ? 1 : 0, x.data_ptr(),
+                             has_res ? residual->data_ptr() : nullptr, cf + 2 * C, cf + 3 * C, y.data_ptr(),
+                             has_mask ? mask->data_ptr<uint8_t>() : nullptr, M, C, G,
+                             at::cuda::getCurrentCUDAStream()));
+    return y;
+}
+
+// returns (partial[G][2][C], dz or undefined); mode 2 needs y and writes dz
+static std::vector<torch::Tensor> bn_kernel_reduce(int mode, torch::Tensor dy, torch::Tensor x,
+                                                   c10::optional<torch::Tensor> y, torch::Tensor coef, int G)
+{
+    long long M; int C;
+    bn_kernel_args(x, coef, M, C);
+    TORCH_CHECK(coef.size(0) >= 4 && mode >= 0 && mode <= 2);
+    same_layout(dy, x);
+    if (mode == 2) { TORCH_CHECK(y.has_value() && y->defined()); same_layout(*y, x); }
+    c10::cuda::CUDAGuard guard(x.get_device());
+    if (G <= 0) G = bn_partial_rows_bwd(M, C);
+    auto partial = torch::empty({G, 2, C}, x.options().dtype(torch::kFloat32));
+    torch::Tensor dz;
+    if (mode == 2) dz = torch::empty_like(x);
+    const float* cf = coef.data_ptr<float>();
+    BN_CHECK(bn_launch_bwd_reduce(dtype_code(x), mode, dy.data_ptr(), x.data_ptr(),
+                                  mode == 2 ? y->data_ptr() : nullptr, cf + 2 * C, cf + 3 * C, cf, cf + C,
+                                  partial.data_ptr<float>(), mode == 2 ? dz.data_ptr() : nullptr, M, C, G,
+                                  at::cuda::getCurrentCUDAStream()));
+    return {partial, dz};
+}
+
+static torch::Tensor bn_kernel_dx(int mode, torch::Tensor dz, torch::Tensor x, torch::Tensor coef,
+                                  torch::Tensor c23, int G)
+{
+    long long M; int C;
+    bn_kernel_args(x, coef, M, C);
+    bn_kernel_args(x, c23, M, C);
+    TORCH_CHECK(coef.size(0) >= 4 && c23.size(0) == 2 && (mode == 0 || mode == 1));
+    same_layout(dz, x);
+    c10::cuda::CUDAGuard guard(x.get_device());
+    auto dx = torch::empty_like(x);
+    const float* cf = coef.data_ptr<float>();
+    const float* k = c23.data_ptr<float>();
+    BN_CHECK(bn_launch_bwd_dx(dtype_code(x), mode, dz.data_ptr(), x.data_ptr(), cf + 2 * C, cf + 3 * C, k, k + C,
+                              dx.data_ptr(), M, C, G, at::cuda::getCurrentCUDAStream()));
+    return dx;
 }
 
 // ---------------------------------------------------------------------------
@@ -458,7 +552,7 @@ static std::vector<torch::Tensor> conv1x1_bn_forward(torch::Tensor x, torch::Ten
     auto out = torch::empty_like(yraw);
     BN_CHECK(bn_launch_apply(f32, relu ? 1 : 0, has_res ? 1 : 0, yraw.data_ptr(),
                              has_res ? residual->data_ptr() : nullptr, mean + 2 * N, mean + 3 * N,
-                             out.data_ptr(), has_mask ? mask->data_ptr<uint8_t>() : nullptr, M, N, st));
+                             out.data_ptr(), has_mask ? mask->data_ptr<uint8_t>() : nullptr, M, N, 0, st));
     return {yraw, out, coef};
 }
 
@@ -536,4 +630,14 @@ void bind_bn(py::module& mod)
     mod.def("bn_forward", &bn_forward);
     mod.def("bn_backward", &bn_backward);
     mod.def("bn_backward_from_partials", &bn_backward_from_partials);
+    mod.def("bn_f32_map", &bn_f32_map, py::arg("value") = -1,
+            "fp32 BatchNorm channel map: returns the one in use (1 = split, 0 = consecutive); "
+            "value >= 0 selects one for the launches that follow");
+    mod.def("bn_kernel_stats", &bn_kernel_stats, py::arg("x"), py::arg("G") = 0);
+    mod.def("bn_kernel_apply", &bn_kernel_apply, py::arg("x"), py::arg("residual"), py::arg("coef"),
+            py::arg("relu"), py::arg("mask") = py::none(), py::arg("G") = 0);
+    mod.def("bn_kernel_reduce", &bn_kernel_reduce, py::arg("mode"), py::arg("dy"), py::arg("x"), py::arg("y"),
+            py::arg("coef"), py::arg("G") = 0);
+    mod.def("bn_kernel_dx", &bn_kernel_dx, py::arg("mode"), py::arg("dz"), py::arg("x"), py::arg("coef"),
+            py::arg("c23"), py::arg("G") = 0);
 }

@@ -11,12 +11,17 @@
 //              and dz is written once because it IS the residual branch's grad.
 //
 // Layout: x is [M, C] row-major (M = N*H*W, NHWC), C % 8 == 0, C <= 2048.
-// One thread owns 8 consecutive channels (16 B of bf16 / 32 B of fp32) and
-// strides over rows, so per-channel constants live in registers and every
-// global access is a full 16-byte vector.
+// One thread owns 8 channels and strides over rows, so per-channel constants
+// live in registers and every global access is a full 16-byte vector.  bf16:
+// 8 consecutive channels, one vector.  fp32 (SPLIT map): channels [4cv, 4cv+4)
+// and [C/2+4cv, C/2+4cv+4), two vectors that each continue the neighbouring
+// lane's, so every warp access covers whole 128-byte lines (8 consecutive fp32
+// channels would be 32 B per lane: each access would use half of every sector
+// and the second one would fetch the same sectors from L2 again).
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <stdint.h>
+#include <stdlib.h>
 
 #include "vec_io.cuh"
 
@@ -34,25 +39,32 @@ template <typename T> struct Unroll {
 
 namespace {
 
-// thread -> (channel vector, row lane) mapping shared by all kernels
+// thread -> (channels, row lane) mapping shared by all kernels.  SPLIT: the fp32 map above
+// (element i < 4 is channel off + i, element i >= 4 is channel off + h + i - 4).
+template <bool SPLIT>
 struct Map {
     int tpr;        // threads per row  = C / 8
     int rpi;        // rows per CTA iteration = 256 / tpr
     int cv;         // this thread's channel-vector index
     int rl;         // this thread's row lane
+    int off;        // first channel of the thread's first half
+    int h;          // channel distance from the first half to the second (4: consecutive)
     bool active;
     __device__ __forceinline__ Map(int C) {
         tpr = C / BN_VEC;
         rpi = BN_THREADS / tpr;
         cv = threadIdx.x % tpr;
         rl = threadIdx.x / tpr;
+        off = SPLIT ? cv * 4 : cv * BN_VEC;
+        h = SPLIT ? C / 2 : 4;
         active = rl < rpi;
     }
 };
 
 // block reduce of 2 x 8 per-thread accumulators across the row lanes that share
 // a channel vector, then one partial row per CTA: partial[blockIdx][2][C]
-__device__ __forceinline__ void reduce_store_partials(const Map& mp, const F8& a, const F8& b,
+template <bool SPLIT>
+__device__ __forceinline__ void reduce_store_partials(const Map<SPLIT>& mp, const F8& a, const F8& b,
                                                       float* __restrict__ partial, int C)
 {
     __shared__ float sm[BN_THREADS * 16];
@@ -69,9 +81,14 @@ __device__ __forceinline__ void reduce_store_partials(const Map& mp, const F8& a
 #pragma unroll
             for (int i = 0; i < 16; ++i) acc[i] += o[i];
         }
-        float* out = partial + (size_t)blockIdx.x * 2 * C + threadIdx.x * BN_VEC;
+        // thread threadIdx.x stands for channel vector cv = threadIdx.x (row lane 0)
+        const unsigned off = SPLIT ? threadIdx.x * 4 : threadIdx.x * BN_VEC;
+        float* out = partial + (size_t)blockIdx.x * 2 * C + off;
 #pragma unroll
-        for (int i = 0; i < 8; ++i) { out[i] = acc[i]; out[C + i] = acc[8 + i]; }
+        for (int i = 0; i < 8; ++i) {
+            const int j = i < 4 ? i : mp.h + i - 4;
+            out[j] = acc[i]; out[C + j] = acc[8 + i];
+        }
     }
 }
 
@@ -80,31 +97,31 @@ __device__ __forceinline__ void reduce_store_partials(const Map& mp, const F8& a
 // ---------------------------------------------------------------------------
 // forward: statistics
 // ---------------------------------------------------------------------------
-template <typename T>
+template <typename T, bool SPLIT = false>
 __global__ void __launch_bounds__(BN_THREADS, 4)
 bn_stats_kernel(const T* __restrict__ x, float* __restrict__ partial, long long M, int C)
 {
-    const Map mp(C);
+    const Map<SPLIT> mp(C);
     F8 s, q;
 #pragma unroll
     for (int i = 0; i < 8; ++i) { s.v[i] = 0.f; q.v[i] = 0.f; }
     if (mp.active) {
         const long long stride = (long long)gridDim.x * mp.rpi;
         long long r = (long long)blockIdx.x * mp.rpi + mp.rl;
-        const T* base = x + mp.cv * BN_VEC;
+        const T* base = x + mp.off;
         // shifted sums: accumulate (x - K) with K = x[row 0] so that
         // var = E[(x-K)^2] - E[x-K]^2 does not cancel when |mean| >> std
-        const F8 k = Io<T>::load(base);
+        const F8 k = Io<T>::load(base, mp.h);
         if (blockIdx.x == 0 && mp.rl == 0) {
-            float* krow = partial + (size_t)gridDim.x * 2 * C + mp.cv * BN_VEC;
+            float* krow = partial + (size_t)gridDim.x * 2 * C + mp.off;
 #pragma unroll
-            for (int i = 0; i < 8; ++i) krow[i] = k.v[i];
+            for (int i = 0; i < 8; ++i) krow[i < 4 ? i : mp.h + i - 4] = k.v[i];
         }
         constexpr int UN = Unroll<T>::N;
         for (; r + (UN - 1) * stride < M; r += UN * stride) {
             typename Io<T>::raw_t raw[UN];
 #pragma unroll
-            for (int u = 0; u < UN; ++u) raw[u] = Io<T>::load_raw(base + (r + u * stride) * C);
+            for (int u = 0; u < UN; ++u) raw[u] = Io<T>::load_raw(base + (r + u * stride) * C, mp.h);
 #pragma unroll
             for (int u = 0; u < UN; ++u) {
                 const F8 d = Io<T>::decode(raw[u]);
@@ -116,7 +133,7 @@ bn_stats_kernel(const T* __restrict__ x, float* __restrict__ partial, long long 
             }
         }
         for (; r < M; r += stride) {
-            const F8 d = Io<T>::load(base + r * C);
+            const F8 d = Io<T>::load(base + r * C, mp.h);
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
                 const float c = d.v[i] - k.v[i];
@@ -223,19 +240,21 @@ __global__ void bn_eval_coeff_kernel(int C, const float* __restrict__ gamma, con
 // ---------------------------------------------------------------------------
 // forward: apply   y = act(x*scale + shift [+ res])
 // MASK: also mask[M, C/8], bit i of byte j = (y[row, 8j+i] > 0) -- the ReLU mask of a residual block's
-// output for the next block's conv1 dgrad (MODE 3 of conv1x1_kernels.cu), 1/32 of y's fp32 bytes
+// output for the next block's conv1 dgrad (MODE 3 of conv1x1_kernels.cu), 1/32 of y's fp32 bytes.
+// With the SPLIT map a byte's 8 channels belong to two neighbouring lanes (C % 16 == 0): the even
+// lane of a pair stores the byte of their first halves, the odd lane the byte of their second halves.
 // ---------------------------------------------------------------------------
-template <typename T, bool RELU, bool ADD, bool MASK = false>
+template <typename T, bool RELU, bool ADD, bool MASK = false, bool SPLIT = false>
 __global__ void __launch_bounds__(BN_THREADS, (sizeof(T) == 4 && ADD) ? 3 : 4)     // fp32 + residual: 80 registers
 bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, const float* __restrict__ scale,
                 const float* __restrict__ shift, T* __restrict__ y, uint8_t* __restrict__ mask, long long M, int C)
 {
-    const Map mp(C);
+    const Map<SPLIT> mp(C);
     if (!mp.active) return;
-    const F8 sc = load_c8(scale + mp.cv * BN_VEC);
-    const F8 sh = load_c8(shift + mp.cv * BN_VEC);
+    const F8 sc = load_c8(scale + mp.off, mp.h);
+    const F8 sh = load_c8(shift + mp.off, mp.h);
     const long long stride = (long long)gridDim.x * mp.rpi;
-    const long long off = mp.cv * BN_VEC;
+    const long long off = mp.off;
     constexpr int UN = Unroll<T>::N;
     for (long long r = (long long)blockIdx.x * mp.rpi + mp.rl; r < M; r += UN * stride) {
         typename Io<T>::raw_t dr[UN], ar[UN];
@@ -243,8 +262,8 @@ bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, const float*
         for (int u = 0; u < UN; ++u) {
             const long long rr = r + u * stride;
             if (rr < M) {
-                dr[u] = Io<T>::load_raw(x + rr * C + off);
-                if (ADD) ar[u] = Io<T>::load_raw(res + rr * C + off);
+                dr[u] = Io<T>::load_raw(x + rr * C + off, mp.h);
+                if (ADD) ar[u] = Io<T>::load_raw(res + rr * C + off, mp.h);
             }
         }
 #pragma unroll
@@ -267,8 +286,14 @@ bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, const float*
                         bits |= (vs > 0.f ? 1u : 0u) << i;
                     }
                 }
-                Io<T>::store(y + rr * C + off, o);
-                if (MASK) mask[rr * (C / BN_VEC) + mp.cv] = (uint8_t)bits;
+                Io<T>::store(y + rr * C + off, o, mp.h);
+                if (MASK && !SPLIT) mask[rr * (C / BN_VEC) + mp.cv] = (uint8_t)bits;
+                if (MASK && SPLIT) {      // both lanes of a pair are on this row
+                    const uint32_t pb = __shfl_xor_sync(3u << (threadIdx.x & 30), bits, 1);
+                    const bool odd = mp.cv & 1;
+                    const uint32_t byte = odd ? (pb >> 4) | (bits & 0xf0u) : (bits & 0x0fu) | (pb << 4);
+                    mask[rr * (C / BN_VEC) + (odd ? C / 16 : 0) + (mp.cv >> 1)] = (uint8_t)byte;
+                }
             }
         }
     }
@@ -279,23 +304,23 @@ bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, const float*
 // MODE 0: dz = dy            MODE 1: dz = dy * (x*scale+shift > 0)
 // MODE 2: dz = dy * (y > 0), dz is also written (gradient of the residual branch)
 // ---------------------------------------------------------------------------
-template <typename T, int MODE>
+template <typename T, int MODE, bool SPLIT = false>
 __global__ void __launch_bounds__(BN_THREADS, 3)
 bn_bwd_reduce_kernel(const T* __restrict__ dy, const T* __restrict__ x, const T* __restrict__ y,
                      const float* __restrict__ scale, const float* __restrict__ shift,
                      const float* __restrict__ mean, const float* __restrict__ invstd,
                      float* __restrict__ partial, T* __restrict__ dz_out, long long M, int C)
 {
-    const Map mp(C);
+    const Map<SPLIT> mp(C);
     F8 s, q;
 #pragma unroll
     for (int i = 0; i < 8; ++i) { s.v[i] = 0.f; q.v[i] = 0.f; }
     if (mp.active) {
-        const long long off = mp.cv * BN_VEC;
-        const F8 mu = load_c8(mean + off);
-        const F8 is = load_c8(invstd + off);
+        const long long off = mp.off;
+        const F8 mu = load_c8(mean + off, mp.h);
+        const F8 is = load_c8(invstd + off, mp.h);
         F8 sc, sh;
-        if (MODE == 1) { sc = load_c8(scale + off); sh = load_c8(shift + off); }
+        if (MODE == 1) { sc = load_c8(scale + off, mp.h); sh = load_c8(shift + off, mp.h); }
         const long long stride = (long long)gridDim.x * mp.rpi;
         constexpr int UN = Unroll<T>::RED;
         for (long long r = (long long)blockIdx.x * mp.rpi + mp.rl; r < M; r += UN * stride) {
@@ -304,9 +329,9 @@ bn_bwd_reduce_kernel(const T* __restrict__ dy, const T* __restrict__ x, const T*
             for (int u = 0; u < UN; ++u) {
                 const long long rr = r + u * stride;
                 if (rr < M) {
-                    gr[u] = Io<T>::load_raw(dy + rr * C + off);
-                    xr[u] = Io<T>::load_raw(x + rr * C + off);
-                    if (MODE == 2) yr[u] = Io<T>::load_raw(y + rr * C + off);
+                    gr[u] = Io<T>::load_raw(dy + rr * C + off, mp.h);
+                    xr[u] = Io<T>::load_raw(x + rr * C + off, mp.h);
+                    if (MODE == 2) yr[u] = Io<T>::load_raw(y + rr * C + off, mp.h);
                 }
             }
 #pragma unroll
@@ -327,7 +352,7 @@ bn_bwd_reduce_kernel(const T* __restrict__ dy, const T* __restrict__ x, const T*
                         s.v[i] += gz;
                         q.v[i] = fmaf(gz, (d.v[i] - mu.v[i]) * is.v[i], q.v[i]);
                     }
-                    if (MODE == 2) Io<T>::store(dz_out + rr * C + off, dz);
+                    if (MODE == 2) Io<T>::store(dz_out + rr * C + off, dz, mp.h);
                 }
             }
         }
@@ -359,20 +384,28 @@ bn_bwd_finalize_kernel(const float* __restrict__ partial, int G, long long M, in
 
 // MODE 0/2: dz given directly (dy, or the dz written by the reduce kernel)
 // MODE 1  : dz = dy * (x*scale+shift > 0) recomputed
-template <typename T, int MODE>
+template <typename T, int MODE, bool SPLIT = false>
 __global__ void __launch_bounds__(BN_THREADS, 3)
 bn_bwd_dx_kernel(const T* __restrict__ dz_in, const T* __restrict__ x, const float* __restrict__ scale,
                  const float* __restrict__ shift, const float* __restrict__ c2,
                  const float* __restrict__ c3, T* __restrict__ dx, long long M, int C)
 {
-    const Map mp(C);
+    // fp32 MODE 1 reads the shift from shared memory at each row: 4 x 8 constants in registers
+    // next to 2 x 2 x 8 loads in flight do not fit its 80-register cap (they spilled)
+    constexpr bool SH_SMEM = MODE == 1 && sizeof(T) == 4;
+    __shared__ float sh_s[SH_SMEM ? 2048 : 1];
+    if (SH_SMEM) {
+        for (int c = threadIdx.x; c < C; c += BN_THREADS) sh_s[c] = shift[c];
+        __syncthreads();
+    }
+    const Map<SPLIT> mp(C);
     if (!mp.active) return;
-    const long long off = mp.cv * BN_VEC;
-    const F8 k1 = load_c8(scale + off);
-    const F8 k2 = load_c8(c2 + off);
-    const F8 k3 = load_c8(c3 + off);
+    const long long off = mp.off;
+    const F8 k1 = load_c8(scale + off, mp.h);
+    const F8 k2 = load_c8(c2 + off, mp.h);
+    const F8 k3 = load_c8(c3 + off, mp.h);
     F8 sh;
-    if (MODE == 1) sh = load_c8(shift + off);
+    if (MODE == 1 && !SH_SMEM) sh = load_c8(shift + off, mp.h);
     const long long stride = (long long)gridDim.x * mp.rpi;
     constexpr int UN = Unroll<T>::N;
     for (long long r = (long long)blockIdx.x * mp.rpi + mp.rl; r < M; r += UN * stride) {
@@ -381,8 +414,8 @@ bn_bwd_dx_kernel(const T* __restrict__ dz_in, const T* __restrict__ x, const flo
         for (int u = 0; u < UN; ++u) {
             const long long rr = r + u * stride;
             if (rr < M) {
-                gr[u] = Io<T>::load_raw(dz_in + rr * C + off);
-                xr[u] = Io<T>::load_raw(x + rr * C + off);
+                gr[u] = Io<T>::load_raw(dz_in + rr * C + off, mp.h);
+                xr[u] = Io<T>::load_raw(x + rr * C + off, mp.h);
             }
         }
 #pragma unroll
@@ -391,6 +424,7 @@ bn_bwd_dx_kernel(const T* __restrict__ dz_in, const T* __restrict__ x, const flo
             if (rr < M) {
                 const F8 g = Io<T>::decode(gr[u]);
                 const F8 d = Io<T>::decode(xr[u]);
+                if (SH_SMEM) sh = load_c8(sh_s + off, mp.h);
                 F8 o;
 #pragma unroll
                 for (int i = 0; i < 8; ++i) {
@@ -398,7 +432,7 @@ bn_bwd_dx_kernel(const T* __restrict__ dz_in, const T* __restrict__ x, const flo
                     if (MODE == 1) gz = (fmaf(d.v[i], k1.v[i], sh.v[i]) > 0.f) ? gz : 0.f;
                     o.v[i] = fmaf(k1.v[i], gz, fmaf(-k2.v[i], d.v[i], k3.v[i]));
                 }
-                Io<T>::store(dx + rr * C + off, o);
+                Io<T>::store(dx + rr * C + off, o, mp.h);
             }
         }
     }
@@ -407,19 +441,40 @@ bn_bwd_dx_kernel(const T* __restrict__ dz_in, const T* __restrict__ x, const flo
 // ---------------------------------------------------------------------------
 // launchers (C linkage; dtype: 0 = bf16, 1 = fp32)
 // ---------------------------------------------------------------------------
-static inline int bn_grid(long long M, int C, int per_sm)
+static inline int bn_grid(long long M, int C, int per_sm, int unroll = BN_UNROLL)
 {
     const int tpr = C / BN_VEC;
     const int rpi = BN_THREADS / tpr;
     long long iters = (M + rpi - 1) / rpi;
-    long long g = (iters + BN_UNROLL - 1) / BN_UNROLL;
+    long long g = (iters + unroll - 1) / unroll;
     const long long cap = 132LL * per_sm;
     if (g > cap) g = cap;
     if (g < 1) g = 1;
     return (int)g;
 }
 
+// fp32 channel map: 1 = SPLIT (default), 0 = the consecutive map of the bf16 kernels with the launch
+// sizing it had.  SGP_B200_BN_F32_MAP=0 selects 0 at start-up; bn_f32_map() switches at run time.
+static int g_bn_f32_map = -1;
+
+static bool f32_split()
+{
+    if (g_bn_f32_map < 0) {
+        const char* e = getenv("SGP_B200_BN_F32_MAP");
+        g_bn_f32_map = (e != nullptr && e[0] == '0') ? 0 : 1;
+    }
+    return g_bn_f32_map == 1;
+}
+
 extern "C" {
+
+// returns the map in use; value >= 0 selects a map for the launches that follow
+int bn_f32_map(int value)
+{
+    const int cur = f32_split() ? 1 : 0;
+    if (value >= 0) g_bn_f32_map = value ? 1 : 0;
+    return cur;
+}
 
 int bn_supported(long long M, int C) { return (C % BN_VEC == 0) && (C / BN_VEC <= BN_THREADS) && M > 0; }
 
@@ -433,6 +488,7 @@ cudaError_t bn_launch_stats(int dtype, const void* x, float* partial, long long 
                             cudaStream_t st)
 {
     if (dtype == 0) bn_stats_kernel<__nv_bfloat16><<<G, BN_THREADS, 0, st>>>((const __nv_bfloat16*)x, partial, M, C);
+    else if (f32_split()) bn_stats_kernel<float, true><<<G, BN_THREADS, 0, st>>>((const float*)x, partial, M, C);
     else            bn_stats_kernel<float><<<G, BN_THREADS, 0, st>>>((const float*)x, partial, M, C);
     return cudaGetLastError();
 }
@@ -454,38 +510,47 @@ cudaError_t bn_launch_eval_coeff(int C, const float* gamma, const float* beta, c
     return cudaGetLastError();
 }
 
-#define BN_APPLY(T, R, A) bn_apply_kernel<T, R, A><<<G, BN_THREADS, 0, st>>>( \
+#define BN_APPLY(T, R, A, S) bn_apply_kernel<T, R, A, false, S><<<G, BN_THREADS, 0, st>>>( \
     (const T*)x, (const T*)res, scale, shift, (T*)y, nullptr, M, C)
 
-// mask (nullable; relu && add only): the 1-bit ReLU mask [M, C/8] of y
+// mask (nullable; relu && add only): the 1-bit ReLU mask [M, C/8] of y (fp32 split map: C % 16 == 0).
+// G <= 0: the default grid
 cudaError_t bn_launch_apply(int dtype, int relu, int add, const void* x, const void* res,
                             const float* scale, const float* shift, void* y, uint8_t* mask, long long M, int C,
-                            cudaStream_t st)
+                            int G, cudaStream_t st)
 {
-    const int G = bn_grid(M, C, (dtype == 1 && add) ? 6 : 8);   // fp32 + residual holds 3 CTAs/SM: 2 waves
+    const bool split = dtype == 1 && f32_split();
+    if (G <= 0) G = bn_grid(M, C, (dtype == 1 && add) ? 6 : 8);   // fp32 + residual holds 3 CTAs/SM: 2 waves
     if (mask != nullptr) {
-        if (!(relu && add)) return cudaErrorInvalidValue;
+        if (!(relu && add) || (split && C % 16 != 0)) return cudaErrorInvalidValue;
         if (dtype == 0) bn_apply_kernel<__nv_bfloat16, true, true, true><<<G, BN_THREADS, 0, st>>>(
             (const __nv_bfloat16*)x, (const __nv_bfloat16*)res, scale, shift, (__nv_bfloat16*)y, mask, M, C);
+        else if (split) bn_apply_kernel<float, true, true, true, true><<<G, BN_THREADS, 0, st>>>(
+            (const float*)x, (const float*)res, scale, shift, (float*)y, mask, M, C);
         else bn_apply_kernel<float, true, true, true><<<G, BN_THREADS, 0, st>>>(
             (const float*)x, (const float*)res, scale, shift, (float*)y, mask, M, C);
         return cudaGetLastError();
     }
     if (dtype == 0) {
-        if (relu && add) BN_APPLY(__nv_bfloat16, true, true);
-        else if (relu)   BN_APPLY(__nv_bfloat16, true, false);
-        else if (add)    BN_APPLY(__nv_bfloat16, false, true);
-        else             BN_APPLY(__nv_bfloat16, false, false);
+        if (relu && add) BN_APPLY(__nv_bfloat16, true, true, false);
+        else if (relu)   BN_APPLY(__nv_bfloat16, true, false, false);
+        else if (add)    BN_APPLY(__nv_bfloat16, false, true, false);
+        else             BN_APPLY(__nv_bfloat16, false, false, false);
+    } else if (split) {
+        if (relu && add) BN_APPLY(float, true, true, true);
+        else if (relu)   BN_APPLY(float, true, false, true);
+        else if (add)    BN_APPLY(float, false, true, true);
+        else             BN_APPLY(float, false, false, true);
     } else {
-        if (relu && add) BN_APPLY(float, true, true);
-        else if (relu)   BN_APPLY(float, true, false);
-        else if (add)    BN_APPLY(float, false, true);
-        else             BN_APPLY(float, false, false);
+        if (relu && add) BN_APPLY(float, true, true, false);
+        else if (relu)   BN_APPLY(float, true, false, false);
+        else if (add)    BN_APPLY(float, false, true, false);
+        else             BN_APPLY(float, false, false, false);
     }
     return cudaGetLastError();
 }
 
-#define BN_RED(T, MODE) bn_bwd_reduce_kernel<T, MODE><<<G, BN_THREADS, 0, st>>>( \
+#define BN_RED(T, MODE, S) bn_bwd_reduce_kernel<T, MODE, S><<<G, BN_THREADS, 0, st>>>( \
     (const T*)dy, (const T*)x, (const T*)y, scale, shift, mean, invstd, partial, (T*)dz, M, C)
 
 cudaError_t bn_launch_bwd_reduce(int dtype, int mode, const void* dy, const void* x, const void* y,
@@ -494,9 +559,12 @@ cudaError_t bn_launch_bwd_reduce(int dtype, int mode, const void* dy, const void
                                  int G, cudaStream_t st)
 {
     if (dtype == 0) {
-        if (mode == 0) BN_RED(__nv_bfloat16, 0); else if (mode == 1) BN_RED(__nv_bfloat16, 1); else BN_RED(__nv_bfloat16, 2);
+        if (mode == 0) BN_RED(__nv_bfloat16, 0, false); else if (mode == 1) BN_RED(__nv_bfloat16, 1, false);
+        else BN_RED(__nv_bfloat16, 2, false);
+    } else if (f32_split()) {
+        if (mode == 0) BN_RED(float, 0, true); else if (mode == 1) BN_RED(float, 1, true); else BN_RED(float, 2, true);
     } else {
-        if (mode == 0) BN_RED(float, 0); else if (mode == 1) BN_RED(float, 1); else BN_RED(float, 2);
+        if (mode == 0) BN_RED(float, 0, false); else if (mode == 1) BN_RED(float, 1, false); else BN_RED(float, 2, false);
     }
     return cudaGetLastError();
 }
@@ -510,16 +578,18 @@ cudaError_t bn_launch_bwd_finalize(const float* partial, int G, long long M, int
     return cudaGetLastError();
 }
 
-#define BN_DX(T, MODE) bn_bwd_dx_kernel<T, MODE><<<G, BN_THREADS, 0, st>>>( \
+#define BN_DX(T, MODE, S) bn_bwd_dx_kernel<T, MODE, S><<<G, BN_THREADS, 0, st>>>( \
     (const T*)dz, (const T*)x, scale, shift, c2, c3, (T*)dx, M, C)
 
+// G <= 0: the default grid
 cudaError_t bn_launch_bwd_dx(int dtype, int mode, const void* dz, const void* x, const float* scale,
                              const float* shift, const float* c2, const float* c3, void* dx,
-                             long long M, int C, cudaStream_t st)
+                             long long M, int C, int G, cudaStream_t st)
 {
-    const int G = bn_grid(M, C, 6);      // 3 CTAs/SM resident -> exactly 2 waves
-    if (dtype == 0) { if (mode == 1) BN_DX(__nv_bfloat16, 1); else BN_DX(__nv_bfloat16, 0); }
-    else            { if (mode == 1) BN_DX(float, 1); else BN_DX(float, 0); }
+    if (G <= 0) G = bn_grid(M, C, 6);      // 3 CTAs/SM resident -> exactly 2 waves
+    if (dtype == 0)       { if (mode == 1) BN_DX(__nv_bfloat16, 1, false); else BN_DX(__nv_bfloat16, 0, false); }
+    else if (f32_split()) { if (mode == 1) BN_DX(float, 1, true); else BN_DX(float, 0, true); }
+    else                  { if (mode == 1) BN_DX(float, 1, false); else BN_DX(float, 0, false); }
     return cudaGetLastError();
 }
 

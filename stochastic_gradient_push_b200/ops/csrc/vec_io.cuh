@@ -1,6 +1,8 @@
 // 16-byte vector I/O helpers shared by the NHWC activation kernels (BatchNorm,
-// max-pool): one thread owns 8 consecutive channels; bf16 loads stay packed in
-// 4 registers until they are decoded.
+// max-pool): one thread owns 8 channels; bf16 loads stay packed in 4 registers
+// until they are decoded.  An fp32 thread's 8 channels are two 16-byte halves
+// h floats apart: h = 4 is 8 consecutive channels, the BatchNorm kernels' split
+// map passes h = C/2 so that each half of a warp's accesses is contiguous.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -14,13 +16,13 @@ template <typename T> struct Io;
 
 template <> struct Io<__nv_bfloat16> {
     typedef uint4 raw_t;      // loads stay packed (4 regs) until they are consumed
-    static __device__ __forceinline__ raw_t load_raw(const __nv_bfloat16* p) {
+    static __device__ __forceinline__ raw_t load_raw(const __nv_bfloat16* p, int = 4) {
         uint4 r;
         asm volatile("ld.global.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
                      : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
         return r;
     }
-    static __device__ __forceinline__ F8 load(const __nv_bfloat16* p) { return decode(load_raw(p)); }
+    static __device__ __forceinline__ F8 load(const __nv_bfloat16* p, int = 4) { return decode(load_raw(p)); }
     // read-only path WITH L1 allocation: for data that neighbouring threads re-read
     // (pooling windows overlap); the streaming loads above bypass L1 on purpose
     static __device__ __forceinline__ F8 load_cached(const __nv_bfloat16* p) {
@@ -36,7 +38,7 @@ template <> struct Io<__nv_bfloat16> {
         }
         return o;
     }
-    static __device__ __forceinline__ void store(__nv_bfloat16* p, const F8& f) {
+    static __device__ __forceinline__ void store(__nv_bfloat16* p, const F8& f, int = 4) {
         uint32_t w[4];
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
@@ -50,7 +52,7 @@ template <> struct Io<__nv_bfloat16> {
 
 template <> struct Io<float> {
     typedef F8 raw_t;
-    static __device__ __forceinline__ raw_t load_raw(const float* p) { return load(p); }
+    static __device__ __forceinline__ raw_t load_raw(const float* p, int h = 4) { return load(p, h); }
     static __device__ __forceinline__ F8 load_cached(const float* p) {
         F8 o;
         const float4 a = __ldg(reinterpret_cast<const float4*>(p));
@@ -60,26 +62,26 @@ template <> struct Io<float> {
         return o;
     }
     static __device__ __forceinline__ F8 decode(const raw_t& r) { return r; }
-    static __device__ __forceinline__ F8 load(const float* p) {
+    static __device__ __forceinline__ F8 load(const float* p, int h = 4) {
         F8 o;
         asm volatile("ld.global.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];"
                      : "=f"(o.v[0]), "=f"(o.v[1]), "=f"(o.v[2]), "=f"(o.v[3]) : "l"(p));
         asm volatile("ld.global.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];"
-                     : "=f"(o.v[4]), "=f"(o.v[5]), "=f"(o.v[6]), "=f"(o.v[7]) : "l"(p + 4));
+                     : "=f"(o.v[4]), "=f"(o.v[5]), "=f"(o.v[6]), "=f"(o.v[7]) : "l"(p + h));
         return o;
     }
-    static __device__ __forceinline__ void store(float* p, const F8& f) {
+    static __device__ __forceinline__ void store(float* p, const F8& f, int h = 4) {
         asm volatile("st.global.v4.f32 [%0], {%1,%2,%3,%4};"
                      :: "l"(p), "f"(f.v[0]), "f"(f.v[1]), "f"(f.v[2]), "f"(f.v[3]) : "memory");
         asm volatile("st.global.v4.f32 [%0], {%1,%2,%3,%4};"
-                     :: "l"(p + 4), "f"(f.v[4]), "f"(f.v[5]), "f"(f.v[6]), "f"(f.v[7]) : "memory");
+                     :: "l"(p + h), "f"(f.v[4]), "f"(f.v[5]), "f"(f.v[6]), "f"(f.v[7]) : "memory");
     }
 };
 
-__device__ __forceinline__ F8 load_c8(const float* p) {   // per-channel constants
+__device__ __forceinline__ F8 load_c8(const float* p, int h = 4) {   // per-channel constants
     F8 o;
     const float4 a = *reinterpret_cast<const float4*>(p);
-    const float4 b = *reinterpret_cast<const float4*>(p + 4);
+    const float4 b = *reinterpret_cast<const float4*>(p + h);
     o.v[0] = a.x; o.v[1] = a.y; o.v[2] = a.z; o.v[3] = a.w;
     o.v[4] = b.x; o.v[5] = b.y; o.v[6] = b.z; o.v[7] = b.w;
     return o;

@@ -28,6 +28,7 @@ the tensor-core stem convolution wrappers.
 
 from __future__ import annotations
 
+import contextlib
 import os
 
 import torch
@@ -51,6 +52,20 @@ USE_STEM_KERNELS = os.environ.get('SGP_B200_STEM', '1') != '0'
 # A residual block's last BN backward reduction runs inside the next block's conv1 dgrad GEMM
 # (MODE 3 of csrc/conv1x1_kernels.cu); SGP_B200_BN_BWD_FUSE=0 keeps the stand-alone reduce pass.
 USE_BN_BWD_FUSE = os.environ.get('SGP_B200_BN_BWD_FUSE', '1') != '0'
+
+
+@contextlib.contextmanager
+def bn_f32_map(split: bool):
+    """Run the fp32 BatchNorm kernels launched inside the block with the split channel map (the
+    default; coalesced 16-byte accesses) or, ``split=False``, with 8 consecutive channels per thread
+    (the bf16 map; ``SGP_B200_BN_F32_MAP=0`` selects it for the whole process).  Both give
+    bit-identical results."""
+    C = native.load()
+    prev = C.bn_f32_map(1 if split else 0)
+    try:
+        yield
+    finally:
+        C.bn_f32_map(prev)
 
 
 def _can_fuse(x: torch.Tensor) -> bool:

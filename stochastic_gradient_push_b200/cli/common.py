@@ -56,6 +56,10 @@ def build_parser(adpsgd: bool = False) -> argparse.ArgumentParser:
     p.add_argument('--momentum', default=0.9, type=float)
     p.add_argument('--weight_decay', default=1e-4, type=float)
     p.add_argument('--nesterov', default=False, **B)
+    p.add_argument('--no_bias_decay', default=False, **B,
+                   help='no weight decay on parameters with ndim <= 1 (BatchNorm weight and bias, all '
+                        'biases): two parameter groups (optim.no_bias_decay_groups), for --fused True '
+                        'and False alike.  SGP / OSGP / D-PSGD')
     p.add_argument('--push_sum', default=True, **B, help='push-sum (SGP) or push-pull (D-PSGD)')
     p.add_argument('--graph_type', default=5, type=int, choices=list(GRAPH_TOPOLOGIES))
     p.add_argument('--mixing_strategy', default=0, type=int, choices=list(MIXING_STRATEGIES))
@@ -217,6 +221,11 @@ def finalize_args(args, adpsgd=False):
                              'measure gossip (SGP, OSGP, D-PSGD)' % unsupported)
         if args.consensus_freq < 0:
             raise ValueError('--consensus_freq must be >= 0')
+    if getattr(args, 'no_bias_decay', False):
+        unsupported = 'AD-PSGD' if adpsgd else '--all_reduce' if args.all_reduce else None
+        if unsupported:
+            raise ValueError('--no_bias_decay is not supported with %s: parameter groups are '
+                             'implemented for SGP, OSGP and D-PSGD' % unsupported)
     if getattr(args, 'slowmo_frequency', 0):
         unsupported = ('AD-PSGD' if adpsgd else '--all_reduce' if args.all_reduce else
                        '--nprocs_per_node > 1' if getattr(args, 'nprocs_per_node', 1) > 1 else None)

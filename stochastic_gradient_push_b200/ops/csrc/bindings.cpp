@@ -234,6 +234,42 @@ public:
 
     int max_grid() const { return max_grid_; }
 
+    // per-parameter-group SGD (SGP_F_GROUPS on every SGD launch of step()): `block_group` uint8
+    // [n / 64], the group of each 64-float block; `hyper_groups` fp32 [groups, HYPER_FLOATS] device
+    // rows, read by the kernels at every launch.  None / None: back to the single hyper row
+    void set_param_groups(c10::optional<torch::Tensor> block_group, c10::optional<torch::Tensor> hyper_groups)
+    {
+        const bool on = block_group.has_value() && block_group->defined();
+        TORCH_CHECK(on == (hyper_groups.has_value() && hyper_groups->defined()),
+                    "set_param_groups takes both the block map and the group rows, or neither");
+        if (!on) {
+            args_.block_group = nullptr;
+            args_.hyper_groups = nullptr;
+            args_.groups = 0;
+            groups_keep_ = {};
+            return;
+        }
+        const torch::Tensor& bg = *block_group;
+        const torch::Tensor& hg = *hyper_groups;
+        TORCH_CHECK(bg.is_cuda() && bg.get_device() == device_ && bg.scalar_type() == torch::kUInt8 &&
+                    bg.is_contiguous() && bg.numel() == args_.n / SGP_GROUP_BLOCK,
+                    "block_group must be a contiguous uint8 tensor of ", args_.n / SGP_GROUP_BLOCK,
+                    " entries on the arena's device");
+        TORCH_CHECK(hg.is_cuda() && hg.get_device() == device_ && hg.scalar_type() == torch::kFloat32 &&
+                    hg.is_contiguous() && hg.dim() == 2 &&
+                    hg.size(1) == (int64_t)(sizeof(SgpHyper) / sizeof(float)),
+                    "hyper_groups must be a contiguous fp32 [groups, HYPER_FLOATS] tensor on the arena's device");
+        TORCH_CHECK(hg.size(0) >= 1 && hg.size(0) <= SGP_MAX_GROUPS, "1 to ", SGP_MAX_GROUPS, " groups");
+        const int groups = (int)hg.size(0);
+        // a block map entry >= groups would index past the shared-memory table
+        TORCH_CHECK(bg.max().item<uint8_t>() < groups, "block_group names a group >= ", groups);
+        args_.block_group = bg.data_ptr<uint8_t>();
+        args_.hyper_groups = reinterpret_cast<const SgpHyper*>(hg.data_ptr<float>());
+        args_.groups = groups;
+        groups_keep_ = {bg, hg};
+    }
+    int param_groups() const { return args_.groups; }
+
     void step(unsigned int flags, int grid)
     {
         check_grid(grid);
@@ -246,6 +282,7 @@ public:
             a.flags |= SGP_F_MSG_BF16;
         }
         if (a.flags & SGP_F_SGD) TORCH_CHECK(a.g && a.m, "SGD needs grad + momentum buffers");
+        if ((a.flags & SGP_F_SGD) && a.groups > 0) a.flags |= SGP_F_GROUPS;
         if (a.flags & SGP_F_FOLD_RES) TORCH_CHECK(a.residual, "fold needs a residual buffer");
         if (a.flags & SGP_F_PUBLISH) TORCH_CHECK(a.outboxes, "publish needs outboxes");
         if (a.flags & SGP_F_PHASE2) TORCH_CHECK(a.flags & SGP_F_PUBLISH, "phase 2 needs publish");
@@ -469,6 +506,7 @@ private:
     torch::Tensor grad_keep_;
     torch::Tensor grad2_keep_;
     torch::Tensor mom_keep_;
+    std::vector<torch::Tensor> groups_keep_;
     torch::Tensor cons_slots_;
     torch::Tensor cons_scratch_;
     torch::Tensor cons_result_;
@@ -763,6 +801,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, mod)
     mod.attr("F_KEEP_Z") = (unsigned)SGP_F_KEEP_Z;
     mod.attr("F_SELF_FROM_Z") = (unsigned)SGP_F_SELF_FROM_Z;
     mod.attr("F_MSG_BF16") = (unsigned)SGP_F_MSG_BF16;
+    mod.attr("F_GROUPS") = (unsigned)SGP_F_GROUPS;
+    mod.attr("MAX_GROUPS") = (int)SGP_MAX_GROUPS;
+    mod.attr("GROUP_BLOCK") = (int)SGP_GROUP_BLOCK;
 
     py::class_<BilatDaemon>(mod, "BilatDaemon")
         .def(py::init<std::shared_ptr<GossipContext>, int, bool, double, int, double>(), py::arg("ctx"),
@@ -800,6 +841,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, mod)
         .def("set_grad", &GossipContext::set_grad)
         .def("set_sgd_buffers", &GossipContext::set_sgd_buffers)
         .def("set_grad2", &GossipContext::set_grad2)
+        .def("set_param_groups", &GossipContext::set_param_groups, py::arg("block_group"), py::arg("hyper_groups"))
+        .def("param_groups", &GossipContext::param_groups)
         .def("set_timeout", &GossipContext::set_timeout)
         .def("set_segments", &GossipContext::set_segments)
         .def("bilat_decide", &GossipContext::bilat_decide, py::arg("pub_grid"), py::arg("passive"),

@@ -112,6 +112,13 @@ struct SgpHyper {
 // keeps c = x - (1 - self_w) * Q(x) in z, and phase 2 mixes c + sum_k in_w[k] * Q(x_k), so the
 // network's push-sum mass sum_i x_i is conserved exactly (up to fp32 rounding)
 #define SGP_F_MSG_BF16   (1u << 13)
+// per-parameter-group SGD (SGD modes of the step kernels only): the 64-float block containing
+// element i belongs to group block_group[i / 64] and takes lr / momentum / weight_decay / nesterov
+// from hyper_groups[group]; do_sgd and grad_scale stay those of *hyper.  Exact because every
+// tensor of the arena starts on a 64-element boundary (utils/arena.py ALIGN_ELEMS)
+#define SGP_F_GROUPS     (1u << 14)
+#define SGP_MAX_GROUPS   16
+#define SGP_GROUP_BLOCK  64     // elements per block_group entry
 
 struct SgpArgs {
     // local buffers (length n, n % SGP_CHUNK == 0)
@@ -140,6 +147,10 @@ struct SgpArgs {
     unsigned long long   timeout_ns;
     unsigned int         flags;
     int                  segments;   // phase-1/phase-2 interleave granularity per CTA
+    // SGP_F_GROUPS (appended last: the offsets of the fields above are unchanged)
+    const SgpHyper*      hyper_groups;   // [groups] rows (device resident, like *hyper)
+    const uint8_t*       block_group;    // [n / SGP_GROUP_BLOCK] group of each 64-float block
+    int                  groups;
 };
 
 #ifdef __CUDACC__

@@ -59,6 +59,26 @@ __device__ __forceinline__ void sgd1(float& x, float g, float& m, float lr, floa
     x = fmaf(-lr, upd, x);
 }
 
+// SGP_F_GROUPS: the group rows {lr, momentum, weight_decay, nesterov} go to shared memory once
+// per CTA (threads [0, groups) copy one row each; the caller synchronises).  A 16-byte access
+// never straddles a 64-float block, so one block_group byte serves all four lanes of a float4
+__device__ __forceinline__ void load_group_rows(const SgpArgs& a, float4* s_rows, int tid) {
+    if (tid < a.groups) {
+        const SgpHyper h = a.hyper_groups[tid];
+        s_rows[tid] = make_float4(h.lr, h.momentum, h.weight_decay, h.nesterov);
+    }
+}
+__device__ __forceinline__ uint32_t block_group_of(const SgpArgs& a, long long i) {
+    return __ldg(a.block_group + (i / SGP_GROUP_BLOCK));
+}
+// sgd1 on the four lanes with one set of hyper-parameters (same fmaf order as the ungrouped path)
+__device__ __forceinline__ void sgd4(float4& xv, const float4& gv, float4& mv, const float4& h) {
+    sgd1(xv.x, gv.x, mv.x, h.x, h.y, h.z, h.w);
+    sgd1(xv.y, gv.y, mv.y, h.x, h.y, h.z, h.w);
+    sgd1(xv.z, gv.z, mv.z, h.x, h.y, h.z, h.w);
+    sgd1(xv.w, gv.w, mv.w, h.x, h.y, h.z, h.w);
+}
+
 // Last-CTA bookkeeping shared by the kernels: returns true in thread 0 of the
 // CTA that finishes last.
 __device__ __forceinline__ bool cta_done_is_last(SgpState* st) {
@@ -77,8 +97,9 @@ __device__ __forceinline__ bool cta_done_is_last(SgpState* st) {
 // Fused step kernel.  MSG_BF16 (SGP_F_MSG_BF16): bf16 messages, full synchronous step only
 // (PHASE1 | PUBLISH | PHASE2; the launcher rejects every other mode): phase 1 publishes Q(x) and
 // keeps c = x - (1 - self_w) Q(x) in z, phase 2 mixes c + sum_k in_w[k] Q(x_k).
+// GROUPS (SGP_F_GROUPS): per-parameter-group SGD, see load_group_rows / block_group_of.
 // ---------------------------------------------------------------------------
-template <bool MSG_BF16>
+template <bool MSG_BF16, bool GROUPS>
 __global__ void __launch_bounds__(SGP_THREADS, 2)
 sgp_step_kernel(const SgpArgs a)
 {
@@ -116,6 +137,13 @@ sgp_step_kernel(const SgpArgs a)
     const uint64_t pol_first = l2_evict_first_policy();
     const uint64_t pol_last = l2_evict_last_policy();
     const bool do_sgd = (flags & SGP_F_SGD) && (hp.do_sgd != 0.f);
+    const float4* s_rows = nullptr;
+    if constexpr (GROUPS) {
+        __shared__ float4 s_group_rows[SGP_MAX_GROUPS];
+        load_group_rows(a, s_group_rows, tid);
+        __syncthreads();
+        s_rows = s_group_rows;
+    }
 
     // Work decomposition: this CTA owns chunks b, b+G, b+2G, ...; they are cut into
     // K contiguous SEGMENTS.  For each segment the CTA runs phase 1 (local update +
@@ -171,6 +199,7 @@ sgp_step_kernel(const SgpArgs a)
                 const long long c = b + it * gridDim.x;
                 const long long base = c * SGP_CHUNK + (long long)tid * SGP_VEC;
                 float4 x[SGP_UNROLL], g[SGP_UNROLL], m[SGP_UNROLL], r[SGP_UNROLL];
+                uint32_t grp[SGP_UNROLL];
 #pragma unroll
                 for (int u = 0; u < SGP_UNROLL; ++u) {
                     const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
@@ -187,6 +216,7 @@ sgp_step_kernel(const SgpArgs a)
                             g[u].x += h.x; g[u].y += h.y; g[u].z += h.z; g[u].w += h.w;
                         }
                         m[u] = ld_once_f4(reinterpret_cast<const float4*>(a.m + i), pol_first);
+                        if constexpr (GROUPS) grp[u] = block_group_of(a, i);
                     }
                     if (flags & SGP_F_FOLD_RES)
                         r[u] = ld_once_f4(reinterpret_cast<const float4*>(a.residual + i), pol_first);
@@ -198,10 +228,14 @@ sgp_step_kernel(const SgpArgs a)
                     if (do_sgd) {
                         float4 gv = mul4(g[u], hp.grad_scale);
                         float4 mv = m[u];
-                        sgd1(xv.x, gv.x, mv.x, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
-                        sgd1(xv.y, gv.y, mv.y, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
-                        sgd1(xv.z, gv.z, mv.z, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
-                        sgd1(xv.w, gv.w, mv.w, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
+                        if constexpr (GROUPS) {
+                            sgd4(xv, gv, mv, s_rows[grp[u]]);
+                        } else {
+                            sgd1(xv.x, gv.x, mv.x, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
+                            sgd1(xv.y, gv.y, mv.y, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
+                            sgd1(xv.z, gv.z, mv.z, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
+                            sgd1(xv.w, gv.w, mv.w, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
+                        }
                         st_f4(reinterpret_cast<float4*>(a.m + i), mv);
                         if (flags & SGP_F_ZERO_GRAD) {
                             if (flags & SGP_F_GRAD_BF16)
@@ -630,7 +664,8 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 // 9 warps x 2 CTAs per SM: the register file is split over 4 sub-partitions (16 K registers
 // each), so 18 warps only fit at <= 102 registers per thread -- __launch_bounds__(288, 2) makes
 // ptxas pick 96.  (At 112 registers the kernel runs one CTA per SM.)
-template <bool MSG_BF16>
+// GROUPS (SGP_F_GROUPS): per-parameter-group SGD as in sgp_step_kernel.
+template <bool MSG_BF16, bool GROUPS>
 __global__ void __launch_bounds__(PIPE_THREADS, 2)
 sgp_step_pipe_kernel(const SgpArgs a)
 {
@@ -683,6 +718,12 @@ sgp_step_pipe_kernel(const SgpArgs a)
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         s_fail = 0;
         s_ok = 1;
+    }
+    const float4* s_rows = nullptr;
+    if constexpr (GROUPS) {
+        __shared__ float4 s_group_rows[SGP_MAX_GROUPS];
+        load_group_rows(a, s_group_rows, tid);
+        s_rows = s_group_rows;
     }
     __syncthreads();
 
@@ -762,6 +803,7 @@ sgp_step_pipe_kernel(const SgpArgs a)
                     const long long c = b + it * gridDim.x;
                     const long long base = c * SGP_CHUNK + (long long)tid * SGP_VEC;
                     float4 x[SGP_UNROLL], g[SGP_UNROLL], m[SGP_UNROLL];
+                    uint32_t grp[SGP_UNROLL];
 #pragma unroll
                     for (int u = 0; u < SGP_UNROLL; ++u) {
                         const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
@@ -778,6 +820,7 @@ sgp_step_pipe_kernel(const SgpArgs a)
                                 g[u].x += h.x; g[u].y += h.y; g[u].z += h.z; g[u].w += h.w;
                             }
                             m[u] = ld_once_f4(reinterpret_cast<const float4*>(a.m + i), pol_first);
+                            if constexpr (GROUPS) grp[u] = block_group_of(a, i);
                         }
                     }
 #pragma unroll
@@ -787,10 +830,14 @@ sgp_step_pipe_kernel(const SgpArgs a)
                         if (do_sgd) {
                             float4 gv = mul4(g[u], hp.grad_scale);
                             float4 mv = m[u];
-                            sgd1(xv.x, gv.x, mv.x, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
-                            sgd1(xv.y, gv.y, mv.y, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
-                            sgd1(xv.z, gv.z, mv.z, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
-                            sgd1(xv.w, gv.w, mv.w, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
+                            if constexpr (GROUPS) {
+                                sgd4(xv, gv, mv, s_rows[grp[u]]);
+                            } else {
+                                sgd1(xv.x, gv.x, mv.x, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
+                                sgd1(xv.y, gv.y, mv.y, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
+                                sgd1(xv.z, gv.z, mv.z, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
+                                sgd1(xv.w, gv.w, mv.w, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
+                            }
                             st_f4(reinterpret_cast<float4*>(a.m + i), mv);
                             if (flags & SGP_F_ZERO_GRAD) {
                                 if (flags & SGP_F_GRAD_BF16)
@@ -1594,64 +1641,95 @@ static bool msg_bf16_mode_ok(unsigned int flags)
     return (flags & full) == full && (flags & partial) == 0u;
 }
 
-template <bool MSG_BF16>
+template <bool MSG_BF16, bool GROUPS>
 static cudaError_t configure_step_pipe()
 {
-    cudaError_t e = cudaFuncSetAttribute(sgp_step_pipe_kernel<MSG_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         PIPE_SMEM);
+    cudaError_t e = cudaFuncSetAttribute(sgp_step_pipe_kernel<MSG_BF16, GROUPS>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, PIPE_SMEM);
     if (e != cudaSuccess) return e;
     // two CTAs x 64 KB per SM: ask for the large shared-memory carve-out (the default one fits
     // a single CTA: launch__occupancy_limit_shared_mem = 1 in the first ncu capture)
-    return cudaFuncSetAttribute(sgp_step_pipe_kernel<MSG_BF16>, cudaFuncAttributePreferredSharedMemoryCarveout,
+    return cudaFuncSetAttribute(sgp_step_pipe_kernel<MSG_BF16, GROUPS>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                 cudaSharedmemCarveoutMaxShared);
+}
+
+static cudaError_t configure_step_pipe_all()
+{
+    cudaError_t e = configure_step_pipe<false, false>();
+    if (e == cudaSuccess) e = configure_step_pipe<true, false>();
+    if (e == cudaSuccess) e = configure_step_pipe<false, true>();
+    if (e == cudaSuccess) e = configure_step_pipe<true, true>();
+    return e;
+}
+
+// SGP_F_GROUPS needs the group table, the block map and 1..SGP_MAX_GROUPS groups
+static bool groups_ok(const SgpArgs* args)
+{
+    if (!(args->flags & SGP_F_GROUPS)) return true;
+    return args->hyper_groups && args->block_group && args->groups >= 1 && args->groups <= SGP_MAX_GROUPS;
 }
 
 extern "C" {
 
 cudaError_t sgp_launch_step(const SgpArgs* args, int grid, cudaStream_t stream)
 {
-    if (!msg_bf16_mode_ok(args->flags)) return cudaErrorInvalidValue;
-    if (args->flags & SGP_F_MSG_BF16)
-        sgp_step_kernel<true><<<grid, SGP_THREADS, 0, stream>>>(*args);
-    else
-        sgp_step_kernel<false><<<grid, SGP_THREADS, 0, stream>>>(*args);
+    if (!msg_bf16_mode_ok(args->flags) || !groups_ok(args)) return cudaErrorInvalidValue;
+    if (args->flags & SGP_F_GROUPS) {
+        if (args->flags & SGP_F_MSG_BF16)
+            sgp_step_kernel<true, true><<<grid, SGP_THREADS, 0, stream>>>(*args);
+        else
+            sgp_step_kernel<false, true><<<grid, SGP_THREADS, 0, stream>>>(*args);
+    } else if (args->flags & SGP_F_MSG_BF16) {
+        sgp_step_kernel<true, false><<<grid, SGP_THREADS, 0, stream>>>(*args);
+    } else {
+        sgp_step_kernel<false, false><<<grid, SGP_THREADS, 0, stream>>>(*args);
+    }
     return cudaGetLastError();
 }
 
 cudaError_t sgp_launch_step_pipe(const SgpArgs* args, int grid, cudaStream_t stream)
 {
-    if (!msg_bf16_mode_ok(args->flags)) return cudaErrorInvalidValue;
+    if (!msg_bf16_mode_ok(args->flags) || !groups_ok(args)) return cudaErrorInvalidValue;
     static bool configured[64] = {};
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64 || !configured[dev]) {
-        cudaError_t e = configure_step_pipe<false>();
-        if (e == cudaSuccess) e = configure_step_pipe<true>();
+        cudaError_t e = configure_step_pipe_all();
         if (e != cudaSuccess) return e;
         if (dev >= 0 && dev < 64) configured[dev] = true;
     }
     // (the bf16 ring uses half of each stage: the occupancy, and so the grid every rank shares,
     // stays that of the fp32 kernel)
-    if (args->flags & SGP_F_MSG_BF16)
-        sgp_step_pipe_kernel<true><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
-    else
-        sgp_step_pipe_kernel<false><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
+    if (args->flags & SGP_F_GROUPS) {
+        if (args->flags & SGP_F_MSG_BF16)
+            sgp_step_pipe_kernel<true, true><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
+        else
+            sgp_step_pipe_kernel<false, true><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
+    } else if (args->flags & SGP_F_MSG_BF16) {
+        sgp_step_pipe_kernel<true, false><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
+    } else {
+        sgp_step_pipe_kernel<false, false><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
+    }
     return cudaGetLastError();
 }
 
-// co-resident CTAs of the pipelined step kernel (dynamic shared memory bound)
+// co-resident CTAs of the pipelined step kernel (dynamic shared memory bound): the minimum over
+// its instantiations, because the ranks of a job share one grid whatever variant each launches
 int sgp_max_resident_ctas_pipe(int device)
 {
-    int sms = 0, per_sm = 0;
+    int sms = 0;
     if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) return 0;
-    configure_step_pipe<false>();
-    configure_step_pipe<true>();
-    int per_sm_bf16 = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sgp_step_pipe_kernel<false>, PIPE_THREADS, PIPE_SMEM)
-        != cudaSuccess) return 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_bf16, sgp_step_pipe_kernel<true>, PIPE_THREADS,
-                                                      PIPE_SMEM) != cudaSuccess) return 0;
-    if (per_sm_bf16 < per_sm) per_sm = per_sm_bf16;
+    configure_step_pipe_all();
+    const void* kernels[] = {(const void*)sgp_step_pipe_kernel<false, false>,
+                             (const void*)sgp_step_pipe_kernel<true, false>,
+                             (const void*)sgp_step_pipe_kernel<false, true>,
+                             (const void*)sgp_step_pipe_kernel<true, true>};
+    int per_sm = 1 << 30;
+    for (const void* k : kernels) {
+        int n = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k, PIPE_THREADS, PIPE_SMEM) != cudaSuccess) return 0;
+        if (n < per_sm) per_sm = n;
+    }
     return sms * per_sm;
 }
 
@@ -1825,9 +1903,12 @@ cudaError_t sgp_launch_slowmo(const SgpArgs* args, float* u, float* x_prev, floa
 cudaError_t sgp_preload_kernels()
 {
     const void* kernels[] = {
-        (const void*)sgp_step_kernel<false>, (const void*)sgp_step_kernel<true>, (const void*)sgp_gather_kernel,
-        (const void*)sgp_gather_tma_kernel, (const void*)sgp_step_pipe_kernel<false>,
-        (const void*)sgp_step_pipe_kernel<true>, (const void*)sgp_probe_kernel, (const void*)sgp_gather_wait_kernel,
+        (const void*)sgp_step_kernel<false, false>, (const void*)sgp_step_kernel<true, false>,
+        (const void*)sgp_step_kernel<false, true>, (const void*)sgp_step_kernel<true, true>,
+        (const void*)sgp_gather_kernel, (const void*)sgp_gather_tma_kernel,
+        (const void*)sgp_step_pipe_kernel<false, false>, (const void*)sgp_step_pipe_kernel<true, false>,
+        (const void*)sgp_step_pipe_kernel<false, true>, (const void*)sgp_step_pipe_kernel<true, true>,
+        (const void*)sgp_probe_kernel, (const void*)sgp_gather_wait_kernel,
         (const void*)sgp_gather_ack_kernel, (const void*)sgp_bilat_decide_kernel, (const void*)sgp_bilat_ctl_kernel,
         (const void*)sgp_allreduce_sgd_kernel, (const void*)sgp_zero_kernel, (const void*)sgp_barrier_kernel,
         (const void*)sgp_scale_kernel, (const void*)sgp_peer_reduce_kernel, (const void*)sgp_snapshot_kernel,
@@ -1845,8 +1926,12 @@ int sgp_max_resident_ctas(int device)
 {
     int sms = 0, per_sm = 0;
     if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) return 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sgp_step_kernel<false>, SGP_THREADS, 0)
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sgp_step_kernel<false, false>, SGP_THREADS, 0)
         != cudaSuccess) return 0;
+    int per_sm_groups = 0;      // (the grouped variant is launched on the same grid)
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_groups, sgp_step_kernel<false, true>, SGP_THREADS, 0)
+        != cudaSuccess) return 0;
+    if (per_sm_groups < per_sm) per_sm = per_sm_groups;
     return sms * per_sm;
 }
 

@@ -12,10 +12,14 @@ import torch
 
 
 def sgd_momentum(x, g, m, lr, momentum, weight_decay, nesterov):
-    """torch.optim.SGD (dampening 0) on the push-sum numerator; returns (x, m)."""
+    """torch.optim.SGD (dampening 0) on the push-sum numerator; returns (x, m).  The
+    hyper-parameters are scalars or per-element tensors (``nesterov`` then a bool tensor)."""
     d = g + weight_decay * x
     m = momentum * m + d
-    upd = d + momentum * m if nesterov else m
+    if isinstance(nesterov, torch.Tensor):
+        upd = torch.where(nesterov, d + momentum * m, m)
+    else:
+        upd = d + momentum * m if nesterov else m
     return x - lr * upd, m
 
 

@@ -115,10 +115,15 @@ class GossipEngine(object):
         self._state_f32[C.STATE_OFF_RES_SCALE // 4] = 1.0
         self._phase_base = 0            # host mirror of SgpState::phase_base
         self._gather_dma_pref = gather_dma
-        self.hyper = torch.zeros(C.HYPER_FLOATS, dtype=torch.float32, device=self.device)
-        # ring of pinned staging rows: an lr change must not rewrite host memory that an earlier,
+        # row 0: the hyper-parameters every SGD launch reads; rows 1..G: per-parameter-group rows
+        # (set_param_groups), all in one buffer so that one H2D copy updates them together
+        self._hyper_rows = torch.zeros(1 + C.MAX_GROUPS, C.HYPER_FLOATS, dtype=torch.float32,
+                                       device=self.device)
+        self.hyper = self._hyper_rows[0]
+        self.groups = 0
+        # ring of pinned staging slots: an lr change must not rewrite host memory that an earlier,
         # still-queued async H2D copy is going to read
-        self._hyper_host = torch.zeros(8, C.HYPER_FLOATS, dtype=torch.float32).pin_memory()
+        self._hyper_host = torch.zeros(8, 1 + C.MAX_GROUPS, C.HYPER_FLOATS, dtype=torch.float32).pin_memory()
         self._hyper_slot = 0
         self._hyper_events = [None] * 8
         self._hyper_cache = None
@@ -153,9 +158,18 @@ class GossipEngine(object):
         world.barrier()
 
     # -- configuration ------------------------------------------------------ #
-    def set_hyper(self, lr, momentum, weight_decay, nesterov, do_sgd=True, grad_scale=1.0):
+    def set_hyper(self, lr, momentum, weight_decay, nesterov, do_sgd=True, grad_scale=1.0, groups=None):
+        """Stage the SGD hyper-parameters for the next launches (device resident: a captured graph
+        reads the new values).  ``groups``: with :meth:`set_param_groups`, one
+        ``(lr, momentum, weight_decay, nesterov)`` per parameter group; ``do_sgd`` and
+        ``grad_scale`` apply to every group."""
         key = (float(lr), float(momentum), float(weight_decay), bool(nesterov),
                bool(do_sgd), float(grad_scale))
+        if groups is not None:
+            if len(groups) != self.groups:
+                raise ValueError('set_hyper got %d group rows, set_param_groups configured %d'
+                                 % (len(groups), self.groups))
+            key += tuple((float(a), float(b), float(c), bool(d)) for a, b, c, d in groups)
         if key == self._hyper_cache:
             return
         self._hyper_cache = key
@@ -163,15 +177,36 @@ class GossipEngine(object):
         self._hyper_slot = (slot + 1) % self._hyper_host.shape[0]
         ev = self._hyper_events[slot]
         if ev is not None:
-            ev.synchronize()                 # the copy that last used this row has executed
-        h = self._hyper_host[slot]
+            ev.synchronize()                 # the copy that last used this slot has executed
+        h = self._hyper_host[slot][0]
         h[0], h[1], h[2] = key[0], key[1], key[2]
         h[3] = 1.0 if key[3] else 0.0
         h[4] = 1.0 if key[4] else 0.0
         h[5] = key[5]
-        self.hyper.copy_(h, non_blocking=True)
+        if groups is None:
+            self.hyper.copy_(h, non_blocking=True)
+        else:
+            rows = self._hyper_host[slot][:1 + len(groups)]
+            for r, (g_lr, g_mu, g_wd, g_nest) in zip(rows[1:], key[6:]):
+                r[0], r[1], r[2], r[3] = g_lr, g_mu, g_wd, 1.0 if g_nest else 0.0
+            self._hyper_rows[:1 + len(groups)].copy_(rows, non_blocking=True)
         ev = self._hyper_events[slot] = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(self.device))
+
+    def set_param_groups(self, block_group: Optional[torch.Tensor], groups: int):
+        """Per-parameter-group SGD: ``block_group`` (uint8, one entry per 64 elements of the arena)
+        names the group of each 64-element block; every SGD launch then takes lr / momentum /
+        weight_decay / nesterov from that group's row, staged by ``set_hyper(..., groups=rows)``.
+        ``block_group=None`` returns to the single set of hyper-parameters."""
+        if block_group is None:
+            self.ctx.set_param_groups(None, None)
+            self.groups = 0
+        else:
+            if not 1 <= groups <= self.C.MAX_GROUPS:
+                raise ValueError('1 to %d parameter groups, got %d' % (self.C.MAX_GROUPS, groups))
+            self.ctx.set_param_groups(block_group, self._hyper_rows[1:1 + groups])
+            self.groups = int(groups)
+        self._hyper_cache = None
 
     def set_schedule(self, graph=None, mixing=None):
         """Re-emit the device tables (e.g. after ``peers_per_itr`` changed).

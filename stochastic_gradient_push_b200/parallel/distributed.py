@@ -675,6 +675,11 @@ class GossipDataParallel(Module):
             self._slowmo_calls = calls
             return None
         gamma = float(optimizer.param_groups[0]['lr'])
+        if any(float(g['lr']) != gamma for g in optimizer.param_groups):
+            # u is the displacement over gamma: one gamma per model (groups may differ in weight
+            # decay or momentum, as with no-bias-decay)
+            raise ValueError('SlowMo needs one base learning rate; the parameter groups have lr %s'
+                             % [float(g['lr']) for g in optimizer.param_groups])
         if not gamma > 0:
             raise ValueError('SlowMo needs a positive base learning rate, got %r' % gamma)
         self._slowmo_calls = calls

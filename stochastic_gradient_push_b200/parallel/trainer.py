@@ -202,12 +202,16 @@ class GossipTrainer(object):
         self._stage_free.record(self.stream)
 
     def _set_lr(self):
-        g = self.opt.param_groups[0]
         # overlap: the SGD of step k runs inside publish(k+1).  After finish() applied it early
         # (end of epoch / checkpoint) the next replay's publish must not apply it again: the
-        # captured kernel reads `do_sgd` from device memory
+        # captured kernel reads `do_sgd` from device memory.  Every parameter group's values go
+        # to the device table too, so a per-group lr change needs no re-capture
         do_sgd = not self._skip_next_sgd
         self._skip_next_sgd = False
+        if isinstance(self.opt, FusedGossipSGD):
+            self.opt.set_engine_hyper(self.engine, do_sgd=do_sgd)
+            return
+        g = self.opt.param_groups[0]          # (the all-reduce / AD-PSGD trainers' one-group facades)
         self.engine.set_hyper(g['lr'], g['momentum'], g['weight_decay'], g['nesterov'],
                               do_sgd=do_sgd, grad_scale=self.opt.grad_scale)
 

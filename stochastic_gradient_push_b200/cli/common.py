@@ -60,6 +60,12 @@ def build_parser(adpsgd: bool = False) -> argparse.ArgumentParser:
                    help='no weight decay on parameters with ndim <= 1 (BatchNorm weight and bias, all '
                         'biases): two parameter groups (optim.no_bias_decay_groups), for --fused True '
                         'and False alike.  SGP / OSGP / D-PSGD')
+    p.add_argument('--lars', default=False, **B,
+                   help='LARS (layer-wise adaptive rate scaling) inside the fused gossip step '
+                        '(FusedGossipSGD(lars=True)); with --no_bias_decay True the groups are '
+                        'optim.lars_groups (no decay and no LARS for ndim <= 1 parameters).  --fused True '
+                        'with SGP / OSGP / D-PSGD only')
+    p.add_argument('--lars_trust', default=0.001, type=float, help='LARS trust coefficient eta')
     p.add_argument('--push_sum', default=True, **B, help='push-sum (SGP) or push-pull (D-PSGD)')
     p.add_argument('--graph_type', default=5, type=int, choices=list(GRAPH_TOPOLOGIES))
     p.add_argument('--mixing_strategy', default=0, type=int, choices=list(MIXING_STRATEGIES))
@@ -226,6 +232,14 @@ def finalize_args(args, adpsgd=False):
         if unsupported:
             raise ValueError('--no_bias_decay is not supported with %s: parameter groups are '
                              'implemented for SGP, OSGP and D-PSGD' % unsupported)
+    if getattr(args, 'lars', False):
+        unsupported = ('AD-PSGD' if adpsgd else '--all_reduce' if args.all_reduce else
+                       '--fused False' if not getattr(args, 'fused', True) else None)
+        if unsupported:
+            raise ValueError('--lars is not supported with %s: LARS is implemented in the fused gossip '
+                             'step (FusedGossipSGD) for SGP, OSGP and D-PSGD' % unsupported)
+        if not args.lars_trust > 0:
+            raise ValueError('--lars_trust must be > 0')
     if getattr(args, 'slowmo_frequency', 0):
         unsupported = ('AD-PSGD' if adpsgd else '--all_reduce' if args.all_reduce else
                        '--nprocs_per_node > 1' if getattr(args, 'nprocs_per_node', 1) > 1 else None)

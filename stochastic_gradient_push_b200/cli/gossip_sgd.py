@@ -47,7 +47,7 @@ def parse_args(argv=None):
 
 
 def build_model_and_optimizer(args, log):
-    from ..optim import FusedGossipSGD, no_bias_decay_groups
+    from ..optim import FusedGossipSGD, lars_groups, no_bias_decay_groups
     from ..parallel.distributed import GossipDataParallel
     net = init_model(args)
     if args.all_reduce:
@@ -72,11 +72,13 @@ def build_model_and_optimizer(args, log):
         compute_dtype=(torch.bfloat16 if (args.cuda_graph and args.amp and args.fused
                                           and args.device == 'cuda' and args.transport != 'c10d')
                        else None))
-    groups = no_bias_decay_groups(net, args.weight_decay) if args.no_bias_decay else None
+    groups = None
+    if args.no_bias_decay:
+        groups = (lars_groups if args.lars else no_bias_decay_groups)(net, args.weight_decay)
     if args.fused:
         optimizer = FusedGossipSGD(model, lr=args.lr, momentum=args.momentum,
                                    weight_decay=args.weight_decay, nesterov=args.nesterov,
-                                   param_groups=groups)
+                                   param_groups=groups, lars=args.lars, trust_coefficient=args.lars_trust)
     else:
         optimizer = torch.optim.SGD(groups if groups is not None else model.parameters(), lr=args.lr,
                                     momentum=args.momentum, weight_decay=args.weight_decay,

@@ -119,6 +119,19 @@ struct SgpHyper {
 #define SGP_F_GROUPS     (1u << 14)
 #define SGP_MAX_GROUPS   16
 #define SGP_GROUP_BLOCK  64     // elements per block_group entry
+// LARS (SGD modes with SGP_F_GROUPS only): phase 1 scales each element's d = g + wd*x by the trust
+// ratio of its tensor, lars_trust[block_tensor[i / 64]], which sgp_lars_norms_kernel and
+// sgp_lars_trust_kernel compute right before the step on the same stream
+#define SGP_F_LARS       (1u << 15)
+#define SGP_LARS_TILE    4096   // elements per norm tile (a tile never crosses a tensor boundary)
+#define SGP_LARS_MAX_TENSORS 65535
+
+// one norm tile: `count` elements of tensor `tensor` from arena element `start` (a multiple of 64)
+struct SgpLarsTile {
+    long long start;
+    int       tensor;
+    int       count;
+};
 
 struct SgpArgs {
     // local buffers (length n, n % SGP_CHUNK == 0)
@@ -151,6 +164,18 @@ struct SgpArgs {
     const SgpHyper*      hyper_groups;   // [groups] rows (device resident, like *hyper)
     const uint8_t*       block_group;    // [n / SGP_GROUP_BLOCK] group of each 64-float block
     int                  groups;
+    // SGP_F_LARS (appended after the group fields for the same reason)
+    const uint16_t*      block_tensor;   // [n / SGP_GROUP_BLOCK] tensor of each 64-float block
+    float*               lars_trust;     // [lars_tensors] trust ratio per tensor (1 where disabled)
+    const uint8_t*       lars_enabled;   // [lars_tensors] 1: the tensor's group has lars=True
+    const SgpLarsTile*   lars_tiles;     // [lars_ntiles], ordered by tensor, then by start
+    const int*           lars_tile_first;// [lars_tensors + 1] first tile of each tensor
+    double*              lars_partials;  // [lars_ntiles][2] sum x^2, sum g^2 of each tile
+    double*              lars_sumsq;     // [lars_tensors][2] sum x^2, sum g^2 of each tensor
+    int                  lars_tensors;
+    int                  lars_ntiles;
+    float                lars_eta;       // trust coefficient
+    float                lars_eps;
 };
 
 #ifdef __CUDACC__
@@ -287,6 +312,8 @@ extern "C" {
 cudaError_t sgp_launch_step(const SgpArgs* args, int grid, cudaStream_t stream);
 cudaError_t sgp_launch_step_pipe(const SgpArgs* args, int grid, cudaStream_t stream);
 int sgp_max_resident_ctas_pipe(int device);
+cudaError_t sgp_launch_lars_norms(const SgpArgs* args, int grid, cudaStream_t stream);
+cudaError_t sgp_launch_lars_trust(const SgpArgs* args, cudaStream_t stream);
 cudaError_t sgp_launch_gather(const SgpArgs* args, int grid, int pub_grid, cudaStream_t stream);
 cudaError_t sgp_launch_gather_tma(const SgpArgs* args, int grid, int pub_grid, cudaStream_t stream);
 cudaError_t sgp_launch_probe(const SgpArgs* args, int pub_grid, uint32_t* host_flag,

@@ -79,6 +79,27 @@ __device__ __forceinline__ void sgd4(float4& xv, const float4& gv, float4& mv, c
     sgd1(xv.w, gv.w, mv.w, h.x, h.y, h.z, h.w);
 }
 
+// SGP_F_LARS: sgd1 with d = t * (g + wd*x), t the trust ratio of the element's tensor.  t == 1
+// (LARS disabled, zero norms) multiplies exactly, so those elements get sgd1's bits
+__device__ __forceinline__ void sgd1_lars(float& x, float g, float& m, float lr, float mu,
+                                          float wd, float nesterov, float t) {
+    const float d = t * fmaf(wd, x, g);
+    m = fmaf(mu, m, d);
+    const float upd = (nesterov != 0.f) ? fmaf(mu, m, d) : m;
+    x = fmaf(-lr, upd, x);
+}
+__device__ __forceinline__ void sgd4_lars(float4& xv, const float4& gv, float4& mv, const float4& h, float t) {
+    sgd1_lars(xv.x, gv.x, mv.x, h.x, h.y, h.z, h.w, t);
+    sgd1_lars(xv.y, gv.y, mv.y, h.x, h.y, h.z, h.w, t);
+    sgd1_lars(xv.z, gv.z, mv.z, h.x, h.y, h.z, h.w, t);
+    sgd1_lars(xv.w, gv.w, mv.w, h.x, h.y, h.z, h.w, t);
+}
+// trust ratio of the tensor that owns the 64-float block of element i (written by
+// sgp_lars_trust_kernel earlier on the stream, so the read-only path is safe)
+__device__ __forceinline__ float lars_trust_of(const SgpArgs& a, long long i) {
+    return __ldg(a.lars_trust + __ldg(a.block_tensor + (i / SGP_GROUP_BLOCK)));
+}
+
 // Last-CTA bookkeeping shared by the kernels: returns true in thread 0 of the
 // CTA that finishes last.
 __device__ __forceinline__ bool cta_done_is_last(SgpState* st) {
@@ -98,8 +119,9 @@ __device__ __forceinline__ bool cta_done_is_last(SgpState* st) {
 // (PHASE1 | PUBLISH | PHASE2; the launcher rejects every other mode): phase 1 publishes Q(x) and
 // keeps c = x - (1 - self_w) Q(x) in z, phase 2 mixes c + sum_k in_w[k] Q(x_k).
 // GROUPS (SGP_F_GROUPS): per-parameter-group SGD, see load_group_rows / block_group_of.
+// LARS (SGP_F_LARS, only with GROUPS): per-tensor trust ratio, see lars_trust_of.
 // ---------------------------------------------------------------------------
-template <bool MSG_BF16, bool GROUPS>
+template <bool MSG_BF16, bool GROUPS, bool LARS>
 __global__ void __launch_bounds__(SGP_THREADS, 2)
 sgp_step_kernel(const SgpArgs a)
 {
@@ -200,6 +222,7 @@ sgp_step_kernel(const SgpArgs a)
                 const long long base = c * SGP_CHUNK + (long long)tid * SGP_VEC;
                 float4 x[SGP_UNROLL], g[SGP_UNROLL], m[SGP_UNROLL], r[SGP_UNROLL];
                 uint32_t grp[SGP_UNROLL];
+                float tr[SGP_UNROLL];
 #pragma unroll
                 for (int u = 0; u < SGP_UNROLL; ++u) {
                     const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
@@ -217,6 +240,7 @@ sgp_step_kernel(const SgpArgs a)
                         }
                         m[u] = ld_once_f4(reinterpret_cast<const float4*>(a.m + i), pol_first);
                         if constexpr (GROUPS) grp[u] = block_group_of(a, i);
+                        if constexpr (LARS) tr[u] = lars_trust_of(a, i);
                     }
                     if (flags & SGP_F_FOLD_RES)
                         r[u] = ld_once_f4(reinterpret_cast<const float4*>(a.residual + i), pol_first);
@@ -228,7 +252,9 @@ sgp_step_kernel(const SgpArgs a)
                     if (do_sgd) {
                         float4 gv = mul4(g[u], hp.grad_scale);
                         float4 mv = m[u];
-                        if constexpr (GROUPS) {
+                        if constexpr (LARS) {
+                            sgd4_lars(xv, gv, mv, s_rows[grp[u]], tr[u]);
+                        } else if constexpr (GROUPS) {
                             sgd4(xv, gv, mv, s_rows[grp[u]]);
                         } else {
                             sgd1(xv.x, gv.x, mv.x, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
@@ -664,8 +690,8 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 // 9 warps x 2 CTAs per SM: the register file is split over 4 sub-partitions (16 K registers
 // each), so 18 warps only fit at <= 102 registers per thread -- __launch_bounds__(288, 2) makes
 // ptxas pick 96.  (At 112 registers the kernel runs one CTA per SM.)
-// GROUPS (SGP_F_GROUPS): per-parameter-group SGD as in sgp_step_kernel.
-template <bool MSG_BF16, bool GROUPS>
+// GROUPS (SGP_F_GROUPS) and LARS (SGP_F_LARS): as in sgp_step_kernel.
+template <bool MSG_BF16, bool GROUPS, bool LARS>
 __global__ void __launch_bounds__(PIPE_THREADS, 2)
 sgp_step_pipe_kernel(const SgpArgs a)
 {
@@ -804,6 +830,7 @@ sgp_step_pipe_kernel(const SgpArgs a)
                     const long long base = c * SGP_CHUNK + (long long)tid * SGP_VEC;
                     float4 x[SGP_UNROLL], g[SGP_UNROLL], m[SGP_UNROLL];
                     uint32_t grp[SGP_UNROLL];
+                    float tr[SGP_UNROLL];
 #pragma unroll
                     for (int u = 0; u < SGP_UNROLL; ++u) {
                         const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
@@ -821,6 +848,7 @@ sgp_step_pipe_kernel(const SgpArgs a)
                             }
                             m[u] = ld_once_f4(reinterpret_cast<const float4*>(a.m + i), pol_first);
                             if constexpr (GROUPS) grp[u] = block_group_of(a, i);
+                            if constexpr (LARS) tr[u] = lars_trust_of(a, i);
                         }
                     }
 #pragma unroll
@@ -830,7 +858,9 @@ sgp_step_pipe_kernel(const SgpArgs a)
                         if (do_sgd) {
                             float4 gv = mul4(g[u], hp.grad_scale);
                             float4 mv = m[u];
-                            if constexpr (GROUPS) {
+                            if constexpr (LARS) {
+                                sgd4_lars(xv, gv, mv, s_rows[grp[u]], tr[u]);
+                            } else if constexpr (GROUPS) {
                                 sgd4(xv, gv, mv, s_rows[grp[u]]);
                             } else {
                                 sgd1(xv.x, gv.x, mv.x, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
@@ -1629,6 +1659,123 @@ sgp_slowmo_kernel(const SgpArgs a, float* u, float* x_prev, float lr, float alph
 }
 
 // ---------------------------------------------------------------------------
+// LARS (SGP_F_LARS): per-tensor trust ratios, computed right before each SGD launch.
+//
+// sgp_lars_norms_kernel: grid-stride over the host-built tile table.  A tile is <= SGP_LARS_TILE
+// elements of ONE tensor; the CTA reads its x = z * wmul and g^ = grad_scale * (g [+ g2]) exactly
+// as phase 1 of the step kernels does (same fp32 operations), and writes the tile's sum x^2 and
+// sum g^2 in fp64 to lars_partials[tile].  Each thread owns fixed elements of the tile, the warps
+// reduce with a fixed shuffle tree and thread 0 adds the warps in order: no atomics, so the
+// partials -- and the trust ratios -- are bit-identical from run to run and for any grid.
+// ---------------------------------------------------------------------------
+__global__ void __launch_bounds__(SGP_THREADS)
+sgp_lars_norms_kernel(const SgpArgs a)
+{
+    __shared__ double s_x[SGP_THREADS / 32], s_g[SGP_THREADS / 32];
+    const SgpState* st = a.st;
+    const uint32_t parity = *((volatile const uint32_t*)&st->step) & 1u;
+    const float w0 = *((volatile const float*)&st->ps_weight[parity]);
+    const float wmul = (a.flags & SGP_F_IN_NUMER) ? 1.f : w0;    // as phase 1
+    const float gscale = a.hyper->grad_scale;
+    const bool g_bf16 = (a.flags & SGP_F_GRAD_BF16) != 0;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    static_assert(SGP_LARS_TILE == SGP_THREADS * SGP_VEC * SGP_UNROLL, "one pass per tile");
+
+    for (int t = blockIdx.x; t < a.lars_ntiles; t += gridDim.x) {
+        const SgpLarsTile tile = a.lars_tiles[t];
+        float4 xv[SGP_UNROLL], gv[SGP_UNROLL];
+#pragma unroll
+        for (int u = 0; u < SGP_UNROLL; ++u) {
+            // tile.start is a multiple of 64 and j of 4, so every float4 is aligned and stays
+            // inside the arena (lanes past tile.count are masked below)
+            const int j = (u * SGP_THREADS + tid) * SGP_VEC;
+            const long long i = tile.start + j;
+            xv[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+            gv[u] = xv[u];
+            if (j < tile.count) {
+                xv[u] = __ldg(reinterpret_cast<const float4*>(a.z + i));
+                if (g_bf16)
+                    gv[u] = bf16x4_to_f4(__ldg(reinterpret_cast<const uint2*>(
+                                reinterpret_cast<const __nv_bfloat16*>(a.g) + i)));
+                else
+                    gv[u] = __ldg(reinterpret_cast<const float4*>(reinterpret_cast<const float*>(a.g) + i));
+                if (a.g2 != nullptr) {
+                    const float4 h = __ldg(reinterpret_cast<const float4*>(a.g2 + i));
+                    gv[u].x += h.x; gv[u].y += h.y; gv[u].z += h.z; gv[u].w += h.w;
+                }
+            }
+        }
+        double sx = 0.0, sg = 0.0;
+#pragma unroll
+        for (int u = 0; u < SGP_UNROLL; ++u) {
+            const int j = (u * SGP_THREADS + tid) * SGP_VEC;
+            const float4 x = mul4(xv[u], wmul), g = mul4(gv[u], gscale);
+            const float xs[4] = {x.x, x.y, x.z, x.w}, gs[4] = {g.x, g.y, g.z, g.w};
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                if (j + k < tile.count) {
+                    sx = fma((double)xs[k], (double)xs[k], sx);
+                    sg = fma((double)gs[k], (double)gs[k], sg);
+                }
+            }
+        }
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) {
+            sx += __shfl_down_sync(0xffffffffu, sx, off);
+            sg += __shfl_down_sync(0xffffffffu, sg, off);
+        }
+        if (lane == 0) { s_x[warp] = sx; s_g[warp] = sg; }
+        __syncthreads();
+        if (tid == 0) {
+            double tx = 0.0, tg = 0.0;
+#pragma unroll
+            for (int w = 0; w < SGP_THREADS / 32; ++w) { tx += s_x[w]; tg += s_g[w]; }
+            a.lars_partials[2 * (long long)t] = tx;
+            a.lars_partials[2 * (long long)t + 1] = tg;
+        }
+        __syncthreads();
+    }
+}
+
+// sgp_lars_trust_kernel: one warp per tensor.  Lane l adds the tensor's tile partials l, l+32, ...
+// in order and a fixed shuffle tree combines the lanes (deterministic); lane 0 writes the sums to
+// lars_sumsq and the trust ratio
+//     t = eta |x| / (|g^| + wd |x| + eps)   if LARS is on for the tensor and |x| > 0 and |g^| > 0,
+//     t = 1                                 otherwise,
+// in fp64, rounded once to fp32.  wd is the weight decay of the tensor's group, read from the
+// device rows at every launch (so a change reaches a captured graph).
+__global__ void __launch_bounds__(SGP_THREADS)
+sgp_lars_trust_kernel(const SgpArgs a)
+{
+    const int t = (int)((blockIdx.x * (unsigned)SGP_THREADS + threadIdx.x) >> 5);
+    const int lane = threadIdx.x & 31;
+    if (t >= a.lars_tensors) return;                  // (whole warps)
+    const int k0 = a.lars_tile_first[t], k1 = a.lars_tile_first[t + 1];
+    double sx = 0.0, sg = 0.0;
+    for (int k = k0 + lane; k < k1; k += 32) {
+        sx += a.lars_partials[2 * (long long)k];
+        sg += a.lars_partials[2 * (long long)k + 1];
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+        sx += __shfl_down_sync(0xffffffffu, sx, off);
+        sg += __shfl_down_sync(0xffffffffu, sg, off);
+    }
+    if (lane == 0) {
+        a.lars_sumsq[2 * t] = sx;
+        a.lars_sumsq[2 * t + 1] = sg;
+        float tr = 1.f;
+        if (a.lars_enabled[t] != 0 && sx > 0.0 && sg > 0.0) {
+            const double nx = sqrt(sx), ng = sqrt(sg);
+            const int grp = a.block_group[a.lars_tiles[k0].start / SGP_GROUP_BLOCK];
+            const double wd = (double)a.hyper_groups[grp].weight_decay;
+            tr = (float)((double)a.lars_eta * nx / (ng + wd * nx + (double)a.lars_eps));
+        }
+        a.lars_trust[t] = tr;
+    }
+}
+
+// ---------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------
 // bf16 messages are implemented for the full synchronous step only
@@ -1641,24 +1788,26 @@ static bool msg_bf16_mode_ok(unsigned int flags)
     return (flags & full) == full && (flags & partial) == 0u;
 }
 
-template <bool MSG_BF16, bool GROUPS>
+template <bool MSG_BF16, bool GROUPS, bool LARS>
 static cudaError_t configure_step_pipe()
 {
-    cudaError_t e = cudaFuncSetAttribute(sgp_step_pipe_kernel<MSG_BF16, GROUPS>,
+    cudaError_t e = cudaFuncSetAttribute(sgp_step_pipe_kernel<MSG_BF16, GROUPS, LARS>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, PIPE_SMEM);
     if (e != cudaSuccess) return e;
     // two CTAs x 64 KB per SM: ask for the large shared-memory carve-out (the default one fits
     // a single CTA: launch__occupancy_limit_shared_mem = 1 in the first ncu capture)
-    return cudaFuncSetAttribute(sgp_step_pipe_kernel<MSG_BF16, GROUPS>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                cudaSharedmemCarveoutMaxShared);
+    return cudaFuncSetAttribute(sgp_step_pipe_kernel<MSG_BF16, GROUPS, LARS>,
+                                cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
 }
 
 static cudaError_t configure_step_pipe_all()
 {
-    cudaError_t e = configure_step_pipe<false, false>();
-    if (e == cudaSuccess) e = configure_step_pipe<true, false>();
-    if (e == cudaSuccess) e = configure_step_pipe<false, true>();
-    if (e == cudaSuccess) e = configure_step_pipe<true, true>();
+    cudaError_t e = configure_step_pipe<false, false, false>();
+    if (e == cudaSuccess) e = configure_step_pipe<true, false, false>();
+    if (e == cudaSuccess) e = configure_step_pipe<false, true, false>();
+    if (e == cudaSuccess) e = configure_step_pipe<true, true, false>();
+    if (e == cudaSuccess) e = configure_step_pipe<false, true, true>();
+    if (e == cudaSuccess) e = configure_step_pipe<true, true, true>();
     return e;
 }
 
@@ -1669,27 +1818,42 @@ static bool groups_ok(const SgpArgs* args)
     return args->hyper_groups && args->block_group && args->groups >= 1 && args->groups <= SGP_MAX_GROUPS;
 }
 
+// SGP_F_LARS needs SGP_F_GROUPS (the rows give each tensor's weight decay) and every LARS buffer
+static bool lars_ok(const SgpArgs* args)
+{
+    if (!(args->flags & SGP_F_LARS)) return true;
+    return (args->flags & SGP_F_GROUPS) && groups_ok(args) && args->block_tensor && args->lars_trust &&
+           args->lars_enabled && args->lars_tiles && args->lars_tile_first && args->lars_partials &&
+           args->lars_sumsq && args->lars_tensors >= 1 && args->lars_tensors <= SGP_LARS_MAX_TENSORS &&
+           args->lars_ntiles >= args->lars_tensors;
+}
+
 extern "C" {
 
 cudaError_t sgp_launch_step(const SgpArgs* args, int grid, cudaStream_t stream)
 {
-    if (!msg_bf16_mode_ok(args->flags) || !groups_ok(args)) return cudaErrorInvalidValue;
-    if (args->flags & SGP_F_GROUPS) {
+    if (!msg_bf16_mode_ok(args->flags) || !groups_ok(args) || !lars_ok(args)) return cudaErrorInvalidValue;
+    if (args->flags & SGP_F_LARS) {
         if (args->flags & SGP_F_MSG_BF16)
-            sgp_step_kernel<true, true><<<grid, SGP_THREADS, 0, stream>>>(*args);
+            sgp_step_kernel<true, true, true><<<grid, SGP_THREADS, 0, stream>>>(*args);
         else
-            sgp_step_kernel<false, true><<<grid, SGP_THREADS, 0, stream>>>(*args);
+            sgp_step_kernel<false, true, true><<<grid, SGP_THREADS, 0, stream>>>(*args);
+    } else if (args->flags & SGP_F_GROUPS) {
+        if (args->flags & SGP_F_MSG_BF16)
+            sgp_step_kernel<true, true, false><<<grid, SGP_THREADS, 0, stream>>>(*args);
+        else
+            sgp_step_kernel<false, true, false><<<grid, SGP_THREADS, 0, stream>>>(*args);
     } else if (args->flags & SGP_F_MSG_BF16) {
-        sgp_step_kernel<true, false><<<grid, SGP_THREADS, 0, stream>>>(*args);
+        sgp_step_kernel<true, false, false><<<grid, SGP_THREADS, 0, stream>>>(*args);
     } else {
-        sgp_step_kernel<false, false><<<grid, SGP_THREADS, 0, stream>>>(*args);
+        sgp_step_kernel<false, false, false><<<grid, SGP_THREADS, 0, stream>>>(*args);
     }
     return cudaGetLastError();
 }
 
 cudaError_t sgp_launch_step_pipe(const SgpArgs* args, int grid, cudaStream_t stream)
 {
-    if (!msg_bf16_mode_ok(args->flags) || !groups_ok(args)) return cudaErrorInvalidValue;
+    if (!msg_bf16_mode_ok(args->flags) || !groups_ok(args) || !lars_ok(args)) return cudaErrorInvalidValue;
     static bool configured[64] = {};
     int dev = 0;
     cudaGetDevice(&dev);
@@ -1700,15 +1864,20 @@ cudaError_t sgp_launch_step_pipe(const SgpArgs* args, int grid, cudaStream_t str
     }
     // (the bf16 ring uses half of each stage: the occupancy, and so the grid every rank shares,
     // stays that of the fp32 kernel)
-    if (args->flags & SGP_F_GROUPS) {
+    if (args->flags & SGP_F_LARS) {
         if (args->flags & SGP_F_MSG_BF16)
-            sgp_step_pipe_kernel<true, true><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
+            sgp_step_pipe_kernel<true, true, true><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
         else
-            sgp_step_pipe_kernel<false, true><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
+            sgp_step_pipe_kernel<false, true, true><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
+    } else if (args->flags & SGP_F_GROUPS) {
+        if (args->flags & SGP_F_MSG_BF16)
+            sgp_step_pipe_kernel<true, true, false><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
+        else
+            sgp_step_pipe_kernel<false, true, false><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
     } else if (args->flags & SGP_F_MSG_BF16) {
-        sgp_step_pipe_kernel<true, false><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
+        sgp_step_pipe_kernel<true, false, false><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
     } else {
-        sgp_step_pipe_kernel<false, false><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
+        sgp_step_pipe_kernel<false, false, false><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
     }
     return cudaGetLastError();
 }
@@ -1720,10 +1889,12 @@ int sgp_max_resident_ctas_pipe(int device)
     int sms = 0;
     if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) return 0;
     configure_step_pipe_all();
-    const void* kernels[] = {(const void*)sgp_step_pipe_kernel<false, false>,
-                             (const void*)sgp_step_pipe_kernel<true, false>,
-                             (const void*)sgp_step_pipe_kernel<false, true>,
-                             (const void*)sgp_step_pipe_kernel<true, true>};
+    const void* kernels[] = {(const void*)sgp_step_pipe_kernel<false, false, false>,
+                             (const void*)sgp_step_pipe_kernel<true, false, false>,
+                             (const void*)sgp_step_pipe_kernel<false, true, false>,
+                             (const void*)sgp_step_pipe_kernel<true, true, false>,
+                             (const void*)sgp_step_pipe_kernel<false, true, true>,
+                             (const void*)sgp_step_pipe_kernel<true, true, true>};
     int per_sm = 1 << 30;
     for (const void* k : kernels) {
         int n = 0;
@@ -1731,6 +1902,23 @@ int sgp_max_resident_ctas_pipe(int device)
         if (n < per_sm) per_sm = n;
     }
     return sms * per_sm;
+}
+
+// the two LARS kernels (see sgp_lars_norms_kernel): any grid >= 1 gives the same bits
+cudaError_t sgp_launch_lars_norms(const SgpArgs* args, int grid, cudaStream_t stream)
+{
+    if (!lars_ok(args) || !(args->flags & SGP_F_LARS) || grid < 1) return cudaErrorInvalidValue;
+    sgp_lars_norms_kernel<<<grid, SGP_THREADS, 0, stream>>>(*args);
+    return cudaGetLastError();
+}
+
+cudaError_t sgp_launch_lars_trust(const SgpArgs* args, cudaStream_t stream)
+{
+    if (!lars_ok(args) || !(args->flags & SGP_F_LARS)) return cudaErrorInvalidValue;
+    const int warps_per_cta = SGP_THREADS / 32;
+    const int grid = (args->lars_tensors + warps_per_cta - 1) / warps_per_cta;
+    sgp_lars_trust_kernel<<<grid, SGP_THREADS, 0, stream>>>(*args);
+    return cudaGetLastError();
 }
 
 cudaError_t sgp_launch_gather(const SgpArgs* args, int grid, int pub_grid, cudaStream_t stream)
@@ -1903,11 +2091,14 @@ cudaError_t sgp_launch_slowmo(const SgpArgs* args, float* u, float* x_prev, floa
 cudaError_t sgp_preload_kernels()
 {
     const void* kernels[] = {
-        (const void*)sgp_step_kernel<false, false>, (const void*)sgp_step_kernel<true, false>,
-        (const void*)sgp_step_kernel<false, true>, (const void*)sgp_step_kernel<true, true>,
+        (const void*)sgp_step_kernel<false, false, false>, (const void*)sgp_step_kernel<true, false, false>,
+        (const void*)sgp_step_kernel<false, true, false>, (const void*)sgp_step_kernel<true, true, false>,
+        (const void*)sgp_step_kernel<false, true, true>, (const void*)sgp_step_kernel<true, true, true>,
         (const void*)sgp_gather_kernel, (const void*)sgp_gather_tma_kernel,
-        (const void*)sgp_step_pipe_kernel<false, false>, (const void*)sgp_step_pipe_kernel<true, false>,
-        (const void*)sgp_step_pipe_kernel<false, true>, (const void*)sgp_step_pipe_kernel<true, true>,
+        (const void*)sgp_step_pipe_kernel<false, false, false>, (const void*)sgp_step_pipe_kernel<true, false, false>,
+        (const void*)sgp_step_pipe_kernel<false, true, false>, (const void*)sgp_step_pipe_kernel<true, true, false>,
+        (const void*)sgp_step_pipe_kernel<false, true, true>, (const void*)sgp_step_pipe_kernel<true, true, true>,
+        (const void*)sgp_lars_norms_kernel, (const void*)sgp_lars_trust_kernel,
         (const void*)sgp_probe_kernel, (const void*)sgp_gather_wait_kernel,
         (const void*)sgp_gather_ack_kernel, (const void*)sgp_bilat_decide_kernel, (const void*)sgp_bilat_ctl_kernel,
         (const void*)sgp_allreduce_sgd_kernel, (const void*)sgp_zero_kernel, (const void*)sgp_barrier_kernel,
@@ -1926,12 +2117,16 @@ int sgp_max_resident_ctas(int device)
 {
     int sms = 0, per_sm = 0;
     if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) return 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sgp_step_kernel<false, false>, SGP_THREADS, 0)
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sgp_step_kernel<false, false, false>, SGP_THREADS, 0)
         != cudaSuccess) return 0;
-    int per_sm_groups = 0;      // (the grouped variant is launched on the same grid)
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_groups, sgp_step_kernel<false, true>, SGP_THREADS, 0)
-        != cudaSuccess) return 0;
-    if (per_sm_groups < per_sm) per_sm = per_sm_groups;
+    // (the grouped and LARS variants are launched on the same grid)
+    const void* variants[] = {(const void*)sgp_step_kernel<false, true, false>,
+                              (const void*)sgp_step_kernel<false, true, true>};
+    for (const void* k : variants) {
+        int n = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k, SGP_THREADS, 0) != cudaSuccess) return 0;
+        if (n < per_sm) per_sm = n;
+    }
     return sms * per_sm;
 }
 

@@ -11,10 +11,13 @@ from typing import List, Sequence, Tuple
 import torch
 
 
-def sgd_momentum(x, g, m, lr, momentum, weight_decay, nesterov):
+def sgd_momentum(x, g, m, lr, momentum, weight_decay, nesterov, trust=None):
     """torch.optim.SGD (dampening 0) on the push-sum numerator; returns (x, m).  The
-    hyper-parameters are scalars or per-element tensors (``nesterov`` then a bool tensor)."""
+    hyper-parameters are scalars or per-element tensors (``nesterov`` then a bool tensor).
+    ``trust``: per-element LARS trust ratios, d = trust * (g + wd * x)."""
     d = g + weight_decay * x
+    if trust is not None:
+        d = trust * d
     m = momentum * m + d
     if isinstance(nesterov, torch.Tensor):
         upd = torch.where(nesterov, d + momentum * m, m)

@@ -208,6 +208,32 @@ class GossipEngine(object):
             self.groups = int(groups)
         self._hyper_cache = None
 
+    def set_lars(self, offsets=None, numels=None, enabled=None, trust_coefficient=0.001, eps=1e-8):
+        """LARS on every SGD launch (needs :meth:`set_param_groups`): the arena holds tensors at
+        ``offsets`` (64-element aligned, ascending) of ``numels`` elements; ``enabled[t]`` turns the
+        trust ratio of tensor t on.  Each SGD launch then runs the norm and trust kernels first and
+        scales d = g + wd*x of tensor t by ``lars_trust[t]``.  ``offsets=None`` turns LARS off."""
+        if offsets is None:
+            self.ctx.set_lars(None, None, None)
+            return
+        as_t = lambda v, dt: torch.as_tensor(v, dtype=dt, device='cpu')
+        self.ctx.set_lars(as_t(offsets, torch.int64), as_t(numels, torch.int64), as_t(enabled, torch.uint8),
+                          float(trust_coefficient), float(eps))
+
+    @property
+    def lars(self) -> bool:
+        return self.ctx.lars()
+
+    @property
+    def lars_trust(self) -> Optional[torch.Tensor]:
+        """fp32 [tensors] trust ratios of the last SGD launch (device tensor, rewritten by the next)"""
+        return self.ctx.lars_trust() if self.ctx.lars() else None
+
+    @property
+    def lars_sumsq(self) -> Optional[torch.Tensor]:
+        """fp64 [tensors, 2]: sum x^2 and sum g^2 per tensor as the last SGD launch saw them"""
+        return self.ctx.lars_sumsq() if self.ctx.lars() else None
+
     def set_schedule(self, graph=None, mixing=None):
         """Re-emit the device tables (e.g. after ``peers_per_itr`` changed).
         Collective in effect: callers drain their streams and barrier first."""

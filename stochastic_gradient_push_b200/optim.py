@@ -25,6 +25,15 @@ momentum, weight_decay and nesterov -- e.g. :func:`no_bias_decay_groups`.  Every
 arena tensor starts on a 64-element boundary, so a uint8 map with one entry per
 64-element block names each element's group exactly; the kernels read it next
 to a device table of the groups' values (DESIGN.md 2.0.3).
+
+``lars=True`` (per group, or for all) adds layer-wise adaptive rate scaling (LARS; You, Gitman,
+Ginsburg, 2017) as apex ``LARC(clip=False)`` puts it in front of SGD: every parameter tensor p of
+such a group takes
+
+    t_p = eta |x_p| / (|g_p| + wd |x_p| + eps)   (1 if |x_p| or |g_p| is 0) ;  d = t_p * (g + wd*x)
+
+with x the push-sum numerator the step acts on.  The kernels compute the norms and t on the device
+before every SGD launch (DESIGN.md 2.0.4); :func:`lars_groups` is the MLPerf ResNet-50 recipe.
 """
 
 from __future__ import annotations
@@ -36,6 +45,7 @@ from .ops import oracle
 MAX_GROUPS = 16           # == SGP_MAX_GROUPS (sgp_common.cuh)
 GROUP_BLOCK = 64          # == SGP_GROUP_BLOCK: elements per block-map entry
 _HYPER_KEYS = ('lr', 'momentum', 'weight_decay', 'nesterov')
+LARS_MAX_TENSORS = 65535  # == SGP_LARS_MAX_TENSORS: the block -> tensor map is uint16
 
 
 def no_bias_decay_groups(module, weight_decay):
@@ -47,23 +57,38 @@ def no_bias_decay_groups(module, weight_decay):
             dict(params=[p for p in params if p.dim() > 1], weight_decay=weight_decay)]
 
 
+def lars_groups(module, weight_decay):
+    """The MLPerf ResNet-50 LARS recipe as two parameter groups: every parameter with ``ndim <= 1``
+    (BatchNorm weight and bias, all biases) with ``weight_decay=0`` and ``lars=False``, then
+    everything else with ``weight_decay`` and ``lars=True``."""
+    params = list(module.parameters())
+    return [dict(params=[p for p in params if p.dim() <= 1], weight_decay=0.0, lars=False),
+            dict(params=[p for p in params if p.dim() > 1], weight_decay=weight_decay, lars=True)]
+
+
 class FusedGossipSGD(object):
 
     def __init__(self, model, lr=0.1, momentum=0.0, weight_decay=0.0, nesterov=False,
-                 grad_scale=1.0, param_groups=None):
+                 grad_scale=1.0, param_groups=None, lars=False, trust_coefficient=0.001, lars_eps=1e-8):
         from .parallel.distributed import GossipDataParallel
         assert isinstance(model, GossipDataParallel)
         if nesterov and momentum <= 0:
             raise ValueError('Nesterov momentum requires a momentum')
+        if not trust_coefficient > 0 or not lars_eps >= 0:
+            raise ValueError('LARS needs trust_coefficient > 0 and lars_eps >= 0')
         self.model = model
         self.defaults = dict(lr=lr, momentum=momentum, weight_decay=weight_decay,
-                             nesterov=nesterov, dampening=0)
+                             nesterov=nesterov, dampening=0, lars=bool(lars))
+        self.trust_coefficient = float(trust_coefficient)
+        self.lars_eps = float(lars_eps)
         if param_groups is None:
             self.param_groups = [dict(self.defaults, params=[p for p in model.module.parameters()])]
         else:
             self.param_groups = self._partition(model, param_groups, self.defaults)
-        # one group runs exactly the ungrouped path; several get the block map (_setup_groups)
-        self._grouped = len(self.param_groups) > 1
+        # one group runs exactly the ungrouped path; several, or LARS, get the block map
+        # (_setup_groups)
+        self._lars_flags = None
+        self._grouped = len(self.param_groups) > 1 or self._lars_on()
         self.grad_scale = grad_scale
         self._arenas = model._arenas
         self.grad_flat, self.momentum_flat = {}, {}
@@ -155,6 +180,60 @@ class FusedGossipSGD(object):
         else:
             for dtype, bmap in self._block_group.items():
                 self._elem_group[dtype] = bmap.long().repeat_interleave(GROUP_BLOCK)
+        self._setup_lars()
+
+    def _lars_on(self):
+        return any(g['lars'] for g in self.param_groups)
+
+    def _setup_lars(self):
+        """per-tensor LARS flags of every arena (fixed until load_state_dict changes them); the
+        kernel plane hands the fp32 arena's layout to the engine, which builds its maps and tiles"""
+        m = self.model
+        lars_of = {}
+        for g in self.param_groups:
+            for p in g['params']:
+                lars_of[id(p)] = bool(g['lars'])
+        self._lars_flags = tuple(bool(g['lars']) for g in self.param_groups)
+        self._tensor_lars, self._elem_tensor, self._tensor_group = {}, {}, {}
+        if not self._lars_on():
+            if m._kernel is not None:
+                m._kernel.engine.set_lars(None)
+            return
+        for dtype, arena in self._arenas.items():
+            params = m._params_by_dtype[dtype]
+            if len(params) > LARS_MAX_TENSORS:
+                raise ValueError('LARS supports at most %d tensors per arena, the %s arena holds %d'
+                                 % (LARS_MAX_TENSORS, dtype, len(params)))
+            self._tensor_lars[dtype] = [lars_of[id(p)] for p in params]
+        k = m._kernel
+        if k is not None:
+            arena = self._arenas[torch.float32]
+            k.engine.set_lars(arena.offsets, arena.numels, self._tensor_lars[torch.float32],
+                              self.trust_coefficient, self.lars_eps)
+        else:
+            for dtype, arena in self._arenas.items():
+                idx = torch.full((arena.total,), len(arena.offsets), dtype=torch.long)   # padding: own bin
+                for t, (off, n) in enumerate(zip(arena.offsets, arena.numels)):
+                    idx[off:off + n] = t
+                self._elem_tensor[dtype] = idx
+                bmap = self._block_group[dtype]
+                self._tensor_group[dtype] = [int(bmap[off // GROUP_BLOCK]) for off in arena.offsets]
+
+    def _c10d_trust(self, dtype, x, g):
+        """per-element LARS trust ratios of one arena: fp64 norms of the numerator and of the scaled
+        gradient per tensor, t = eta |x| / (|g| + wd |x| + eps) where the tensor's group has lars=True
+        and both norms are > 0, else 1"""
+        idx = self._elem_tensor[dtype].to(x.device)
+        T = len(self._tensor_lars[dtype])
+        sx = torch.zeros(T + 1, dtype=torch.float64, device=x.device).index_add_(0, idx, x.double() ** 2)
+        sg = torch.zeros(T + 1, dtype=torch.float64, device=x.device).index_add_(0, idx, g.double() ** 2)
+        nx, ng = sx[:T].sqrt(), sg[:T].sqrt()
+        wd = torch.tensor([float(self.param_groups[gi]['weight_decay']) for gi in self._tensor_group[dtype]],
+                          dtype=torch.float64, device=x.device)
+        on = torch.tensor(self._tensor_lars[dtype], device=x.device) & (nx > 0) & (ng > 0)
+        t = torch.where(on, self.trust_coefficient * nx / (ng + wd * nx + self.lars_eps),
+                        torch.ones_like(nx))
+        return torch.cat([t, t.new_ones(1)]).to(x.dtype)[idx]
 
     # -- torch.optim-like surface -------------------------------------------- #
     def _hyper(self):
@@ -207,8 +286,10 @@ class FusedGossipSGD(object):
                     g = g * self.grad_scale
                 if rows is not None:
                     lr, mu, wd, nest = self._c10d_vectors(dtype, rows)
+                trust = self._c10d_trust(dtype, arena.flat, g) if self._lars_flags and any(self._lars_flags) \
+                    else None
                 x, mom = oracle.sgd_momentum(arena.flat, g, self.momentum_flat[dtype],
-                                             lr, mu, wd, nest)
+                                             lr, mu, wd, nest, trust=trust)
                 arena.flat.copy_(x)
                 self.momentum_flat[dtype].copy_(mom)
         self._steps += 1
@@ -229,23 +310,38 @@ class FusedGossipSGD(object):
         self.model._flush_pending()
         groups = [{k: v for k, v in g.items() if k != 'params'} for g in self.param_groups]
         return {'param_groups': groups, 'steps': self._steps,
+                'lars': {'trust_coefficient': self.trust_coefficient, 'eps': self.lars_eps},
                 'momentum': {str(dt): m.detach().cpu().clone()
                              for dt, m in self.momentum_flat.items()}}
 
     def load_state_dict(self, sd):
         """Restores every group's hyper-parameters.  A checkpoint of a one-group optimizer also
         loads into a grouped one: its lr (the schedule's state) goes to every group, and each group
-        keeps its own momentum, weight decay and nesterov."""
+        keeps its own momentum, weight decay and nesterov.  The groups' ``lars`` flags, the trust
+        coefficient and eps are restored too; if they change, the LARS maps are rebuilt (a CUDA graph
+        captured before then has to be captured again)."""
         saved = sd['param_groups']
+        before = (tuple(bool(g['lars']) for g in self.param_groups), self.trust_coefficient, self.lars_eps)
+        if 'lars' in sd:
+            self.trust_coefficient = float(sd['lars']['trust_coefficient'])
+            self.lars_eps = float(sd['lars']['eps'])
         if len(saved) == len(self.param_groups):
             for g, s in zip(self.param_groups, saved):
                 g.update({k: v for k, v in s.items() if k != 'params'})
+                g['lars'] = bool(g.get('lars', False))
         elif len(saved) == 1:
             for g in self.param_groups:
                 g['lr'] = saved[0]['lr']
         else:
             raise ValueError('checkpoint has %d parameter groups, this optimizer %d'
                              % (len(saved), len(self.param_groups)))
+        after = (tuple(bool(g['lars']) for g in self.param_groups), self.trust_coefficient, self.lars_eps)
+        if after != before:
+            if self._grouped:
+                self._setup_lars()
+            else:
+                self._grouped = True
+                self._setup_groups()
         self._steps = sd.get('steps', 0)
         for dt, m in self.momentum_flat.items():
             m.copy_(sd['momentum'][str(dt)])

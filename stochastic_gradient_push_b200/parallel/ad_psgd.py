@@ -584,12 +584,15 @@ class _BilatEngineShim(object):
 
 
 def make_bilat_trainer(model: BilatGossipDataParallel, lr, criterion=None, amp_dtype=None,
-                       use_cuda_graph=True, warmup_iters=3, channels_last=True):
+                       use_cuda_graph=True, warmup_iters=3, channels_last=True, lars=False):
     """AD-PSGD counterpart of :class:`~.trainer.GossipTrainer`: forward + fused loss/accuracy +
     backward are captured ONCE as a CUDA graph; after every replay the gradients are handed to
     the gossip side with :meth:`BilatGossipDataParallel.handoff` (fused SGD on the gossip copy +
     model pull, enqueued on the daemon's stream under its lock).  The bilateral averaging itself
     runs asynchronously on the native daemon's low-priority stream the whole time."""
+    if lars:
+        raise ValueError('LARS is not supported with AD-PSGD: its SGD runs on the gossip daemon\'s '
+                         'copy, outside FusedGossipSGD')
     from .trainer import GossipTrainer
 
     class BilatTrainer(GossipTrainer):

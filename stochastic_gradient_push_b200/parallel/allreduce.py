@@ -188,7 +188,10 @@ class ARTrainer(GossipTrainer):
 
     def __init__(self, model: AllReduceDataParallel, lr, momentum=0.9, weight_decay=1e-4,
                  nesterov=True, criterion=None, amp_dtype=torch.bfloat16, use_cuda_graph=True,
-                 warmup_iters=3, channels_last=True):
+                 warmup_iters=3, channels_last=True, lars=False):
+        if lars:
+            raise ValueError('LARS is not supported by the all-reduce optimizer: its sharded fused step '
+                             'holds 1/n of each tensor, so no rank sees a whole tensor\'s norm')
         self.model = model
         self.ar = model
 

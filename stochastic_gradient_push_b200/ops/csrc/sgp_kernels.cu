@@ -8,11 +8,30 @@
 //   sgp_step_kernel    phase 1: x = z*w ; SGD-momentum ; (+residual) ; publish
 //                      phase 2: acquire in-neighbours' flags ; weighted P2P
 //                               loads ; push-sum weight update ; de-bias ; store
-//   sgp_gather_kernel  Overlap-SGP: residual = sum_k w_k * outbox_k  (side stream)
+//   sgp_step_pipe_kernel   the same full step, warp-specialised: a producer warp feeds phase 2
+//                      through a TMA ring while the consumers run phase 1 (SGP / D-PSGD hot path)
+//   sgp_gather_kernel, sgp_gather_tma_kernel
+//                      Overlap-SGP: residual = sum_k w_k * outbox_k  (side stream)
+//   sgp_gather_wait_kernel, sgp_gather_ack_kernel
+//                      the same gather on a copy engine: flag wait before, bookkeeping after
 //   sgp_probe_kernel   AD-PSGD passive poll ("has my partner published?")
-//   sgp_allreduce_sgd  AR-SGD comparator: one-shot P2P all-reduce fused with SGD
+//   sgp_bilat_decide_kernel, sgp_bilat_ctl_kernel   AD-PSGD round state machine
+//   sgp_allreduce_sgd  AR-SGD comparator: one-shot P2P all-reduce fused with SGD (+ sgp_zero_kernel)
 //   sgp_barrier_kernel device-side barrier over the signal pads
 //   sgp_scale_kernel   flat x *= w  /  x /= w  (ps_numerator / unbias API parity)
+//   sgp_peer_reduce_kernel   dst = scale * sum of flat buffers on peer devices
+//   sgp_snapshot_kernel, sgp_consensus_kernel, sgp_consensus_finalize_kernel
+//                      consensus distance and the push-sum average model
+//   sgp_slowmo_kernel  SlowMo: exact average + slow-momentum update
+//   sgp_lars_norms_kernel, sgp_lars_trust_kernel   LARS trust ratios for the step kernels
+//
+// What several kernels share is written once, ahead of the kernels:
+//   phase1_chunk       phase 1 of both step kernels for one chunk (sgd4, store_z)
+//   TmaRing            the single-producer TMA ring of the gather, consensus and SlowMo kernels
+//   clamped_segments, wait_pub_flags, pub_flags_visible, wait_outbox_acks, outbox_acks_ok,
+//   gather_epilogue    the flag / ack protocol
+// and, ahead of the launchers, for_each_step_variant (the legal instantiations of the step
+// kernels), ensure_dynamic_smem (per-device shared-memory opt-in) and flat_grid.
 #include "sgp_common.cuh"
 
 #include <type_traits>
@@ -49,50 +68,36 @@ __device__ __forceinline__ float4 mul4(float4 a, float s) {
     return make_float4(a.x * s, a.y * s, a.z * s, a.w * s);
 }
 
-// SGD with momentum on the push-sum numerator (torch.optim.SGD semantics,
-// dampening 0): d = g + wd*x ; m = mu*m + d ; x -= lr * (nesterov ? d + mu*m : m)
-__device__ __forceinline__ void sgd1(float& x, float g, float& m, float lr, float mu,
-                                     float wd, float nesterov) {
-    const float d = fmaf(wd, x, g);
-    m = fmaf(mu, m, d);
-    const float upd = (nesterov != 0.f) ? fmaf(mu, m, d) : m;
-    x = fmaf(-lr, upd, x);
+// SGD with momentum on the four lanes of the push-sum numerator (torch.optim.SGD semantics,
+// dampening 0): d = g + wd*x ; m = mu*m + d ; x -= lr * (nesterov ? d + mu*m : m), with the
+// hyper-parameters as one row h = {lr, mu, wd, nesterov}.
+// LARS (SGP_F_LARS): d = t * (g + wd*x), t the trust ratio of the element's tensor.  t == 1 (LARS
+// disabled, zero norms) multiplies exactly, so those elements get the bits of the plain update
+template <bool LARS>
+__device__ __forceinline__ void sgd4(float4& xv, const float4& gv, float4& mv, const float4& h, float t) {
+#define SGP_SGD_LANE(e)                                                        \
+    {                                                                          \
+        float d = fmaf(h.z, xv.e, gv.e);                                       \
+        if constexpr (LARS) d = t * d;                                         \
+        mv.e = fmaf(h.y, mv.e, d);                                             \
+        const float upd = (h.w != 0.f) ? fmaf(h.y, mv.e, d) : mv.e;            \
+        xv.e = fmaf(-h.x, upd, xv.e);                                          \
+    }
+    SGP_SGD_LANE(x) SGP_SGD_LANE(y) SGP_SGD_LANE(z) SGP_SGD_LANE(w)
+#undef SGP_SGD_LANE
+}
+__device__ __forceinline__ float4 hyper_row(const SgpHyper& h) {
+    return make_float4(h.lr, h.momentum, h.weight_decay, h.nesterov);
 }
 
 // SGP_F_GROUPS: the group rows {lr, momentum, weight_decay, nesterov} go to shared memory once
 // per CTA (threads [0, groups) copy one row each; the caller synchronises).  A 16-byte access
 // never straddles a 64-float block, so one block_group byte serves all four lanes of a float4
 __device__ __forceinline__ void load_group_rows(const SgpArgs& a, float4* s_rows, int tid) {
-    if (tid < a.groups) {
-        const SgpHyper h = a.hyper_groups[tid];
-        s_rows[tid] = make_float4(h.lr, h.momentum, h.weight_decay, h.nesterov);
-    }
+    if (tid < a.groups) s_rows[tid] = hyper_row(a.hyper_groups[tid]);
 }
 __device__ __forceinline__ uint32_t block_group_of(const SgpArgs& a, long long i) {
     return __ldg(a.block_group + (i / SGP_GROUP_BLOCK));
-}
-// sgd1 on the four lanes with one set of hyper-parameters (same fmaf order as the ungrouped path)
-__device__ __forceinline__ void sgd4(float4& xv, const float4& gv, float4& mv, const float4& h) {
-    sgd1(xv.x, gv.x, mv.x, h.x, h.y, h.z, h.w);
-    sgd1(xv.y, gv.y, mv.y, h.x, h.y, h.z, h.w);
-    sgd1(xv.z, gv.z, mv.z, h.x, h.y, h.z, h.w);
-    sgd1(xv.w, gv.w, mv.w, h.x, h.y, h.z, h.w);
-}
-
-// SGP_F_LARS: sgd1 with d = t * (g + wd*x), t the trust ratio of the element's tensor.  t == 1
-// (LARS disabled, zero norms) multiplies exactly, so those elements get sgd1's bits
-__device__ __forceinline__ void sgd1_lars(float& x, float g, float& m, float lr, float mu,
-                                          float wd, float nesterov, float t) {
-    const float d = t * fmaf(wd, x, g);
-    m = fmaf(mu, m, d);
-    const float upd = (nesterov != 0.f) ? fmaf(mu, m, d) : m;
-    x = fmaf(-lr, upd, x);
-}
-__device__ __forceinline__ void sgd4_lars(float4& xv, const float4& gv, float4& mv, const float4& h, float t) {
-    sgd1_lars(xv.x, gv.x, mv.x, h.x, h.y, h.z, h.w, t);
-    sgd1_lars(xv.y, gv.y, mv.y, h.x, h.y, h.z, h.w, t);
-    sgd1_lars(xv.z, gv.z, mv.z, h.x, h.y, h.z, h.w, t);
-    sgd1_lars(xv.w, gv.w, mv.w, h.x, h.y, h.z, h.w, t);
 }
 // trust ratio of the tensor that owns the 64-float block of element i (written by
 // sgp_lars_trust_kernel earlier on the stream, so the read-only path is safe)
@@ -110,6 +115,296 @@ __device__ __forceinline__ bool cta_done_is_last(SgpState* st) {
         return true;
     }
     return false;
+}
+
+// ---- chunk decomposition ----------------------------------------------------
+// CTA b of a grid owns chunks b, b + G, b + 2G, ... of `nchunks`: how many that is
+__device__ __forceinline__ long long cta_chunks(long long nchunks, int b) {
+    return (nchunks > b) ? (nchunks - 1 - b) / gridDim.x + 1 : 0;
+}
+// Thread `tid` makes SGP_UNROLL 16-byte accesses to chunk c, SGP_THREADS * SGP_VEC elements apart:
+// chunk_base is the first one's element, chunk_elem(base, u) the u-th one's
+__device__ __forceinline__ long long chunk_base(long long c, int tid) {
+    return c * SGP_CHUNK + (long long)tid * SGP_VEC;
+}
+__device__ __forceinline__ long long chunk_elem(long long base, int u) {
+    return base + (long long)u * SGP_THREADS * SGP_VEC;
+}
+// de-biased parameters and, with SGP_F_SHADOW, their bf16 copy
+__device__ __forceinline__ void store_z(const SgpArgs& a, uint32_t flags, long long i, const float4& zv) {
+    st_f4(reinterpret_cast<float4*>(a.z + i), zv);
+    if (flags & SGP_F_SHADOW) st_u2(reinterpret_cast<uint2*>(a.shadow + i), f4_to_bf16x4(zv));
+}
+
+// ---- phase 1 of the step kernels, one chunk -----------------------------------
+// All SGP_UNROLL loads first, then per access: x = z * wmul ; SGD (clearing the gradient with
+// SGP_F_ZERO_GRAD) ; + rscale * residual ; publish ; z = x / w1.
+// MSG_BF16: publish Q(x) = bf16(x) and keep what was not sent, c = x - (1 - self_w) Q(x), in z.
+// FULL_STEP (sgp_step_pipe_kernel: always PHASE1 | PUBLISH | PHASE2, never FOLD_RES) compiles the
+// residual fold, the test of SGP_F_PUBLISH and the z store out; rscale, inv_w1 and write_z are
+// then unused.  Ranks of one job may run either step kernel, so both must get these bits.
+template <bool MSG_BF16, bool GROUPS, bool LARS, bool FULL_STEP>
+__device__ __forceinline__ void phase1_chunk(
+    const SgpArgs& a, const uint32_t flags, const long long c, const int tid, const SgpHyper& hp,
+    const bool do_sgd, const float4* s_rows, const float wmul, const float self_w,
+    typename std::conditional<MSG_BF16, __nv_bfloat16, float>::type* my_out, const uint64_t pol_first,
+    const uint64_t pol_last, const float rscale, const float inv_w1, const bool write_z)
+{
+    const bool fold = !FULL_STEP && (flags & SGP_F_FOLD_RES);
+    const long long base = chunk_base(c, tid);
+    float4 x[SGP_UNROLL], g[SGP_UNROLL], m[SGP_UNROLL], r[SGP_UNROLL];
+    uint32_t grp[SGP_UNROLL];
+    float tr[SGP_UNROLL];
+#pragma unroll
+    for (int u = 0; u < SGP_UNROLL; ++u) {
+        const long long i = chunk_elem(base, u);
+        x[u] = ld_once_f4(reinterpret_cast<const float4*>(a.z + i), pol_first);
+        if (do_sgd) {
+            if (flags & SGP_F_GRAD_BF16)
+                g[u] = bf16x4_to_f4(ld_once_u2(reinterpret_cast<const uint2*>(
+                           reinterpret_cast<const __nv_bfloat16*>(a.g) + i), pol_first));
+            else
+                g[u] = ld_once_f4(reinterpret_cast<const float4*>(
+                           reinterpret_cast<const float*>(a.g) + i), pol_first);
+            if (a.g2 != nullptr) {
+                const float4 h = ld_once_f4(reinterpret_cast<const float4*>(a.g2 + i), pol_first);
+                g[u].x += h.x; g[u].y += h.y; g[u].z += h.z; g[u].w += h.w;
+            }
+            m[u] = ld_once_f4(reinterpret_cast<const float4*>(a.m + i), pol_first);
+            if constexpr (GROUPS) grp[u] = block_group_of(a, i);
+            if constexpr (LARS) tr[u] = lars_trust_of(a, i);
+        }
+        if (fold) r[u] = ld_once_f4(reinterpret_cast<const float4*>(a.residual + i), pol_first);
+    }
+#pragma unroll
+    for (int u = 0; u < SGP_UNROLL; ++u) {
+        const long long i = chunk_elem(base, u);
+        float4 xv = mul4(x[u], wmul);               // numerator (exact if w == 1)
+        if (do_sgd) {
+            const float4 gv = mul4(g[u], hp.grad_scale);
+            float4 mv = m[u];
+            float t = 1.f;
+            if constexpr (LARS) t = tr[u];
+            if constexpr (GROUPS) sgd4<LARS>(xv, gv, mv, s_rows[grp[u]], t);
+            else                  sgd4<LARS>(xv, gv, mv, hyper_row(hp), t);
+            st_f4(reinterpret_cast<float4*>(a.m + i), mv);
+            if (flags & SGP_F_ZERO_GRAD) {
+                if (flags & SGP_F_GRAD_BF16)
+                    st_u2(reinterpret_cast<uint2*>(
+                              reinterpret_cast<__nv_bfloat16*>(a.g) + i), make_uint2(0u, 0u));
+                else
+                    st_f4(reinterpret_cast<float4*>(reinterpret_cast<float*>(a.g) + i),
+                          make_float4(0.f, 0.f, 0.f, 0.f));
+                if (a.g2 != nullptr)
+                    st_f4(reinterpret_cast<float4*>(a.g2 + i), make_float4(0.f, 0.f, 0.f, 0.f));
+            }
+        }
+        if (fold)      // (rscale: 1 after a gather kernel, the edge weight after a DMA gather)
+            xv = fma4(r[u], rscale, xv);
+        if constexpr (MSG_BF16) {
+            const uint2 q = f4_to_bf16x4(xv);
+            st_hint_u2(reinterpret_cast<uint2*>(my_out + i), q, pol_last);
+            st_hint_f4(reinterpret_cast<float4*>(a.z + i), fma4(bf16x4_to_f4(q), self_w - 1.f, xv), pol_last);
+        } else if (FULL_STEP || (flags & SGP_F_PUBLISH)) {   // keep the outbox in L2 for phase 2 / peers
+            st_hint_f4(reinterpret_cast<float4*>(my_out + i), xv, pol_last);
+        }
+        if (!FULL_STEP && write_z) store_z(a, flags, i, mul4(xv, inv_w1));
+    }
+}
+
+// ---- mbarrier / bulk-copy (TMA) helpers ---------------------------------------
+#define SGP_TMA_BYTES  (SGP_CHUNK * 4)      // one 4096-float chunk = 16 KB per stage
+
+__device__ __forceinline__ uint32_t smem_u32(const void* p) {
+    return static_cast<uint32_t>(__cvta_generic_to_shared(p));
+}
+__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(smem_u32(bar)), "r"(count));
+}
+__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;"
+                 :: "r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "WAIT_%=:\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+        "@p bra DONE_%=;\n\t"
+        "bra WAIT_%=;\n\t"
+        "DONE_%=:\n\t}"
+        :: "r"(smem_u32(bar)), "r"(parity) : "memory");
+}
+__device__ __forceinline__ void tma_load_1d(void* smem_dst, const void* gmem_src, uint32_t bytes,
+                                            uint64_t* bar) {
+    asm volatile(
+        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+        :: "r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
+
+// ---- single-producer TMA ring ---------------------------------------------------
+// The snapshot readers (TMA gather, consensus, SlowMo) should saturate NVLink from few SMs.
+// Register-staged loads need ~300 CTAs of in-flight 16-byte requests to cover the ~2 us NVLink
+// latency; here thread 0 of the CTA keeps a ring of SGP_RING_STAGES x 16 KB bulk copies
+// (cp.async.bulk, global[peer] -> shared, mbarrier complete_tx) in flight, i.e. ~100 KB per CTA
+// instead of ~16 KB, and the whole CTA only touches a chunk once it has landed in shared memory.
+// The CTA's work is a sequence of items 0, 1, 2, ..., one fp32 chunk each; item i uses stage
+// i % STAGES, and `src_of(item)` gives the chunk's global address.
+#define SGP_RING_STAGES 6
+#define SGP_RING_SMEM   (SGP_RING_STAGES * SGP_TMA_BYTES + SGP_RING_STAGES * 8 + 64)
+
+struct TmaRing {
+    float*    data;                                   // [STAGES][CHUNK]
+    uint64_t* full;                                   // [STAGES] "the stage's copy has landed"
+
+    // smem: the kernel's dynamic shared memory (SGP_RING_SMEM bytes, 128-byte aligned)
+    __device__ __forceinline__ explicit TmaRing(unsigned char* smem)
+        : data(reinterpret_cast<float*>(smem)),
+          full(reinterpret_cast<uint64_t*>(smem + SGP_RING_STAGES * SGP_TMA_BYTES)) {}
+
+    // thread 0, followed by a block barrier before anything else touches the ring
+    __device__ __forceinline__ void init() const {
+        for (int i = 0; i < SGP_RING_STAGES; ++i) mbar_init(&full[i], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __device__ __forceinline__ void issue(long long item, const float* src) const {
+        const int stage = (int)(item % SGP_RING_STAGES);
+        mbar_expect_tx(&full[stage], SGP_TMA_BYTES);
+        tma_load_1d(data + (size_t)stage * SGP_CHUNK, src, SGP_TMA_BYTES, &full[stage]);
+    }
+    // thread 0: start the first STAGES items
+    template <class SrcOf>
+    __device__ __forceinline__ void fill(long long items, SrcOf&& src_of) const {
+        for (long long i = 0; i < items && i < SGP_RING_STAGES; ++i) issue(i, src_of(i));
+    }
+    // every thread: wait until `item` has landed; returns its chunk
+    __device__ __forceinline__ const float4* wait(long long item) const {
+        const int stage = (int)(item % SGP_RING_STAGES);
+        mbar_wait(&full[stage], (uint32_t)((item / SGP_RING_STAGES) & 1));
+        return reinterpret_cast<const float4*>(data + (size_t)stage * SGP_CHUNK);
+    }
+    // every thread, after its last read of `item`: once the whole block is done with the stage,
+    // thread 0 refills it with item + STAGES
+    template <class SrcOf>
+    __device__ __forceinline__ void refill(long long item, long long items, SrcOf&& src_of) const {
+        __syncthreads();
+        if (threadIdx.x == 0 && item + SGP_RING_STAGES < items) {
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads -> async write
+            issue(item + SGP_RING_STAGES, src_of(item + SGP_RING_STAGES));
+        }
+    }
+};
+
+// Factors of the weighted running mean over the ranks' snapshots (consensus, SlowMo):
+// f[j] = w_j / W_j with W_j = w_0 + .. + w_j, so that zbar_j = zbar_{j-1} + f[j] (z_j - zbar_{j-1}).
+// One thread; the same operations in the same order wherever it is called, so every kernel and
+// every rank forms zbar with the same bits
+__device__ __forceinline__ void running_mean_factors(const SgpArgs& a, float* f) {
+    float wsum = 0.f;
+    for (int j = 0; j < a.world; ++j) {
+        const float wj = ld_relaxed_sys_f32(&a.pads[j]->snap_w);
+        wsum += wj;
+        f[j] = wj / wsum;
+    }
+}
+
+// ---- flag / ack protocol ----------------------------------------------------------
+// pub_seq counts segments within a step, so at most SGP_SEQ_STRIDE - 1 of them
+__device__ __forceinline__ int clamped_segments(const SgpArgs& a) {
+    int segs = a.segments < 1 ? 1 : a.segments;
+    if (segs > SGP_SEQ_STRIDE - 1) segs = SGP_SEQ_STRIDE - 1;
+    return segs;
+}
+
+// The whole block waits until ALL pub_grid publish flags of every in-neighbour of `row` have
+// reached `want` (block-parallel poll, heartbeat timeout).  Returns false in every thread when a
+// wait gave up.  Its first barrier also orders what thread 0 initialised before the call
+__device__ __forceinline__ bool wait_pub_flags(const SgpArgs& a, const RowInfo& row, uint32_t want, int pub_grid) {
+    __shared__ int s_ok;
+    if (threadIdx.x == 0) s_ok = 1;
+    __syncthreads();
+    for (int k = 0; k < row.n_in; ++k) {
+        const int j = row.in[k];
+        if (j < 0) continue;
+        const SgpSignalPad* pj = a.pads[j];
+        for (int f = threadIdx.x; f < pub_grid; f += blockDim.x)
+            if (!spin_wait_geq(&pj->pub_seq[f], want, a.st, a.timeout_ns, SGP_ERR_TIMEOUT_PUB))
+                s_ok = 0;
+    }
+    __syncthreads();
+    return s_ok != 0;
+}
+
+// The same question without waiting: one look at every flag.  Returns the answer in every thread;
+// ends with a barrier, so it may be called again at once
+__device__ __forceinline__ bool pub_flags_visible(const SgpArgs& a, const RowInfo& row, uint32_t want, int pub_grid) {
+    __shared__ int s_all;
+    if (threadIdx.x == 0) s_all = 1;
+    __syncthreads();
+    for (int k = 0; k < row.n_in; ++k) {
+        const int j = row.in[k];
+        if (j < 0) continue;
+        for (int f = threadIdx.x; f < pub_grid; f += blockDim.x)
+            if ((int32_t)(ld_acquire_sys(&a.pads[j]->pub_seq[f]) - want) < 0) s_all = 0;
+    }
+    __syncthreads();
+    const bool all = s_all != 0;
+    __syncthreads();
+    return all;
+}
+
+// WAR fence of the outbox: outbox[step & 1] was last read at step - 2 by that step's
+// out-neighbours, and may be overwritten once each of them has acked (ack_seq >= step - 1).
+// That holds from step ack_from + 2 on (outbox_was_read); before, there is nothing to wait for.
+// One thread: wait_outbox_acks spins (heartbeat timeout -> false), outbox_acks_ok looks once
+__device__ __forceinline__ bool outbox_was_read(const SgpArgs& a, uint32_t step) {
+    return step >= a.st->ack_from + 2u;
+}
+__device__ __forceinline__ bool wait_outbox_acks(const SgpArgs& a, uint32_t step) {
+    RowInfo prev;
+    load_row(a, step - 2u, prev);
+    int ok = 1;
+    for (int k = 0; k < prev.n_out; ++k) {
+        const int o = prev.out[k];
+        if (o == a.rank || o < 0) continue;
+        ok &= spin_wait_geq(&a.pads[a.rank]->ack_seq[o], step - 1u, a.st, a.timeout_ns,
+                            SGP_ERR_TIMEOUT_ACK) ? 1 : 0;
+    }
+    return ok != 0;
+}
+__device__ __forceinline__ bool outbox_acks_ok(const SgpArgs& a, uint32_t step) {
+    RowInfo prev;
+    load_row(a, step - 2u, prev);
+    bool ok = true;
+    for (int k = 0; k < prev.n_out; ++k) {
+        const int o = prev.out[k];
+        if (o < 0 || o == a.rank) continue;
+        if ((int32_t)(ld_acquire_sys(&a.pads[a.rank]->ack_seq[o]) - (step - 1u)) < 0) ok = false;
+    }
+    return ok;
+}
+
+// End of a gather of step s, one thread: the residual's push-sum weight, the factor the next
+// publish folds it with, and the acks that release the in-neighbours' outboxes.  ok = false (a
+// publish flag never came) leaves an empty residual.
+// dma: a copy engine brought the raw outbox of the single in-neighbour, so the factor is that
+// edge's weight; otherwise a gather kernel already applied the weights and resets done_ctas
+__device__ __forceinline__ void gather_epilogue(const SgpArgs& a, const RowInfo& row, uint32_t s, bool ok, bool dma) {
+    float wr = 0.f, scale = dma ? 0.f : 1.f;
+    for (int k = 0; k < row.n_in; ++k) {
+        const int j = row.in[k];
+        if (j < 0) continue;
+        if (dma) scale = row.in_w[k];               // (single in-neighbour: enforced by the host)
+        wr = fmaf(row.in_w[k], ld_relaxed_sys_f32(&a.pads[j]->psw[s & 1u]), wr);
+        if (j != a.rank) st_release_sys(&a.pads[j]->ack_seq[a.rank], s + 1u);
+    }
+    *((volatile float*)&a.st->res_weight) = ok ? wr : 0.f;
+    *((volatile float*)&a.st->res_scale) = (ok || !dma) ? scale : 0.f;
+    if (!dma) *((volatile uint32_t*)&a.st->done_ctas) = 0u;
+    __threadfence();
 }
 
 }  // namespace
@@ -175,26 +470,12 @@ sgp_step_kernel(const SgpArgs a)
     // CTAs sharing an SM drift apart, so one CTA's NVLink phase overlaps another's
     // HBM phase and the kernel approaches max(HBM time, NVLink time) instead of
     // their sum; the own-term re-read of phase 2 always hits L2.
-    const long long my_chunks = (nchunks > b) ? (nchunks - 1 - b) / gridDim.x + 1 : 0;
-    int K = a.segments < 1 ? 1 : a.segments;
-    if (K > SGP_SEQ_STRIDE - 1) K = SGP_SEQ_STRIDE - 1;
+    const long long my_chunks = cta_chunks(nchunks, b);
+    const int K = clamped_segments(a);
     const uint32_t seq_base = step * (uint32_t)SGP_SEQ_STRIDE;
 
-    if ((flags & SGP_F_PHASE1) && (flags & SGP_F_PUBLISH) && step >= st->ack_from + 2u) {
-        // WAR fence: outbox[parity] was last read at step-2 by that step's
-        // out-neighbours; wait for their acks before overwriting it.
-        if (tid == 0) {
-            RowInfo prev;
-            load_row(a, step - 2u, prev);
-            int ok = 1;
-            for (int k = 0; k < prev.n_out; ++k) {
-                const int o = prev.out[k];
-                if (o == a.rank || o < 0) continue;
-                ok &= spin_wait_geq(&mypad->ack_seq[o], step - 1u, st, a.timeout_ns,
-                                    SGP_ERR_TIMEOUT_ACK) ? 1 : 0;
-            }
-            s_ok = ok;
-        }
+    if ((flags & SGP_F_PHASE1) && (flags & SGP_F_PUBLISH) && outbox_was_read(a, step)) {
+        if (tid == 0) s_ok = wait_outbox_acks(a, step) ? 1 : 0;      // before overwriting outbox[parity]
         __syncthreads();
     }
 
@@ -217,84 +498,10 @@ sgp_step_kernel(const SgpArgs a)
 
         // ---------------- phase 1: local update + publish ------------------
         if (flags & SGP_F_PHASE1) {
-            for (long long it = it_lo; it < it_hi; ++it) {
-                const long long c = b + it * gridDim.x;
-                const long long base = c * SGP_CHUNK + (long long)tid * SGP_VEC;
-                float4 x[SGP_UNROLL], g[SGP_UNROLL], m[SGP_UNROLL], r[SGP_UNROLL];
-                uint32_t grp[SGP_UNROLL];
-                float tr[SGP_UNROLL];
-#pragma unroll
-                for (int u = 0; u < SGP_UNROLL; ++u) {
-                    const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
-                    x[u] = ld_once_f4(reinterpret_cast<const float4*>(a.z + i), pol_first);
-                    if (do_sgd) {
-                        if (flags & SGP_F_GRAD_BF16)
-                            g[u] = bf16x4_to_f4(ld_once_u2(reinterpret_cast<const uint2*>(
-                                       reinterpret_cast<const __nv_bfloat16*>(a.g) + i), pol_first));
-                        else
-                            g[u] = ld_once_f4(reinterpret_cast<const float4*>(
-                                       reinterpret_cast<const float*>(a.g) + i), pol_first);
-                        if (a.g2 != nullptr) {
-                            const float4 h = ld_once_f4(reinterpret_cast<const float4*>(a.g2 + i), pol_first);
-                            g[u].x += h.x; g[u].y += h.y; g[u].z += h.z; g[u].w += h.w;
-                        }
-                        m[u] = ld_once_f4(reinterpret_cast<const float4*>(a.m + i), pol_first);
-                        if constexpr (GROUPS) grp[u] = block_group_of(a, i);
-                        if constexpr (LARS) tr[u] = lars_trust_of(a, i);
-                    }
-                    if (flags & SGP_F_FOLD_RES)
-                        r[u] = ld_once_f4(reinterpret_cast<const float4*>(a.residual + i), pol_first);
-                }
-#pragma unroll
-                for (int u = 0; u < SGP_UNROLL; ++u) {
-                    const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
-                    float4 xv = mul4(x[u], wmul);               // numerator (exact if w == 1)
-                    if (do_sgd) {
-                        float4 gv = mul4(g[u], hp.grad_scale);
-                        float4 mv = m[u];
-                        if constexpr (LARS) {
-                            sgd4_lars(xv, gv, mv, s_rows[grp[u]], tr[u]);
-                        } else if constexpr (GROUPS) {
-                            sgd4(xv, gv, mv, s_rows[grp[u]]);
-                        } else {
-                            sgd1(xv.x, gv.x, mv.x, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
-                            sgd1(xv.y, gv.y, mv.y, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
-                            sgd1(xv.z, gv.z, mv.z, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
-                            sgd1(xv.w, gv.w, mv.w, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
-                        }
-                        st_f4(reinterpret_cast<float4*>(a.m + i), mv);
-                        if (flags & SGP_F_ZERO_GRAD) {
-                            if (flags & SGP_F_GRAD_BF16)
-                                st_u2(reinterpret_cast<uint2*>(
-                                          reinterpret_cast<__nv_bfloat16*>(a.g) + i), make_uint2(0u, 0u));
-                            else
-                                st_f4(reinterpret_cast<float4*>(reinterpret_cast<float*>(a.g) + i),
-                                      make_float4(0.f, 0.f, 0.f, 0.f));
-                            if (a.g2 != nullptr)
-                                st_f4(reinterpret_cast<float4*>(a.g2 + i), make_float4(0.f, 0.f, 0.f, 0.f));
-                        }
-                    }
-                    if (flags & SGP_F_FOLD_RES) {      // (rscale: 1 after a gather kernel, the edge weight after a DMA gather)
-                        xv.x = fmaf(r[u].x, rscale, xv.x); xv.y = fmaf(r[u].y, rscale, xv.y);
-                        xv.z = fmaf(r[u].z, rscale, xv.z); xv.w = fmaf(r[u].w, rscale, xv.w);
-                    }
-                    if constexpr (MSG_BF16) {
-                        // publish Q(x); z keeps what was not sent: c = x - (1 - self_w) Q(x)
-                        const uint2 q = f4_to_bf16x4(xv);
-                        st_hint_u2(reinterpret_cast<uint2*>(my_out + i), q, pol_last);
-                        st_hint_f4(reinterpret_cast<float4*>(a.z + i),
-                                   fma4(bf16x4_to_f4(q), row.self_w - 1.f, xv), pol_last);
-                    } else if (flags & SGP_F_PUBLISH) {   // keep the outbox in L2 for phase 2 / peers
-                        st_hint_f4(reinterpret_cast<float4*>(my_out + i), xv, pol_last);
-                    }
-                    if (write_z) {
-                        const float4 zv = mul4(xv, inv_w1);
-                        st_f4(reinterpret_cast<float4*>(a.z + i), zv);
-                        if (flags & SGP_F_SHADOW)
-                            st_u2(reinterpret_cast<uint2*>(a.shadow + i), f4_to_bf16x4(zv));
-                    }
-                }
-            }
+            for (long long it = it_lo; it < it_hi; ++it)
+                phase1_chunk<MSG_BF16, GROUPS, LARS, false>(a, flags, b + it * gridDim.x, tid, hp, do_sgd, s_rows,
+                                                            wmul, row.self_w, my_out, pol_first, pol_last,
+                                                            rscale, inv_w1, write_z);
             if (flags & SGP_F_PUBLISH) {
                 __syncthreads();
                 if (tid == 0) {
@@ -330,12 +537,12 @@ sgp_step_kernel(const SgpArgs a)
             if (pull_ok) {
                 for (long long it = it_lo; it < it_hi; ++it) {
                     const long long c = b + it * gridDim.x;
-                    const long long base = c * SGP_CHUNK + (long long)tid * SGP_VEC;
+                    const long long base = chunk_base(c, tid);
                     float4 acc[SGP_UNROLL];
                     float4 pv[SGP_UNROLL];
 #pragma unroll
                     for (int u = 0; u < SGP_UNROLL; ++u) {
-                        const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
+                        const long long i = chunk_elem(base, u);
                         if constexpr (MSG_BF16) {
                             // own term: c, kept in z by phase 1 (already carries the self weight)
                             acc[u] = ld_once_f4(reinterpret_cast<const float4*>(a.z + i), pol_first);
@@ -354,7 +561,7 @@ sgp_step_kernel(const SgpArgs a)
                         if (po == nullptr) continue;
 #pragma unroll
                         for (int u = 0; u < SGP_UNROLL; ++u) {
-                            const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
+                            const long long i = chunk_elem(base, u);
                             if constexpr (MSG_BF16)
                                 pv[u] = bf16x4_to_f4(ld_stream_u2(reinterpret_cast<const uint2*>(po + i)));
                             else
@@ -366,11 +573,9 @@ sgp_step_kernel(const SgpArgs a)
                     }
 #pragma unroll
                     for (int u = 0; u < SGP_UNROLL; ++u) {
-                        const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
+                        const long long i = chunk_elem(base, u);
                         const float4 zv = mul4(acc[u], inv_wn);
-                        st_f4(reinterpret_cast<float4*>(a.z + i), zv);
-                        if (flags & SGP_F_SHADOW)
-                            st_u2(reinterpret_cast<uint2*>(a.shadow + i), f4_to_bf16x4(zv));
+                        store_z(a, flags, i, zv);
                     }
                 }
             }
@@ -385,15 +590,13 @@ sgp_step_kernel(const SgpArgs a)
                 if constexpr (MSG_BF16) own = a.z; else own = my_out;
                 for (long long it = it_lo; it < it_hi; ++it) {
                     const long long c = b + it * gridDim.x;
-                    const long long base = c * SGP_CHUNK + (long long)tid * SGP_VEC;
+                    const long long base = chunk_base(c, tid);
 #pragma unroll
                     for (int u = 0; u < SGP_UNROLL; ++u) {
-                        const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
+                        const long long i = chunk_elem(base, u);
                         const float4 zv = mul4(ld_once_f4(reinterpret_cast<const float4*>(own + i), pol_first),
                                                inv_own);
-                        st_f4(reinterpret_cast<float4*>(a.z + i), zv);
-                        if (flags & SGP_F_SHADOW)
-                            st_u2(reinterpret_cast<uint2*>(a.shadow + i), f4_to_bf16x4(zv));
+                        store_z(a, flags, i, zv);
                     }
                 }
             }
@@ -436,7 +639,6 @@ sgp_step_kernel(const SgpArgs a)
 __global__ void __launch_bounds__(SGP_THREADS, 2)
 sgp_gather_kernel(const SgpArgs a, const int pub_grid)
 {
-    __shared__ int s_ok;
     SgpState* st = a.st;
     const uint32_t s      = *((volatile uint32_t*)&st->step) - 1u;
     const uint32_t parity = s & 1u;
@@ -445,31 +647,16 @@ sgp_gather_kernel(const SgpArgs a, const int pub_grid)
 
     RowInfo row;
     load_row(a, s, row);
-    int segs = a.segments < 1 ? 1 : a.segments;
-    if (segs > SGP_SEQ_STRIDE - 1) segs = SGP_SEQ_STRIDE - 1;
+    const bool ok = wait_pub_flags(a, row, s * (uint32_t)SGP_SEQ_STRIDE + (uint32_t)clamped_segments(a), pub_grid);
 
-    // every CTA waits for ALL publisher CTAs of every in-neighbour (block-parallel poll)
-    if (tid == 0) s_ok = 1;
-    __syncthreads();
-    for (int k = 0; k < row.n_in; ++k) {
-        const int j = row.in[k];
-        if (j < 0) continue;
-        const SgpSignalPad* pj = a.pads[j];
-        for (int f = tid; f < pub_grid; f += SGP_THREADS)
-            if (!spin_wait_geq(&pj->pub_seq[f], s * (uint32_t)SGP_SEQ_STRIDE + (uint32_t)segs, st,
-                               a.timeout_ns, SGP_ERR_TIMEOUT_PUB))
-                s_ok = 0;
-    }
-    __syncthreads();
-
-    if (s_ok) {
+    if (ok) {
         const float* peer_out[SGP_MAX_PEERS];
 #pragma unroll
         for (int k = 0; k < SGP_MAX_PEERS; ++k)
             peer_out[k] = (k < row.n_in && row.in[k] >= 0)
                               ? a.outboxes[row.in[k]] + (size_t)parity * a.n : nullptr;
         for (long long c = blockIdx.x; c < nchunks; c += gridDim.x) {
-            const long long base = c * SGP_CHUNK + (long long)tid * SGP_VEC;
+            const long long base = chunk_base(c, tid);
             float4 acc[SGP_UNROLL], pv[SGP_UNROLL];
 #pragma unroll
             for (int u = 0; u < SGP_UNROLL; ++u) acc[u] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -478,80 +665,30 @@ sgp_gather_kernel(const SgpArgs a, const int pub_grid)
                 if (po == nullptr) continue;
 #pragma unroll
                 for (int u = 0; u < SGP_UNROLL; ++u)
-                    pv[u] = ld_stream_f4(reinterpret_cast<const float4*>(
-                                po + base + (long long)u * SGP_THREADS * SGP_VEC));
+                    pv[u] = ld_stream_f4(reinterpret_cast<const float4*>(po + chunk_elem(base, u)));
 #pragma unroll
                 for (int u = 0; u < SGP_UNROLL; ++u) acc[u] = fma4(pv[u], row.in_w[k], acc[u]);
             }
 #pragma unroll
             for (int u = 0; u < SGP_UNROLL; ++u)
-                st_f4(reinterpret_cast<float4*>(a.residual + base +
-                                                (long long)u * SGP_THREADS * SGP_VEC), acc[u]);
+                st_f4(reinterpret_cast<float4*>(a.residual + chunk_elem(base, u)), acc[u]);
         }
     }
 
     __syncthreads();
-    if (tid == 0 && cta_done_is_last(st)) {
-        float wr = 0.f;
-        for (int k = 0; k < row.n_in; ++k) {
-            const int j = row.in[k];
-            if (j < 0) continue;
-            wr = fmaf(row.in_w[k], ld_relaxed_sys_f32(&a.pads[j]->psw[parity]), wr);
-            if (j != a.rank) st_release_sys(&a.pads[j]->ack_seq[a.rank], s + 1u);
-        }
-        *((volatile float*)&st->res_weight) = s_ok ? wr : 0.f;
-        *((volatile float*)&st->res_scale) = 1.f;
-        *((volatile uint32_t*)&st->done_ctas) = 0u;
-        __threadfence();
-    }
+    if (tid == 0 && cta_done_is_last(st)) gather_epilogue(a, row, s, ok, false);
 }
 
 // ---------------------------------------------------------------------------
 // Overlap-SGP gather, TMA variant.  The gather runs on a side stream next to the
-// forward/backward pass, so it should saturate NVLink from as FEW SMs as possible.
-// Register-staged loads need ~300 CTAs of in-flight 16-byte requests to cover the
-// ~2 us NVLink latency; here one elected thread per CTA keeps a ring of
-// SGP_TMA_STAGES x 16 KB bulk copies (cp.async.bulk, global[peer] -> shared,
-// mbarrier complete_tx) in flight, i.e. ~100 KB per CTA instead of ~16 KB, and the
-// whole CTA only touches the data once it has landed in shared memory.
+// forward/backward pass, so it should saturate NVLink from as FEW SMs as possible: the peers'
+// chunks come through the TmaRing; items are (chunk, in-peer) pairs, peer fastest.
 // ---------------------------------------------------------------------------
-#define SGP_TMA_STAGES 6
-#define SGP_TMA_BYTES  (SGP_CHUNK * 4)      // one 4096-float chunk = 16 KB per stage
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-    return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;"
-                 :: "r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "WAIT_%=:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra DONE_%=;\n\t"
-        "bra WAIT_%=;\n\t"
-        "DONE_%=:\n\t}"
-        :: "r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_load_1d(void* smem_dst, const void* gmem_src, uint32_t bytes,
-                                            uint64_t* bar) {
-    asm volatile(
-        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-        :: "r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-
 __global__ void __launch_bounds__(SGP_THREADS, 1)
 sgp_gather_tma_kernel(const SgpArgs a, const int pub_grid)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    float* ring = reinterpret_cast<float*>(smem_raw);                       // [STAGES][CHUNK]
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + SGP_TMA_STAGES * SGP_TMA_BYTES);
-    __shared__ int s_ok;
+    const TmaRing ring(smem_raw);
 
     SgpState* st = a.st;
     const uint32_t s      = *((volatile uint32_t*)&st->step) - 1u;
@@ -561,50 +698,25 @@ sgp_gather_tma_kernel(const SgpArgs a, const int pub_grid)
 
     RowInfo row;
     load_row(a, s, row);
-    int segs = a.segments < 1 ? 1 : a.segments;
-    if (segs > SGP_SEQ_STRIDE - 1) segs = SGP_SEQ_STRIDE - 1;
 
-    if (tid == 0) {
-        s_ok = 1;
-        for (int i = 0; i < SGP_TMA_STAGES; ++i) mbar_init(&full[i], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    for (int k = 0; k < row.n_in; ++k) {
-        const int j = row.in[k];
-        if (j < 0) continue;
-        const SgpSignalPad* pj = a.pads[j];
-        for (int f = tid; f < pub_grid; f += SGP_THREADS)
-            if (!spin_wait_geq(&pj->pub_seq[f], s * (uint32_t)SGP_SEQ_STRIDE + (uint32_t)segs, st,
-                               a.timeout_ns, SGP_ERR_TIMEOUT_PUB))
-                s_ok = 0;
-    }
-    __syncthreads();
+    if (tid == 0) ring.init();
+    const bool ok = wait_pub_flags(a, row, s * (uint32_t)SGP_SEQ_STRIDE + (uint32_t)clamped_segments(a), pub_grid);
 
     const int n_in = row.n_in;
-    const long long my_chunks = (nchunks > blockIdx.x) ? (nchunks - 1 - blockIdx.x) / gridDim.x + 1 : 0;
-    const long long items = s_ok ? my_chunks * n_in : 0;     // (chunk, in-peer) pairs, peer fastest
-
-    auto issue = [&](long long item) {
+    const long long items = ok ? cta_chunks(nchunks, blockIdx.x) * n_in : 0;     // (chunk, in-peer) pairs, peer fastest
+    const auto src_of = [&](long long item) -> const float* {
         const long long it = item / n_in;
         const int k = (int)(item - it * n_in);
         const long long c = blockIdx.x + it * gridDim.x;
-        const int stage = (int)(item % SGP_TMA_STAGES);
-        const float* src = a.outboxes[row.in[k]] + (size_t)parity * a.n + c * SGP_CHUNK;
-        mbar_expect_tx(&full[stage], SGP_TMA_BYTES);
-        tma_load_1d(ring + (size_t)stage * SGP_CHUNK, src, SGP_TMA_BYTES, &full[stage]);
+        return a.outboxes[row.in[k]] + (size_t)parity * a.n + c * SGP_CHUNK;
     };
-
-    if (tid == 0)
-        for (long long i = 0; i < items && i < SGP_TMA_STAGES; ++i) issue(i);
+    if (tid == 0) ring.fill(items, src_of);
 
     float4 acc[SGP_UNROLL];
     for (long long item = 0; item < items; ++item) {
         const long long it = item / n_in;
         const int k = (int)(item - it * n_in);
-        const int stage = (int)(item % SGP_TMA_STAGES);
-        mbar_wait(&full[stage], (uint32_t)((item / SGP_TMA_STAGES) & 1));
-        const float4* src = reinterpret_cast<const float4*>(ring + (size_t)stage * SGP_CHUNK);
+        const float4* src = ring.wait(item);
         const float wk = row.in_w[k];
 #pragma unroll
         for (int u = 0; u < SGP_UNROLL; ++u) {
@@ -617,27 +729,11 @@ sgp_gather_tma_kernel(const SgpArgs a, const int pub_grid)
 #pragma unroll
             for (int u = 0; u < SGP_UNROLL; ++u) st_f4(dst + tid + u * SGP_THREADS, acc[u]);
         }
-        __syncthreads();                         // every thread is done with this stage
-        if (tid == 0 && item + SGP_TMA_STAGES < items) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads -> async write
-            issue(item + SGP_TMA_STAGES);
-        }
+        ring.refill(item, items, src_of);
     }
 
     __syncthreads();
-    if (tid == 0 && cta_done_is_last(st)) {
-        float wr = 0.f;
-        for (int k = 0; k < row.n_in; ++k) {
-            const int j = row.in[k];
-            if (j < 0) continue;
-            wr = fmaf(row.in_w[k], ld_relaxed_sys_f32(&a.pads[j]->psw[parity]), wr);
-            if (j != a.rank) st_release_sys(&a.pads[j]->ack_seq[a.rank], s + 1u);
-        }
-        *((volatile float*)&st->res_weight) = s_ok ? wr : 0.f;
-        *((volatile float*)&st->res_scale) = 1.f;
-        *((volatile uint32_t*)&st->done_ctas) = 0u;
-        __threadfence();
-    }
+    if (tid == 0 && cta_done_is_last(st)) gather_epilogue(a, row, s, ok, false);
 }
 
 // ---------------------------------------------------------------------------
@@ -683,10 +779,6 @@ sgp_gather_tma_kernel(const SgpArgs a, const int pub_grid)
 #define PIPE_THREADS   (PIPE_CONSUMERS + 32)
 #define PIPE_SMEM      (PIPE_STAGES * SGP_TMA_BYTES + 2 * PIPE_STAGES * 8 + 64)
 
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(smem_u32(bar)) : "memory");
-}
-
 // 9 warps x 2 CTAs per SM: the register file is split over 4 sub-partitions (16 K registers
 // each), so 18 warps only fit at <= 102 registers per thread -- __launch_bounds__(288, 2) makes
 // ptxas pick 96.  (At 112 registers the kernel runs one CTA per SM.)
@@ -725,9 +817,8 @@ sgp_step_pipe_kernel(const SgpArgs a)
     SgpSignalPad* mypad = a.pads[a.rank];
     Msg* my_out = reinterpret_cast<Msg*>(a.outboxes[a.rank]) + (size_t)parity * a.n;
 
-    const long long my_chunks = (nchunks > b) ? (nchunks - 1 - b) / gridDim.x + 1 : 0;
-    int K = a.segments < 1 ? 1 : a.segments;
-    if (K > SGP_SEQ_STRIDE - 1) K = SGP_SEQ_STRIDE - 1;
+    const long long my_chunks = cta_chunks(nchunks, b);
+    const int K = clamped_segments(a);
     const uint32_t seq_base = step * (uint32_t)SGP_SEQ_STRIDE;
 
     // compacted in-neighbour list (table entries < 0 are holes)
@@ -800,19 +891,8 @@ sgp_step_pipe_kernel(const SgpArgs a)
         const bool do_sgd = (flags & SGP_F_SGD) && (hp.do_sgd != 0.f);
         const int lane = tid & 31;
 
-        if (step >= st->ack_from + 2u) {
-            // WAR fence: outbox[parity] was last read at step-2 by that step's out-neighbours
-            if (tid == 0) {
-                RowInfo prev;
-                load_row(a, step - 2u, prev);
-                int ok = 1;
-                for (int k = 0; k < prev.n_out; ++k) {
-                    const int o = prev.out[k];
-                    if (o == a.rank || o < 0) continue;
-                    ok &= spin_wait_geq(&mypad->ack_seq[o], step - 1u, st, a.timeout_ns, SGP_ERR_TIMEOUT_ACK) ? 1 : 0;
-                }
-                s_ok = ok;
-            }
+        if (outbox_was_read(a, step)) {
+            if (tid == 0) s_ok = wait_outbox_acks(a, step) ? 1 : 0;      // before overwriting outbox[parity]
             asm volatile("bar.sync 1, %0;" :: "n"(PIPE_CONSUMERS) : "memory");
         }
 
@@ -825,72 +905,10 @@ sgp_step_pipe_kernel(const SgpArgs a)
             // ---------------- phase 1 of segment `seg`: local update + publish ----------------
             if (seg < K) {
                 const long long it_lo = my_chunks * seg / K, it_hi = my_chunks * (seg + 1) / K;
-                for (long long it = it_lo; it < it_hi; ++it) {
-                    const long long c = b + it * gridDim.x;
-                    const long long base = c * SGP_CHUNK + (long long)tid * SGP_VEC;
-                    float4 x[SGP_UNROLL], g[SGP_UNROLL], m[SGP_UNROLL];
-                    uint32_t grp[SGP_UNROLL];
-                    float tr[SGP_UNROLL];
-#pragma unroll
-                    for (int u = 0; u < SGP_UNROLL; ++u) {
-                        const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
-                        x[u] = ld_once_f4(reinterpret_cast<const float4*>(a.z + i), pol_first);
-                        if (do_sgd) {
-                            if (flags & SGP_F_GRAD_BF16)
-                                g[u] = bf16x4_to_f4(ld_once_u2(reinterpret_cast<const uint2*>(
-                                           reinterpret_cast<const __nv_bfloat16*>(a.g) + i), pol_first));
-                            else
-                                g[u] = ld_once_f4(reinterpret_cast<const float4*>(
-                                           reinterpret_cast<const float*>(a.g) + i), pol_first);
-                            if (a.g2 != nullptr) {
-                                const float4 h = ld_once_f4(reinterpret_cast<const float4*>(a.g2 + i), pol_first);
-                                g[u].x += h.x; g[u].y += h.y; g[u].z += h.z; g[u].w += h.w;
-                            }
-                            m[u] = ld_once_f4(reinterpret_cast<const float4*>(a.m + i), pol_first);
-                            if constexpr (GROUPS) grp[u] = block_group_of(a, i);
-                            if constexpr (LARS) tr[u] = lars_trust_of(a, i);
-                        }
-                    }
-#pragma unroll
-                    for (int u = 0; u < SGP_UNROLL; ++u) {
-                        const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
-                        float4 xv = mul4(x[u], wmul);
-                        if (do_sgd) {
-                            float4 gv = mul4(g[u], hp.grad_scale);
-                            float4 mv = m[u];
-                            if constexpr (LARS) {
-                                sgd4_lars(xv, gv, mv, s_rows[grp[u]], tr[u]);
-                            } else if constexpr (GROUPS) {
-                                sgd4(xv, gv, mv, s_rows[grp[u]]);
-                            } else {
-                                sgd1(xv.x, gv.x, mv.x, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
-                                sgd1(xv.y, gv.y, mv.y, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
-                                sgd1(xv.z, gv.z, mv.z, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
-                                sgd1(xv.w, gv.w, mv.w, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
-                            }
-                            st_f4(reinterpret_cast<float4*>(a.m + i), mv);
-                            if (flags & SGP_F_ZERO_GRAD) {
-                                if (flags & SGP_F_GRAD_BF16)
-                                    st_u2(reinterpret_cast<uint2*>(
-                                              reinterpret_cast<__nv_bfloat16*>(a.g) + i), make_uint2(0u, 0u));
-                                else
-                                    st_f4(reinterpret_cast<float4*>(reinterpret_cast<float*>(a.g) + i),
-                                          make_float4(0.f, 0.f, 0.f, 0.f));
-                                if (a.g2 != nullptr)
-                                    st_f4(reinterpret_cast<float4*>(a.g2 + i), make_float4(0.f, 0.f, 0.f, 0.f));
-                            }
-                        }
-                        if constexpr (MSG_BF16) {
-                            // publish Q(x); z keeps what was not sent: c = x - (1 - self_w) Q(x)
-                            const uint2 q = f4_to_bf16x4(xv);
-                            st_hint_u2(reinterpret_cast<uint2*>(my_out + i), q, pol_last);
-                            st_hint_f4(reinterpret_cast<float4*>(a.z + i),
-                                       fma4(bf16x4_to_f4(q), row.self_w - 1.f, xv), pol_last);
-                        } else {
-                            st_hint_f4(reinterpret_cast<float4*>(my_out + i), xv, pol_last);
-                        }
-                    }
-                }
+                for (long long it = it_lo; it < it_hi; ++it)
+                    phase1_chunk<MSG_BF16, GROUPS, LARS, true>(a, flags, b + it * gridDim.x, tid, hp, do_sgd, s_rows,
+                                                               wmul, row.self_w, my_out, pol_first, pol_last,
+                                                               1.f, inv_w1, false);
                 asm volatile("bar.sync 1, %0;" :: "n"(PIPE_CONSUMERS) : "memory");
                 if (tid == 0) {
                     if (seg == 0) st_relaxed_sys_f32(&mypad->psw[parity], w1);
@@ -908,11 +926,11 @@ sgp_step_pipe_kernel(const SgpArgs a)
                 const long long it_lo = my_chunks * ps / K, it_hi = my_chunks * (ps + 1) / K;
                 for (long long it = it_lo; it < it_hi; ++it) {
                     const long long c = b + it * gridDim.x;
-                    const long long base = c * SGP_CHUNK + (long long)tid * SGP_VEC;
+                    const long long base = chunk_base(c, tid);
                     float4 acc[SGP_UNROLL];
 #pragma unroll
                     for (int u = 0; u < SGP_UNROLL; ++u) {
-                        const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
+                        const long long i = chunk_elem(base, u);
                         if constexpr (MSG_BF16)      // c already carries the self weight
                             acc[u] = ld_once_f4(reinterpret_cast<const float4*>(a.z + i), pol_first);   // L2 hit
                         else
@@ -939,7 +957,7 @@ sgp_step_pipe_kernel(const SgpArgs a)
                     const bool failed = s_fail != 0;           // (rare: re-read the own numerator)
 #pragma unroll
                     for (int u = 0; u < SGP_UNROLL; ++u) {
-                        const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
+                        const long long i = chunk_elem(base, u);
                         float4 zv;
                         if constexpr (MSG_BF16)    // own numerator c (still in z) over the weight kept
                             zv = failed ? mul4(ld_once_f4(reinterpret_cast<const float4*>(a.z + i), pol_first),
@@ -949,9 +967,7 @@ sgp_step_pipe_kernel(const SgpArgs a)
                             zv = failed
                                 ? mul4(ld_once_f4(reinterpret_cast<const float4*>(my_out + i), pol_first), inv_w1)
                                 : mul4(acc[u], inv_wn);
-                        st_f4(reinterpret_cast<float4*>(a.z + i), zv);
-                        if (flags & SGP_F_SHADOW)
-                            st_u2(reinterpret_cast<uint2*>(a.shadow + i), f4_to_bf16x4(zv));
+                        store_z(a, flags, i, zv);
                     }
                 }
             }
@@ -975,40 +991,19 @@ sgp_step_pipe_kernel(const SgpArgs a)
 // ---------------------------------------------------------------------------
 __global__ void sgp_probe_kernel(const SgpArgs a, const int pub_grid, uint32_t* host_flag)
 {
-    __shared__ int s_all;
     SgpState* st = a.st;
     const uint32_t step = *((volatile uint32_t*)&st->step);
     RowInfo row;
     load_row(a, step, row);
-    int segs = a.segments < 1 ? 1 : a.segments;
-    if (segs > SGP_SEQ_STRIDE - 1) segs = SGP_SEQ_STRIDE - 1;
-    if (threadIdx.x == 0) s_all = 1;
-    __syncthreads();
-    for (int k = 0; k < row.n_in; ++k) {
-        const int j = row.in[k];
-        if (j < 0) continue;
-        for (int f = threadIdx.x; f < pub_grid; f += blockDim.x)
-            if ((int32_t)(ld_acquire_sys(&a.pads[j]->pub_seq[f]) -
-                          (step * (uint32_t)SGP_SEQ_STRIDE + (uint32_t)segs)) < 0) s_all = 0;
-    }
-    __syncthreads();
+    const uint32_t all = pub_flags_visible(a, row, step * (uint32_t)SGP_SEQ_STRIDE + (uint32_t)clamped_segments(a),
+                                           pub_grid) ? 1u : 0u;
     if (threadIdx.x == 0) {
         // may outbox[step&1] be overwritten?  (the publish kernel would otherwise
         // spin on these acks; the host checks first so no kernel ever waits)
-        uint32_t acks_ok = 1u;
-        if (step >= st->ack_from + 2u) {
-            RowInfo prev;
-            load_row(a, step - 2u, prev);
-            for (int k = 0; k < prev.n_out; ++k) {
-                const int o = prev.out[k];
-                if (o < 0 || o == a.rank) continue;
-                if ((int32_t)(ld_acquire_sys(&a.pads[a.rank]->ack_seq[o]) - (step - 1u)) < 0)
-                    acks_ok = 0u;
-            }
-        }
-        st->bilat_done = (uint32_t)s_all;
+        const uint32_t acks_ok = (!outbox_was_read(a, step) || outbox_acks_ok(a, step)) ? 1u : 0u;
+        st->bilat_done = all;
         if (host_flag) {
-            ((volatile uint32_t*)host_flag)[0] = (uint32_t)s_all;
+            ((volatile uint32_t*)host_flag)[0] = all;
             ((volatile uint32_t*)host_flag)[1] = acks_ok;
         }
         __threadfence_system();
@@ -1032,37 +1027,19 @@ __global__ void sgp_gather_wait_kernel(const SgpArgs a, const int pub_grid)
     const uint32_t s = *((volatile uint32_t*)&st->step) - 1u;
     RowInfo row;
     load_row(a, s, row);
-    int segs = a.segments < 1 ? 1 : a.segments;
-    if (segs > SGP_SEQ_STRIDE - 1) segs = SGP_SEQ_STRIDE - 1;
-    for (int k = 0; k < row.n_in; ++k) {
-        const int j = row.in[k];
-        if (j < 0) continue;
-        for (int f = threadIdx.x; f < pub_grid; f += blockDim.x)
-            spin_wait_geq(&a.pads[j]->pub_seq[f], s * (uint32_t)SGP_SEQ_STRIDE + (uint32_t)segs, st,
-                          a.timeout_ns, SGP_ERR_TIMEOUT_PUB);
-    }
+    // (a timeout is left in st->status, where sgp_gather_ack_kernel finds it)
+    wait_pub_flags(a, row, s * (uint32_t)SGP_SEQ_STRIDE + (uint32_t)clamped_segments(a), pub_grid);
 }
 
 __global__ void sgp_gather_ack_kernel(const SgpArgs a)
 {
     SgpState* st = a.st;
     const uint32_t s = *((volatile uint32_t*)&st->step) - 1u;
-    const uint32_t parity = s & 1u;
     RowInfo row;
     load_row(a, s, row);
     const bool ok = *((volatile uint32_t*)&st->status) == SGP_OK;
-    float wr = 0.f, scale = 0.f;
     __threadfence_system();                         // the DMA copy before this kernel has completed
-    for (int k = 0; k < row.n_in; ++k) {
-        const int j = row.in[k];
-        if (j < 0) continue;
-        scale = row.in_w[k];                        // (single in-neighbour: enforced by the host)
-        wr = fmaf(row.in_w[k], ld_relaxed_sys_f32(&a.pads[j]->psw[parity]), wr);
-        if (j != a.rank) st_release_sys(&a.pads[j]->ack_seq[a.rank], s + 1u);
-    }
-    *((volatile float*)&st->res_weight) = ok ? wr : 0.f;
-    *((volatile float*)&st->res_scale) = ok ? scale : 0.f;
-    __threadfence();
+    gather_epilogue(a, row, s, ok, true);
 }
 
 // ---------------------------------------------------------------------------
@@ -1082,15 +1059,13 @@ __global__ void sgp_gather_ack_kernel(const SgpArgs a)
 __global__ void sgp_bilat_decide_kernel(const SgpArgs a, const int pub_grid, const int passive,
                                         const unsigned long long max_wait_ns, uint32_t* host_fb)
 {
-    __shared__ int s_all, s_stop;
+    __shared__ int s_stop;
     __shared__ uint32_t s_published, s_may_start;
     SgpState* st = a.st;
     const uint32_t step = *((volatile uint32_t*)&st->step);
     RowInfo row;
     load_row(a, step, row);
-    int segs = a.segments < 1 ? 1 : a.segments;
-    if (segs > SGP_SEQ_STRIDE - 1) segs = SGP_SEQ_STRIDE - 1;
-    const uint32_t want = step * (uint32_t)SGP_SEQ_STRIDE + (uint32_t)segs;
+    const uint32_t want = step * (uint32_t)SGP_SEQ_STRIDE + (uint32_t)clamped_segments(a);
     // bilat_budget / bilat_enabled are rewritten asynchronously (sgp_bilat_ctl_kernel on the
     // training stream): ONE thread samples them and the whole CTA uses that sample, so that every
     // thread takes the same branch around the barrier loop below
@@ -1108,37 +1083,19 @@ __global__ void sgp_bilat_decide_kernel(const SgpArgs a, const int pub_grid, con
     if (engaged) {
         const unsigned long long t0 = globaltimer_ns();
         while (true) {
-            if (threadIdx.x == 0) s_all = 1;
-            __syncthreads();
-            for (int k = 0; k < row.n_in; ++k) {
-                const int j = row.in[k];
-                if (j < 0) continue;
-                for (int f = threadIdx.x; f < pub_grid; f += blockDim.x)
-                    if ((int32_t)(ld_acquire_sys(&a.pads[j]->pub_seq[f]) - want) < 0) s_all = 0;
-            }
-            __syncthreads();
+            ready = pub_flags_visible(a, row, want, pub_grid) ? 1 : 0;
             // ONE thread decides whether to stop (the deadline must not be evaluated per thread:
             // threads straddling it would leave the barrier loop at different iterations)
-            if (threadIdx.x == 0) s_stop = (s_all != 0) || (globaltimer_ns() - t0 > max_wait_ns);
+            if (threadIdx.x == 0) s_stop = (ready != 0) || (globaltimer_ns() - t0 > max_wait_ns);
             __syncthreads();
-            ready = s_all;
             const int stop = s_stop;
-            __syncthreads();                  // s_all / s_stop are rewritten by the next iteration
+            __syncthreads();                  // s_stop is rewritten by the next iteration
             if (stop) break;
             __nanosleep(500);
         }
     }
     if (threadIdx.x != 0) return;
-    uint32_t acks_ok = 1u;
-    if (step >= st->ack_from + 2u) {
-        RowInfo prev;
-        load_row(a, step - 2u, prev);
-        for (int k = 0; k < prev.n_out; ++k) {
-            const int o = prev.out[k];
-            if (o < 0 || o == a.rank) continue;
-            if ((int32_t)(ld_acquire_sys(&a.pads[a.rank]->ack_seq[o]) - (step - 1u)) < 0) acks_ok = 0u;
-        }
-    }
+    const bool acks_ok = !outbox_was_read(a, step) || outbox_acks_ok(a, step);
     const bool do_publish = !published && may_start && acks_ok && (ready || !passive);
     const bool do_pull = ready && (published || do_publish);
     uint32_t cmd = 0u;
@@ -1207,7 +1164,7 @@ sgp_allreduce_sgd_kernel(const SgpArgs a, void* const* grad_peers)
     if (s_ok) {
         const float inv_world = hp.grad_scale / (float)a.world;
         for (long long c = b; c < nchunks; c += gridDim.x) {
-            const long long base = c * SGP_CHUNK + (long long)tid * SGP_VEC;
+            const long long base = chunk_base(c, tid);
             float4 acc[SGP_UNROLL];
 #pragma unroll
             for (int u = 0; u < SGP_UNROLL; ++u) acc[u] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -1215,7 +1172,7 @@ sgp_allreduce_sgd_kernel(const SgpArgs a, void* const* grad_peers)
                 float4 gv[SGP_UNROLL];
 #pragma unroll
                 for (int u = 0; u < SGP_UNROLL; ++u) {
-                    const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
+                    const long long i = chunk_elem(base, u);
                     if (flags & SGP_F_GRAD_BF16) {
                         uint2 raw;
                         const uint2* p = reinterpret_cast<const uint2*>(
@@ -1236,18 +1193,13 @@ sgp_allreduce_sgd_kernel(const SgpArgs a, void* const* grad_peers)
             }
 #pragma unroll
             for (int u = 0; u < SGP_UNROLL; ++u) {
-                const long long i = base + (long long)u * SGP_THREADS * SGP_VEC;
+                const long long i = chunk_elem(base, u);
                 float4 xv = ld_once_f4(reinterpret_cast<const float4*>(a.z + i), pol_first);
                 float4 mv = ld_once_f4(reinterpret_cast<const float4*>(a.m + i), pol_first);
                 const float4 gv = mul4(acc[u], inv_world);
-                sgd1(xv.x, gv.x, mv.x, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
-                sgd1(xv.y, gv.y, mv.y, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
-                sgd1(xv.z, gv.z, mv.z, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
-                sgd1(xv.w, gv.w, mv.w, hp.lr, hp.momentum, hp.weight_decay, hp.nesterov);
+                sgd4<false>(xv, gv, mv, hyper_row(hp), 1.f);
                 st_f4(reinterpret_cast<float4*>(a.m + i), mv);
-                st_f4(reinterpret_cast<float4*>(a.z + i), xv);
-                if (flags & SGP_F_SHADOW)
-                    st_u2(reinterpret_cast<uint2*>(a.shadow + i), f4_to_bf16x4(xv));
+                store_z(a, flags, i, xv);
             }
         }
     }
@@ -1359,8 +1311,6 @@ sgp_peer_reduce_kernel(float* __restrict__ dst, const SgpPtrList srcs, long long
 // The snapshot never touches pub_seq / ack_seq / psw: the next gossip step publishes with the
 // sequence numbers it would have used anyway.
 // ---------------------------------------------------------------------------
-#define SGP_CONS_STAGES 6
-#define SGP_CONS_SMEM   (SGP_CONS_STAGES * SGP_TMA_BYTES + SGP_CONS_STAGES * 8 + 64)
 #define SGP_CONS_SLOT   4      // doubles per rank: [sum_j (z_j - zbar)^2, |zbar|^2, |z_rank - zbar|^2, -]
 
 __global__ void __launch_bounds__(SGP_THREADS)
@@ -1389,8 +1339,7 @@ __global__ void __launch_bounds__(SGP_THREADS, 2)
 sgp_consensus_kernel(const SgpArgs a, double* const* partials, double* scratch, float* avg_out)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    float* ring = reinterpret_cast<float*>(smem_raw);                       // [STAGES][CHUNK]
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + SGP_CONS_STAGES * SGP_TMA_BYTES);
+    const TmaRing ring(smem_raw);
     __shared__ float  s_f[SGP_MAX_RANKS];              // w_j / W_j   (weighted running mean)
     __shared__ float  s_inv[SGP_MAX_RANKS];            // 1 / (j + 1) (Welford)
     __shared__ double s_red[3][SGP_THREADS / 32];
@@ -1403,32 +1352,20 @@ sgp_consensus_kernel(const SgpArgs a, double* const* partials, double* scratch, 
     const long long hi = FULL ? nchunks : nchunks * (a.rank + 1) / world;
 
     if (tid == 0) {
-        float wsum = 0.f;
-        for (int j = 0; j < world; ++j) {
-            const float wj = ld_relaxed_sys_f32(&a.pads[j]->snap_w);
-            wsum += wj;
-            s_f[j] = wj / wsum;
-            s_inv[j] = 1.f / (float)(j + 1);
-        }
-        for (int i = 0; i < SGP_CONS_STAGES; ++i) mbar_init(&full[i], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        running_mean_factors(a, s_f);
+        for (int j = 0; j < world; ++j) s_inv[j] = 1.f / (float)(j + 1);
+        ring.init();
     }
     __syncthreads();
 
-    const long long span = hi - lo;
-    const long long my_chunks = (span > blockIdx.x) ? (span - 1 - blockIdx.x) / gridDim.x + 1 : 0;
-    const long long items = my_chunks * world;
-
-    auto issue = [&](long long item) {
+    const long long items = cta_chunks(hi - lo, blockIdx.x) * world;     // (chunk, rank) pairs, rank fastest
+    const auto src_of = [&](long long item) -> const float* {
         const long long it = item / world;
         const int j = (int)(item - it * world);
         const long long c = lo + blockIdx.x + it * gridDim.x;
-        const int stage = (int)(item % SGP_CONS_STAGES);
-        mbar_expect_tx(&full[stage], SGP_TMA_BYTES);
-        tma_load_1d(ring + (size_t)stage * SGP_CHUNK, a.outboxes[j] + c * SGP_CHUNK, SGP_TMA_BYTES, &full[stage]);
+        return a.outboxes[j] + c * SGP_CHUNK;
     };
-    if (tid == 0)
-        for (long long i = 0; i < items && i < SGP_CONS_STAGES; ++i) issue(i);
+    if (tid == 0) ring.fill(items, src_of);
 
     float4 zb[SGP_UNROLL], mu[SGP_UNROLL], m2[SGP_UNROLL], own[SGP_UNROLL];
     double acc_d = 0.0, acc_n = 0.0, acc_o = 0.0;
@@ -1436,9 +1373,7 @@ sgp_consensus_kernel(const SgpArgs a, double* const* partials, double* scratch, 
     for (long long item = 0; item < items; ++item) {
         const long long it = item / world;
         const int j = (int)(item - it * world);
-        const int stage = (int)(item % SGP_CONS_STAGES);
-        mbar_wait(&full[stage], (uint32_t)((item / SGP_CONS_STAGES) & 1));
-        const float4* src = reinterpret_cast<const float4*>(ring + (size_t)stage * SGP_CHUNK);
+        const float4* src = ring.wait(item);
         const float fj = s_f[j], ij = s_inv[j];
 #pragma unroll
         for (int u = 0; u < SGP_UNROLL; ++u) {
@@ -1484,11 +1419,7 @@ sgp_consensus_kernel(const SgpArgs a, double* const* partials, double* scratch, 
                     st_f4(reinterpret_cast<float4*>(avg_out + c * SGP_CHUNK) + tid + u * SGP_THREADS, zb[u]);
             }
         }
-        __syncthreads();                         // every thread is done with this stage
-        if (tid == 0 && item + SGP_CONS_STAGES < items) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads -> async write
-            issue(item + SGP_CONS_STAGES);
-        }
+        ring.refill(item, items, src_of);
     }
 
     // CTA reduction in a fixed order (shuffle tree, then warps 0..7), then the grid: the last CTA
@@ -1568,8 +1499,7 @@ sgp_slowmo_kernel(const SgpArgs a, float* u, float* x_prev, float lr, float alph
     if (*((volatile uint32_t*)&a.st->status) != SGP_OK) return;
 
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    float* ring = reinterpret_cast<float*>(smem_raw);                       // [STAGES][CHUNK]
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + SGP_CONS_STAGES * SGP_TMA_BYTES);
+    const TmaRing ring(smem_raw);
     __shared__ float s_f[SGP_MAX_RANKS];              // w_j / W_j   (weighted running mean)
 
     const int tid = threadIdx.x;
@@ -1577,14 +1507,8 @@ sgp_slowmo_kernel(const SgpArgs a, float* u, float* x_prev, float lr, float alph
     const long long nchunks = a.n / SGP_CHUNK;
 
     if (tid == 0) {
-        float wsum = 0.f;
-        for (int j = 0; j < world; ++j) {
-            const float wj = ld_relaxed_sys_f32(&a.pads[j]->snap_w);
-            wsum += wj;
-            s_f[j] = wj / wsum;
-        }
-        for (int i = 0; i < SGP_CONS_STAGES; ++i) mbar_init(&full[i], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        running_mean_factors(a, s_f);
+        ring.init();
         if (blockIdx.x == 0) {
             *((volatile float*)&a.st->ps_weight[0]) = 1.f;
             *((volatile float*)&a.st->ps_weight[1]) = 1.f;
@@ -1592,19 +1516,14 @@ sgp_slowmo_kernel(const SgpArgs a, float* u, float* x_prev, float lr, float alph
     }
     __syncthreads();
 
-    const long long my_chunks = (nchunks > blockIdx.x) ? (nchunks - 1 - blockIdx.x) / gridDim.x + 1 : 0;
-    const long long items = my_chunks * world;
-
-    auto issue = [&](long long item) {
+    const long long items = cta_chunks(nchunks, blockIdx.x) * world;     // (chunk, rank) pairs, rank fastest
+    const auto src_of = [&](long long item) -> const float* {
         const long long it = item / world;
         const int j = (int)(item - it * world);
         const long long c = blockIdx.x + it * gridDim.x;
-        const int stage = (int)(item % SGP_CONS_STAGES);
-        mbar_expect_tx(&full[stage], SGP_TMA_BYTES);
-        tma_load_1d(ring + (size_t)stage * SGP_CHUNK, a.outboxes[j] + c * SGP_CHUNK, SGP_TMA_BYTES, &full[stage]);
+        return a.outboxes[j] + c * SGP_CHUNK;
     };
-    if (tid == 0)
-        for (long long i = 0; i < items && i < SGP_CONS_STAGES; ++i) issue(i);
+    if (tid == 0) ring.fill(items, src_of);
 
     const uint64_t pol_first = l2_evict_first_policy();
     const float alr = alpha * lr;
@@ -1612,9 +1531,7 @@ sgp_slowmo_kernel(const SgpArgs a, float* u, float* x_prev, float lr, float alph
     for (long long item = 0; item < items; ++item) {
         const long long it = item / world;
         const int j = (int)(item - it * world);
-        const int stage = (int)(item % SGP_CONS_STAGES);
-        mbar_wait(&full[stage], (uint32_t)((item / SGP_CONS_STAGES) & 1));
-        const float4* src = reinterpret_cast<const float4*>(ring + (size_t)stage * SGP_CHUNK);
+        const float4* src = ring.wait(item);
         const float fj = s_f[j];
 #pragma unroll
         for (int k = 0; k < SGP_UNROLL; ++k) {
@@ -1628,11 +1545,7 @@ sgp_slowmo_kernel(const SgpArgs a, float* u, float* x_prev, float lr, float alph
                 zb[k].w = fmaf(fj, v.w - zb[k].w, zb[k].w);
             }
         }
-        __syncthreads();                         // every thread is done with this stage
-        if (tid == 0 && item + SGP_CONS_STAGES < items) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads -> async write
-            issue(item + SGP_CONS_STAGES);
-        }
+        ring.refill(item, items, src_of);
         if (j == world - 1) {
             const long long c = blockIdx.x + it * gridDim.x;
 #pragma unroll
@@ -1788,27 +1701,86 @@ static bool msg_bf16_mode_ok(unsigned int flags)
     return (flags & full) == full && (flags & partial) == 0u;
 }
 
+// The instantiations of the two step kernels: MSG_BF16 is free, LARS needs GROUPS.  Whatever has
+// to know every variant (launch, shared-memory opt-in, occupancy, preloading) goes through
+// for_each_step_variant, so a new variant is one more line here.
 template <bool MSG_BF16, bool GROUPS, bool LARS>
-static cudaError_t configure_step_pipe()
+struct StepVariant {
+    static constexpr auto step = &sgp_step_kernel<MSG_BF16, GROUPS, LARS>;
+    static constexpr auto pipe = &sgp_step_pipe_kernel<MSG_BF16, GROUPS, LARS>;
+    // (lars_ok: SGP_F_LARS only comes with SGP_F_GROUPS)
+    static bool selected_by(unsigned int flags) {
+        return MSG_BF16 == ((flags & SGP_F_MSG_BF16) != 0u) && LARS == ((flags & SGP_F_LARS) != 0u) &&
+               GROUPS == ((flags & (SGP_F_GROUPS | SGP_F_LARS)) != 0u);
+    }
+};
+
+template <class F>
+static void for_each_step_variant(F&& f)
 {
-    cudaError_t e = cudaFuncSetAttribute(sgp_step_pipe_kernel<MSG_BF16, GROUPS, LARS>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, PIPE_SMEM);
-    if (e != cudaSuccess) return e;
-    // two CTAs x 64 KB per SM: ask for the large shared-memory carve-out (the default one fits
-    // a single CTA: launch__occupancy_limit_shared_mem = 1 in the first ncu capture)
-    return cudaFuncSetAttribute(sgp_step_pipe_kernel<MSG_BF16, GROUPS, LARS>,
-                                cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    f(StepVariant<false, false, false>{});
+    f(StepVariant<true, false, false>{});
+    f(StepVariant<false, true, false>{});
+    f(StepVariant<true, true, false>{});
+    f(StepVariant<false, true, true>{});
+    f(StepVariant<true, true, true>{});
 }
 
-static cudaError_t configure_step_pipe_all()
+// f(variant) -> cudaError_t for the variant that `flags` selects
+template <class F>
+static cudaError_t with_step_variant(unsigned int flags, F&& f)
 {
-    cudaError_t e = configure_step_pipe<false, false, false>();
-    if (e == cudaSuccess) e = configure_step_pipe<true, false, false>();
-    if (e == cudaSuccess) e = configure_step_pipe<false, true, false>();
-    if (e == cudaSuccess) e = configure_step_pipe<true, true, false>();
-    if (e == cudaSuccess) e = configure_step_pipe<false, true, true>();
-    if (e == cudaSuccess) e = configure_step_pipe<true, true, true>();
+    cudaError_t e = cudaErrorInvalidValue;
+    for_each_step_variant([&](auto v) { if (v.selected_by(flags)) e = f(v); });
     return e;
+}
+
+// Opt Kernel in to `bytes` of dynamic shared memory (and, with max_carveout, to the large
+// shared-memory carve-out) on the current device.  The attribute belongs to the device's context
+// and one process can drive several devices, so it is set once per kernel AND device.
+template <auto Kernel>
+static cudaError_t ensure_dynamic_smem(int bytes, bool max_carveout = false)
+{
+    static bool configured[64] = {};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    const bool remember = dev >= 0 && dev < 64;
+    if (remember && configured[dev]) return cudaSuccess;
+    cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess && max_carveout)
+        e = cudaFuncSetAttribute(Kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    if (e == cudaSuccess && remember) configured[dev] = true;
+    return e;
+}
+
+// Co-resident CTAs of a step kernel: the minimum over its variants, because the ranks of a job
+// share one grid whatever variant each of them launches.
+// pipe: two CTAs x 64 KB per SM need the large shared-memory carve-out (the default one fits a
+// single CTA).  The bf16 ring uses half of each stage but asks for the same PIPE_SMEM, so the
+// occupancy stays that of the fp32 kernel
+static int step_resident_ctas(int device, bool pipe)
+{
+    int sms = 0, per_sm = 1 << 30;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) return 0;
+    for_each_step_variant([&](auto v) {
+        int n = 0;
+        cudaError_t e = pipe ? ensure_dynamic_smem<v.pipe>(PIPE_SMEM, true) : cudaSuccess;
+        if (e == cudaSuccess)
+            e = pipe ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, v.pipe, PIPE_THREADS, PIPE_SMEM)
+                     : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, v.step, SGP_THREADS, 0);
+        if (e != cudaSuccess) n = 0;
+        if (n < per_sm) per_sm = n;
+    });
+    return sms * per_sm;
+}
+
+// grid of the flat grid-stride kernels over n_vec 16-byte accesses
+static int flat_grid(long long n_vec)
+{
+    long long grid = (n_vec + SGP_THREADS - 1) / SGP_THREADS;
+    if (grid > 132 * 8) grid = 132 * 8;
+    if (grid < 1) grid = 1;
+    return (int)grid;
 }
 
 // SGP_F_GROUPS needs the group table, the block map and 1..SGP_MAX_GROUPS groups
@@ -1833,76 +1805,25 @@ extern "C" {
 cudaError_t sgp_launch_step(const SgpArgs* args, int grid, cudaStream_t stream)
 {
     if (!msg_bf16_mode_ok(args->flags) || !groups_ok(args) || !lars_ok(args)) return cudaErrorInvalidValue;
-    if (args->flags & SGP_F_LARS) {
-        if (args->flags & SGP_F_MSG_BF16)
-            sgp_step_kernel<true, true, true><<<grid, SGP_THREADS, 0, stream>>>(*args);
-        else
-            sgp_step_kernel<false, true, true><<<grid, SGP_THREADS, 0, stream>>>(*args);
-    } else if (args->flags & SGP_F_GROUPS) {
-        if (args->flags & SGP_F_MSG_BF16)
-            sgp_step_kernel<true, true, false><<<grid, SGP_THREADS, 0, stream>>>(*args);
-        else
-            sgp_step_kernel<false, true, false><<<grid, SGP_THREADS, 0, stream>>>(*args);
-    } else if (args->flags & SGP_F_MSG_BF16) {
-        sgp_step_kernel<true, false, false><<<grid, SGP_THREADS, 0, stream>>>(*args);
-    } else {
-        sgp_step_kernel<false, false, false><<<grid, SGP_THREADS, 0, stream>>>(*args);
-    }
-    return cudaGetLastError();
+    return with_step_variant(args->flags, [&](auto v) {
+        v.step<<<grid, SGP_THREADS, 0, stream>>>(*args);
+        return cudaGetLastError();
+    });
 }
 
 cudaError_t sgp_launch_step_pipe(const SgpArgs* args, int grid, cudaStream_t stream)
 {
     if (!msg_bf16_mode_ok(args->flags) || !groups_ok(args) || !lars_ok(args)) return cudaErrorInvalidValue;
-    static bool configured[64] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64 || !configured[dev]) {
-        cudaError_t e = configure_step_pipe_all();
+    return with_step_variant(args->flags, [&](auto v) {
+        const cudaError_t e = ensure_dynamic_smem<v.pipe>(PIPE_SMEM, true);
         if (e != cudaSuccess) return e;
-        if (dev >= 0 && dev < 64) configured[dev] = true;
-    }
-    // (the bf16 ring uses half of each stage: the occupancy, and so the grid every rank shares,
-    // stays that of the fp32 kernel)
-    if (args->flags & SGP_F_LARS) {
-        if (args->flags & SGP_F_MSG_BF16)
-            sgp_step_pipe_kernel<true, true, true><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
-        else
-            sgp_step_pipe_kernel<false, true, true><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
-    } else if (args->flags & SGP_F_GROUPS) {
-        if (args->flags & SGP_F_MSG_BF16)
-            sgp_step_pipe_kernel<true, true, false><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
-        else
-            sgp_step_pipe_kernel<false, true, false><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
-    } else if (args->flags & SGP_F_MSG_BF16) {
-        sgp_step_pipe_kernel<true, false, false><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
-    } else {
-        sgp_step_pipe_kernel<false, false, false><<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
-    }
-    return cudaGetLastError();
+        v.pipe<<<grid, PIPE_THREADS, PIPE_SMEM, stream>>>(*args);
+        return cudaGetLastError();
+    });
 }
 
-// co-resident CTAs of the pipelined step kernel (dynamic shared memory bound): the minimum over
-// its instantiations, because the ranks of a job share one grid whatever variant each launches
-int sgp_max_resident_ctas_pipe(int device)
-{
-    int sms = 0;
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) return 0;
-    configure_step_pipe_all();
-    const void* kernels[] = {(const void*)sgp_step_pipe_kernel<false, false, false>,
-                             (const void*)sgp_step_pipe_kernel<true, false, false>,
-                             (const void*)sgp_step_pipe_kernel<false, true, false>,
-                             (const void*)sgp_step_pipe_kernel<true, true, false>,
-                             (const void*)sgp_step_pipe_kernel<false, true, true>,
-                             (const void*)sgp_step_pipe_kernel<true, true, true>};
-    int per_sm = 1 << 30;
-    for (const void* k : kernels) {
-        int n = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k, PIPE_THREADS, PIPE_SMEM) != cudaSuccess) return 0;
-        if (n < per_sm) per_sm = n;
-    }
-    return sms * per_sm;
-}
+int sgp_max_resident_ctas_pipe(int device) { return step_resident_ctas(device, true); }
+int sgp_max_resident_ctas(int device) { return step_resident_ctas(device, false); }
 
 // the two LARS kernels (see sgp_lars_norms_kernel): any grid >= 1 gives the same bits
 cudaError_t sgp_launch_lars_norms(const SgpArgs* args, int grid, cudaStream_t stream)
@@ -1931,15 +1852,9 @@ cudaError_t sgp_launch_gather(const SgpArgs* args, int grid, int pub_grid, cudaS
 cudaError_t sgp_launch_gather_tma(const SgpArgs* args, int grid, int pub_grid, cudaStream_t stream)
 {
     if (args->flags & SGP_F_MSG_BF16) return cudaErrorInvalidValue;
-    const int smem = SGP_TMA_STAGES * SGP_TMA_BYTES + SGP_TMA_STAGES * 8 + 64;
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(sgp_gather_tma_kernel,
-                                             cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        if (e != cudaSuccess) return e;
-        configured = true;
-    }
-    sgp_gather_tma_kernel<<<grid, SGP_THREADS, smem, stream>>>(*args, pub_grid);
+    const cudaError_t e = ensure_dynamic_smem<sgp_gather_tma_kernel>(SGP_RING_SMEM);
+    if (e != cudaSuccess) return e;
+    sgp_gather_tma_kernel<<<grid, SGP_THREADS, SGP_RING_SMEM, stream>>>(*args, pub_grid);
     return cudaGetLastError();
 }
 
@@ -1990,20 +1905,14 @@ cudaError_t sgp_launch_peer_reduce(float* dst, const float* const* srcs, int nsr
     l.n = nsrc;
     for (int k = 0; k < nsrc; ++k) l.p[k] = srcs[k];
     const long long n4 = n / 4;
-    int grid = (int)((n4 + SGP_THREADS - 1) / SGP_THREADS);
-    if (grid > 132 * 8) grid = 132 * 8;
-    if (grid < 1) grid = 1;
-    sgp_peer_reduce_kernel<<<grid, SGP_THREADS, 0, stream>>>(dst, l, n4, scale);
+    sgp_peer_reduce_kernel<<<flat_grid(n4), SGP_THREADS, 0, stream>>>(dst, l, n4, scale);
     return cudaGetLastError();
 }
 
 cudaError_t sgp_launch_zero(void* p, long long bytes, cudaStream_t stream)
 {
     const long long n16 = bytes / 16;
-    int grid = (int)((n16 + SGP_THREADS - 1) / SGP_THREADS);
-    if (grid > 132 * 8) grid = 132 * 8;
-    if (grid < 1) grid = 1;
-    sgp_zero_kernel<<<grid, SGP_THREADS, 0, stream>>>(reinterpret_cast<float4*>(p), n16);
+    sgp_zero_kernel<<<flat_grid(n16), SGP_THREADS, 0, stream>>>(reinterpret_cast<float4*>(p), n16);
     return cudaGetLastError();
 }
 
@@ -2017,22 +1926,14 @@ cudaError_t sgp_launch_barrier(SgpSignalPad* const* pads, SgpState* st, int rank
 cudaError_t sgp_launch_scale(float* x, long long n, const float* scalar, int invert,
                              __nv_bfloat16* shadow, cudaStream_t stream)
 {
-    long long n4 = n / 4;
-    int grid = (int)((n4 + SGP_THREADS - 1) / SGP_THREADS);
-    if (grid > 132 * 8) grid = 132 * 8;
-    if (grid < 1) grid = 1;
-    sgp_scale_kernel<<<grid, SGP_THREADS, 0, stream>>>(x, n, scalar, invert, shadow);
+    sgp_scale_kernel<<<flat_grid(n / 4), SGP_THREADS, 0, stream>>>(x, n, scalar, invert, shadow);
     return cudaGetLastError();
 }
 
 cudaError_t sgp_launch_snapshot(const SgpArgs* args, cudaStream_t stream)
 {
     if (!args->outboxes || (args->n & 3)) return cudaErrorInvalidValue;
-    const long long n4 = args->n / 4;
-    int grid = (int)((n4 + SGP_THREADS - 1) / SGP_THREADS);
-    if (grid > 132 * 8) grid = 132 * 8;
-    if (grid < 1) grid = 1;
-    sgp_snapshot_kernel<<<grid, SGP_THREADS, 0, stream>>>(*args);
+    sgp_snapshot_kernel<<<flat_grid(args->n / 4), SGP_THREADS, 0, stream>>>(*args);
     return cudaGetLastError();
 }
 
@@ -2041,22 +1942,13 @@ cudaError_t sgp_launch_consensus(const SgpArgs* args, double* const* partials, d
                                  int full, int grid, cudaStream_t stream)
 {
     if (!args->outboxes || grid < 1 || grid > SGP_MAX_CTAS || (full && !avg_out)) return cudaErrorInvalidValue;
-    static bool configured[64] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64 || !configured[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(sgp_consensus_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             SGP_CONS_SMEM);
-        if (e == cudaSuccess)
-            e = cudaFuncSetAttribute(sgp_consensus_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     SGP_CONS_SMEM);
-        if (e != cudaSuccess) return e;
-        if (dev >= 0 && dev < 64) configured[dev] = true;
-    }
+    const cudaError_t e = full ? ensure_dynamic_smem<sgp_consensus_kernel<true>>(SGP_RING_SMEM)
+                               : ensure_dynamic_smem<sgp_consensus_kernel<false>>(SGP_RING_SMEM);
+    if (e != cudaSuccess) return e;
     if (full)
-        sgp_consensus_kernel<true><<<grid, SGP_THREADS, SGP_CONS_SMEM, stream>>>(*args, partials, scratch, avg_out);
+        sgp_consensus_kernel<true><<<grid, SGP_THREADS, SGP_RING_SMEM, stream>>>(*args, partials, scratch, avg_out);
     else
-        sgp_consensus_kernel<false><<<grid, SGP_THREADS, SGP_CONS_SMEM, stream>>>(*args, partials, scratch, avg_out);
+        sgp_consensus_kernel<false><<<grid, SGP_THREADS, SGP_RING_SMEM, stream>>>(*args, partials, scratch, avg_out);
     return cudaGetLastError();
 }
 
@@ -2071,16 +1963,9 @@ cudaError_t sgp_launch_slowmo(const SgpArgs* args, float* u, float* x_prev, floa
                               int init, int grid, cudaStream_t stream)
 {
     if (!args->outboxes || !u || !x_prev || grid < 1 || grid > SGP_MAX_CTAS) return cudaErrorInvalidValue;
-    static bool configured[64] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64 || !configured[dev]) {
-        const cudaError_t e = cudaFuncSetAttribute(sgp_slowmo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                   SGP_CONS_SMEM);
-        if (e != cudaSuccess) return e;
-        if (dev >= 0 && dev < 64) configured[dev] = true;
-    }
-    sgp_slowmo_kernel<<<grid, SGP_THREADS, SGP_CONS_SMEM, stream>>>(*args, u, x_prev, lr, alpha, beta, init);
+    const cudaError_t e = ensure_dynamic_smem<sgp_slowmo_kernel>(SGP_RING_SMEM);
+    if (e != cudaSuccess) return e;
+    sgp_slowmo_kernel<<<grid, SGP_THREADS, SGP_RING_SMEM, stream>>>(*args, u, x_prev, lr, alpha, beta, init);
     return cudaGetLastError();
 }
 
@@ -2090,14 +1975,14 @@ cudaError_t sgp_launch_slowmo(const SgpArgs* args, float* u, float* x_prev, floa
 // rank's spinning gossip kernel whose in-neighbour's publish it has not launched yet.
 cudaError_t sgp_preload_kernels()
 {
+    cudaError_t e = cudaSuccess;
+    const auto load = [&](const void* kernel) {
+        cudaFuncAttributes attr;
+        if (e == cudaSuccess) e = cudaFuncGetAttributes(&attr, kernel);
+    };
+    for_each_step_variant([&](auto v) { load((const void*)v.step); load((const void*)v.pipe); });
     const void* kernels[] = {
-        (const void*)sgp_step_kernel<false, false, false>, (const void*)sgp_step_kernel<true, false, false>,
-        (const void*)sgp_step_kernel<false, true, false>, (const void*)sgp_step_kernel<true, true, false>,
-        (const void*)sgp_step_kernel<false, true, true>, (const void*)sgp_step_kernel<true, true, true>,
         (const void*)sgp_gather_kernel, (const void*)sgp_gather_tma_kernel,
-        (const void*)sgp_step_pipe_kernel<false, false, false>, (const void*)sgp_step_pipe_kernel<true, false, false>,
-        (const void*)sgp_step_pipe_kernel<false, true, false>, (const void*)sgp_step_pipe_kernel<true, true, false>,
-        (const void*)sgp_step_pipe_kernel<false, true, true>, (const void*)sgp_step_pipe_kernel<true, true, true>,
         (const void*)sgp_lars_norms_kernel, (const void*)sgp_lars_trust_kernel,
         (const void*)sgp_probe_kernel, (const void*)sgp_gather_wait_kernel,
         (const void*)sgp_gather_ack_kernel, (const void*)sgp_bilat_decide_kernel, (const void*)sgp_bilat_ctl_kernel,
@@ -2105,29 +1990,8 @@ cudaError_t sgp_preload_kernels()
         (const void*)sgp_scale_kernel, (const void*)sgp_peer_reduce_kernel, (const void*)sgp_snapshot_kernel,
         (const void*)sgp_consensus_kernel<false>, (const void*)sgp_consensus_kernel<true>,
         (const void*)sgp_consensus_finalize_kernel, (const void*)sgp_slowmo_kernel};
-    for (const void* k : kernels) {
-        cudaFuncAttributes attr;
-        const cudaError_t e = cudaFuncGetAttributes(&attr, k);
-        if (e != cudaSuccess) return e;
-    }
-    return cudaSuccess;
-}
-
-int sgp_max_resident_ctas(int device)
-{
-    int sms = 0, per_sm = 0;
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) return 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sgp_step_kernel<false, false, false>, SGP_THREADS, 0)
-        != cudaSuccess) return 0;
-    // (the grouped and LARS variants are launched on the same grid)
-    const void* variants[] = {(const void*)sgp_step_kernel<false, true, false>,
-                              (const void*)sgp_step_kernel<false, true, true>};
-    for (const void* k : variants) {
-        int n = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k, SGP_THREADS, 0) != cudaSuccess) return 0;
-        if (n < per_sm) per_sm = n;
-    }
-    return sms * per_sm;
+    for (const void* k : kernels) load(k);
+    return e;
 }
 
 }  // extern "C"

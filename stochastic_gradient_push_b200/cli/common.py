@@ -75,7 +75,20 @@ def build_parser(adpsgd: bool = False) -> argparse.ArgumentParser:
                    help='epoch num_peers epoch num_peers ...; must contain epoch 0')
     p.add_argument('--overlap', default=False, **B)
     p.add_argument('--synch_freq', default=0, type=int)
-    p.add_argument('--warmup', default=False, **B, help='5-epoch linear LR warm-up')
+    p.add_argument('--warmup', default=False, **B, help='linear LR warm-up over --warmup_epochs epochs')
+    p.add_argument('--warmup_epochs', default=5, type=int,
+                   help='length of the --warmup ramp from --lr to the scaled target learning rate')
+    p.add_argument('--lr_policy', default='step', choices=['step', 'poly'],
+                   help='after the warm-up: step = multiply by the --schedule factors (Goyal et al.); '
+                        'poly = end_lr + (target - end_lr) * (1 - progress) ** poly_power, set every '
+                        'iteration (the MLPerf ResNet-50 recipe, with --lars)')
+    p.add_argument('--poly_power', default=2.0, type=float, help='exponent of --lr_policy poly')
+    p.add_argument('--end_lr', default=0.0001, type=float,
+                   help='learning rate that --lr_policy poly reaches at the end (absolute, not scaled)')
+    p.add_argument('--label_smoothing', default=0.0, type=float,
+                   help='label smoothing eps in [0, 1] of the training loss (as in '
+                        'torch.nn.CrossEntropyLoss(label_smoothing=eps); on the fused loss kernel with '
+                        '--cuda_graph True); validation keeps the plain cross-entropy')
     p.add_argument('--seed', default=47, type=int)
     p.add_argument('--resume', default=False, **B)
     p.add_argument('--backend', default='nccl', choices=['nccl', 'gloo', 'mpi'])
@@ -248,6 +261,9 @@ def finalize_args(args, adpsgd=False):
                              'SGP, OSGP and D-PSGD' % unsupported)
         from ..parallel.distributed import check_slowmo_args
         check_slowmo_args(args.slowmo_frequency, args.slowmo_lr, args.slowmo_momentum)
+    check_schedule_args(args)
+    if not 0.0 <= getattr(args, 'label_smoothing', 0.0) <= 1.0:
+        raise ValueError('--label_smoothing must be in [0, 1], got %r' % (args.label_smoothing,))
     args.consensus_fname = '{}{}consensus_r{}_n{}.csv'.format(args.checkpoint_dir, args.tag, args.rank,
                                                               args.world_size)
 
@@ -291,16 +307,49 @@ def finalize_args(args, adpsgd=False):
 # --------------------------------------------------------------------------- #
 # schedules
 # --------------------------------------------------------------------------- #
+def check_schedule_args(args):
+    """ValueError for learning-rate policy flags that contradict each other."""
+    policy = getattr(args, 'lr_policy', 'step')
+    warmup_epochs = getattr(args, 'warmup_epochs', 5)
+    if warmup_epochs < 0:
+        raise ValueError('--warmup_epochs must be >= 0, got %r' % (warmup_epochs,))
+    if policy != 'poly':
+        return
+    if getattr(args, 'schedule', None) is not None:
+        raise ValueError('--schedule sets the step policy\'s factors; it cannot be combined with '
+                         '--lr_policy poly')
+    if not args.poly_power > 0:
+        raise ValueError('--poly_power must be > 0, got %r' % (args.poly_power,))
+    if not args.end_lr >= 0:
+        raise ValueError('--end_lr must be >= 0, got %r' % (args.end_lr,))
+    if args.warmup and warmup_epochs >= args.num_epochs:
+        raise ValueError('--lr_policy poly needs the warm-up (%d epochs) to end before --num_epochs (%d)'
+                         % (warmup_epochs, args.num_epochs))
+
+
 def learning_rate_at(args, epoch, itr=None, itr_per_epoch=None, scale=1):
     """Goyal et al. policy (``gossip_sgd.py:508-536``): target = lr*bs*ws/256,
-    optional 5-epoch linear warm-up from ``lr``, then multiplicative steps."""
+    optional linear warm-up from ``lr`` over ``warmup_epochs`` (default 5) epochs, then
+    multiplicative steps (``lr_policy='step'``) or polynomial decay to ``end_lr``
+    (``lr_policy='poly'``, the MLPerf ResNet-50 recipe): with ``count`` iterations done,
+    ``T`` in all and ``W`` of warm-up, ``p = clamp((count - W) / (T - W), 0, 1)`` and
+    ``lr = end_lr + (target - end_lr) * (1 - p) ** poly_power``.  So the first iteration after the
+    warm-up runs at ``target``.  Without ``itr`` the counts are whole epochs."""
     target = args.lr * args.batch_size * scale * args.world_size / 256
-    if args.warmup and epoch < 5:
+    warmup_epochs = getattr(args, 'warmup_epochs', 5)
+    if args.warmup and epoch < warmup_epochs:
         if target <= args.lr:
             return target
         assert itr is not None and itr_per_epoch is not None
         count = epoch * itr_per_epoch + itr + 1
-        return args.lr + (target - args.lr) * (count / (5 * itr_per_epoch))
+        return args.lr + (target - args.lr) * (count / (warmup_epochs * itr_per_epoch))
+    if getattr(args, 'lr_policy', 'step') == 'poly':
+        per_epoch = 1 if itr is None else itr_per_epoch
+        count = epoch * per_epoch + (0 if itr is None else itr)
+        total = args.num_epochs * per_epoch
+        warm = (warmup_epochs if args.warmup else 0) * per_epoch
+        p = min(max((count - warm) / max(total - warm, 1), 0.0), 1.0)
+        return args.end_lr + (target - args.end_lr) * (1.0 - p) ** args.poly_power
     lr = target
     for e, factor in args.lr_schedule.items():
         if epoch >= e:

@@ -126,13 +126,18 @@ def main(argv=None):
         tracing.enable(args.trace_file, rank=args.rank)
     model, optimizer = build_model_and_optimizer(args, log)
     criterion = nn.CrossEntropyLoss()      # == KLDiv(log_softmax, one_hot) of the reference
+    # the training loss carries --label_smoothing; validation keeps the plain cross-entropy so that
+    # validation losses stay comparable across runs
+    train_criterion = nn.CrossEntropyLoss(label_smoothing=args.label_smoothing)
     optimizer.zero_grad()
     args._trainer = None
     if args.cuda_graph and not args.all_reduce and args.fused and getattr(model, '_kernel', None):
+        from ..ops.fused_loss import FusedCrossEntropyWithAccuracy
         from ..parallel.trainer import GossipTrainer
-        # criterion=None: the trainer's fused softmax-xent + prec@1/5 kernel (same value as
-        # nn.CrossEntropyLoss; tests/test_fused_loss_gpu.py)
-        args._trainer = GossipTrainer(model, optimizer, None,
+        # the fused softmax-xent + prec@1/5 kernel, captured in the graph (same value as
+        # nn.CrossEntropyLoss(label_smoothing=...); tests/test_fused_loss_gpu.py)
+        args._trainer = GossipTrainer(model, optimizer,
+                                      FusedCrossEntropyWithAccuracy(label_smoothing=args.label_smoothing),
                                       amp_dtype=torch.bfloat16 if args.amp else None)
 
     state = fresh_state(model.state_dict(), optimizer.state_dict())
@@ -170,7 +175,7 @@ def main(argv=None):
         if not args.all_reduce:
             update_peers_per_itr(args, model, epoch)
             model.block()
-        train(args, model, criterion, optimizer, batch_meter, data_meter, nn_meter, loader,
+        train(args, model, train_criterion, optimizer, batch_meter, data_meter, nn_meter, loader,
               epoch, start_itr, csv, log)
         start_itr = 0
         if not args.train_fast:
@@ -247,7 +252,9 @@ def train(args, model, criterion, optimizer, batch_meter, data_meter, nn_meter, 
         t_data = time.time() - t_batch
         tracing.counter('data_ms', t_data * 1e3)
         t_nn = time.time()
-        if i % 100 == 0:
+        # the step policy changes the rate at most every 100 iterations (as the reference sets it);
+        # poly decays it every iteration (a device-resident value: no graph re-capture)
+        if i % 100 == 0 or args.lr_policy == 'poly':
             update_learning_rate(args, optimizer, epoch, itr=i, itr_per_epoch=len(loader))
         if trainer is not None:
             # whole step = one CUDA-graph replay (forward+backward+fused gossip kernel);

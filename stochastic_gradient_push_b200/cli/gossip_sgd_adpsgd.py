@@ -91,6 +91,8 @@ def main(argv=None):
         verbose=args.verbose, network_interface_type=args.network_interface_type,
         transport=args.transport)
     criterion = nn.CrossEntropyLoss()
+    # --label_smoothing applies to the training loss; validation keeps the plain cross-entropy
+    train_criterion = nn.CrossEntropyLoss(label_smoothing=args.label_smoothing)
     optimizer = torch.optim.SGD(model.parameters(), lr=args.lr, momentum=args.momentum,
                                 weight_decay=args.weight_decay, nesterov=args.nesterov)
     optimizer.zero_grad(set_to_none=False)
@@ -122,7 +124,7 @@ def main(argv=None):
     best = 0
     while global_epoch < args.num_epochs:
         sampler.set_epoch(local_epoch + args.seed * 90)
-        global_itr = train(args, model, criterion, optimizer, batch_meter, data_meter, nn_meter,
+        global_itr = train(args, model, train_criterion, optimizer, batch_meter, data_meter, nn_meter,
                            loader, local_epoch, csv, log, itr_per_epoch)
         global_epoch, _ = global_epoch_of(args, global_itr, itr_per_epoch)
         local_epoch += 1

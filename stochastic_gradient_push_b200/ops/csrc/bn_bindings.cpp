@@ -561,9 +561,16 @@ static std::vector<torch::Tensor> conv1x1_bn_forward(torch::Tensor x, torch::Ten
 // ---------------------------------------------------------------------------
 extern "C" {
 cudaError_t xent_launch_fwd(int dtype, const void* logits, const long long* target, float* lse, float* out3, int B,
-                            int C, cudaStream_t st);
+                            int C, float eps, cudaStream_t st);
 cudaError_t xent_launch_bwd(int dtype, const void* logits, const long long* target, const float* lse,
-                            const float* grad_out, void* dlogits, int B, int C, cudaStream_t st);
+                            const float* grad_out, void* dlogits, int B, int C, float eps, cudaStream_t st);
+}
+
+// torch.nn.functional.cross_entropy accepts label_smoothing in [0, 1]; so do the kernels
+static float xent_check_smoothing(double label_smoothing)
+{
+    TORCH_CHECK(label_smoothing >= 0.0 && label_smoothing <= 1.0, "label_smoothing must be in [0, 1]");
+    return (float)label_smoothing;
 }
 
 static bool xent_can_fuse(const torch::Tensor& logits, const torch::Tensor& target)
@@ -574,10 +581,11 @@ static bool xent_can_fuse(const torch::Tensor& logits, const torch::Tensor& targ
            target.size(0) == logits.size(0) && logits.size(0) > 0 && logits.size(1) > 0;
 }
 
-// returns (metrics[3] = mean loss, prec@1 %, prec@5 %; lse[B])
-static std::vector<torch::Tensor> xent_forward(torch::Tensor logits, torch::Tensor target)
+// returns (metrics[3] = mean loss (label-smoothed when label_smoothing > 0), prec@1 %, prec@5 %; lse[B])
+static std::vector<torch::Tensor> xent_forward(torch::Tensor logits, torch::Tensor target, double label_smoothing)
 {
     TORCH_CHECK(xent_can_fuse(logits, target), "xent_forward: unsupported tensors");
+    const float eps = xent_check_smoothing(label_smoothing);
     c10::cuda::CUDAGuard guard(logits.get_device());
     auto st = at::cuda::getCurrentCUDAStream();
     auto fopt = torch::TensorOptions().dtype(torch::kFloat32).device(logits.device());
@@ -587,20 +595,21 @@ static std::vector<torch::Tensor> xent_forward(torch::Tensor logits, torch::Tens
     BN_CHECK(cudaMemsetAsync(out3.data_ptr(), 0, 3 * sizeof(float), st));
     BN_CHECK(xent_launch_fwd(dtype_code(logits), logits.data_ptr(),
                              reinterpret_cast<const long long*>(target.data_ptr<int64_t>()),
-                             lse.data_ptr<float>(), out3.data_ptr<float>(), B, C, st));
+                             lse.data_ptr<float>(), out3.data_ptr<float>(), B, C, eps, st));
     return {out3, lse};
 }
 
 static torch::Tensor xent_backward(torch::Tensor logits, torch::Tensor target, torch::Tensor lse,
-                                   torch::Tensor grad_out)
+                                   torch::Tensor grad_out, double label_smoothing)
 {
     TORCH_CHECK(xent_can_fuse(logits, target) && lse.is_cuda() && lse.scalar_type() == torch::kFloat32 &&
                 grad_out.is_cuda() && grad_out.scalar_type() == torch::kFloat32 && grad_out.numel() == 1);
+    const float eps = xent_check_smoothing(label_smoothing);
     c10::cuda::CUDAGuard guard(logits.get_device());
     auto dl = torch::empty_like(logits);
     BN_CHECK(xent_launch_bwd(dtype_code(logits), logits.data_ptr(),
                              reinterpret_cast<const long long*>(target.data_ptr<int64_t>()), lse.data_ptr<float>(),
-                             grad_out.data_ptr<float>(), dl.data_ptr(), (int)logits.size(0), (int)logits.size(1),
+                             grad_out.data_ptr<float>(), dl.data_ptr(), (int)logits.size(0), (int)logits.size(1), eps,
                              at::cuda::getCurrentCUDAStream()));
     return dl;
 }
@@ -608,8 +617,9 @@ static torch::Tensor xent_backward(torch::Tensor logits, torch::Tensor target, t
 void bind_bn(py::module& mod)
 {
     mod.def("xent_can_fuse", &xent_can_fuse);
-    mod.def("xent_forward", &xent_forward);
-    mod.def("xent_backward", &xent_backward);
+    mod.def("xent_forward", &xent_forward, py::arg("logits"), py::arg("target"), py::arg("label_smoothing") = 0.0);
+    mod.def("xent_backward", &xent_backward, py::arg("logits"), py::arg("target"), py::arg("lse"),
+            py::arg("grad_out"), py::arg("label_smoothing") = 0.0);
     mod.def("conv1x1_can_fuse", &conv1x1_can_fuse);
     mod.def("conv1x1_plan", &conv1x1_plan, py::arg("M"), py::arg("N"), py::arg("K"), py::arg("num_sms") = 132,
             py::arg("residual") = false, py::arg("f32") = false, py::arg("bn_reduce") = false);

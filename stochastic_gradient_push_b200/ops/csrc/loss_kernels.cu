@@ -11,6 +11,14 @@
 //             loss_i = lse - z_t ; rank_i = #{ j : z_j > z_t }   (top-k hit <=> rank < k)
 //             out[0] += loss_i / B ; out[1] += 100/B [rank == 0] ; out[2] += 100/B [rank < 5]
 //   backward: dz_ij = g * (exp(z_ij - lse_i) - [j == t_i]) / B
+//
+// Label smoothing eps (torch.nn.functional.cross_entropy(label_smoothing=eps), mean reduction):
+//   forward : loss_i = lse_i - (1 - eps) z_t - (eps / C) sum_j z_j   (sum_j z_j: one more per-lane
+//             accumulator in the same pass, so each logit is still read once)
+//   backward: dz_ij = g * (exp(z_ij - lse_i) - (1 - eps)[j == t_i] - eps / C) / B
+// SMOOTH is a template parameter: eps == 0 launches the SMOOTH = false kernels, whose code is the
+// unsmoothed kernels' instruction for instruction (no 0 * sum_j z_j, which is NaN for inf logits).
+// A row whose target is out of range adds no loss and gets a zero gradient either way.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -39,10 +47,10 @@ __device__ __forceinline__ float warp_sum(float v)
     return v;
 }
 
-template <typename T>
+template <typename T, bool SMOOTH>
 __global__ void __launch_bounds__(XE_THREADS)
 xent_fwd_kernel(const T* __restrict__ logits, const long long* __restrict__ target, float* __restrict__ lse_out,
-                float* __restrict__ out3, int B, int C)
+                float* __restrict__ out3, int B, int C, float eps)
 {
     __shared__ float s_acc[3];
     if (threadIdx.x < 3) s_acc[threadIdx.x] = 0.f;
@@ -56,23 +64,26 @@ xent_fwd_kernel(const T* __restrict__ logits, const long long* __restrict__ targ
         if (!valid) t = 0;
         const float zt = to_f<T>(z[t]);
         // online softmax: one pass for max + sum, rank counted in the same pass
-        float m = -INFINITY, s = 0.f, above = 0.f;
+        float m = -INFINITY, s = 0.f, above = 0.f, sum_z = 0.f;
         for (int j = lane; j < C; j += 32) {
             const float v = to_f<T>(z[j]);
             const float mn = fmaxf(m, v);
             s = s * __expf(m - mn) + __expf(v - mn);
             m = mn;
             above += (v > zt) ? 1.f : 0.f;
+            if (SMOOTH) sum_z += v;
         }
         const float mw = warp_max(m);
         s = warp_sum(s * __expf(m - mw));
         above = warp_sum(above);
+        if (SMOOTH) sum_z = warp_sum(sum_z);
         const float lse = mw + __logf(s);
         if (lane == 0) {
             lse_out[row] = lse;
             if (valid) {
                 const float inv_b = 1.f / (float)B;
-                atomicAdd(&s_acc[0], (lse - zt) * inv_b);
+                const float loss = SMOOTH ? lse - (1.f - eps) * zt - eps * (sum_z / (float)C) : lse - zt;
+                atomicAdd(&s_acc[0], loss * inv_b);
                 if (above < 0.5f) atomicAdd(&s_acc[1], 100.f * inv_b);
                 if (above < 4.5f) atomicAdd(&s_acc[2], 100.f * inv_b);
             }
@@ -82,10 +93,10 @@ xent_fwd_kernel(const T* __restrict__ logits, const long long* __restrict__ targ
     if (threadIdx.x < 3) atomicAdd(out3 + threadIdx.x, s_acc[threadIdx.x]);
 }
 
-template <typename T>
+template <typename T, bool SMOOTH>
 __global__ void __launch_bounds__(XE_THREADS)
 xent_bwd_kernel(const T* __restrict__ logits, const long long* __restrict__ target, const float* __restrict__ lse,
-                const float* __restrict__ grad_out, T* __restrict__ dlogits, int B, int C)
+                const float* __restrict__ grad_out, T* __restrict__ dlogits, int B, int C, float eps)
 {
     const int lane = threadIdx.x & 31;
     const int row = blockIdx.x * (XE_THREADS / 32) + (threadIdx.x >> 5);
@@ -96,9 +107,12 @@ xent_bwd_kernel(const T* __restrict__ logits, const long long* __restrict__ targ
     const long long t = target[row];
     const bool valid = t >= 0 && t < C;
     const float l = lse[row];
+    const float eps_c = SMOOTH ? eps / (float)C : 0.f;        // smoothed target mass of every class
+    const float hit = SMOOTH ? 1.f - eps + eps_c : 1.f;       // ... and of the target class
     for (int j = lane; j < C; j += 32) {
         float p = __expf(to_f<T>(z[j]) - l);
-        if (j == t) p -= 1.f;
+        if (j == t) p -= hit;
+        else if (SMOOTH) p -= eps_c;
         dz[j] = from_f<T>(valid ? g * p : 0.f);
     }
 }
@@ -107,28 +121,36 @@ xent_bwd_kernel(const T* __restrict__ logits, const long long* __restrict__ targ
 
 extern "C" {
 
-// dtype: 0 = bf16 logits, 1 = fp32 logits; out3 must be zeroed by the caller (same stream)
+// dtype: 0 = bf16 logits, 1 = fp32 logits; out3 must be zeroed by the caller (same stream);
+// eps = label smoothing in [0, 1] (checked by the caller), 0 = plain cross-entropy
 cudaError_t xent_launch_fwd(int dtype, const void* logits, const long long* target, float* lse, float* out3, int B,
-                            int C, cudaStream_t st)
+                            int C, float eps, cudaStream_t st)
 {
     const int grid = (B + XE_THREADS / 32 - 1) / (XE_THREADS / 32);
-    if (dtype == 0)
-        xent_fwd_kernel<__nv_bfloat16><<<grid, XE_THREADS, 0, st>>>((const __nv_bfloat16*)logits, target, lse, out3, B, C);
-    else
-        xent_fwd_kernel<float><<<grid, XE_THREADS, 0, st>>>((const float*)logits, target, lse, out3, B, C);
+    const bool smooth = eps != 0.f;
+    if (dtype == 0) {
+        auto k = smooth ? xent_fwd_kernel<__nv_bfloat16, true> : xent_fwd_kernel<__nv_bfloat16, false>;
+        k<<<grid, XE_THREADS, 0, st>>>((const __nv_bfloat16*)logits, target, lse, out3, B, C, eps);
+    } else {
+        auto k = smooth ? xent_fwd_kernel<float, true> : xent_fwd_kernel<float, false>;
+        k<<<grid, XE_THREADS, 0, st>>>((const float*)logits, target, lse, out3, B, C, eps);
+    }
     return cudaGetLastError();
 }
 
 cudaError_t xent_launch_bwd(int dtype, const void* logits, const long long* target, const float* lse,
-                            const float* grad_out, void* dlogits, int B, int C, cudaStream_t st)
+                            const float* grad_out, void* dlogits, int B, int C, float eps, cudaStream_t st)
 {
     const int grid = (B + XE_THREADS / 32 - 1) / (XE_THREADS / 32);
-    if (dtype == 0)
-        xent_bwd_kernel<__nv_bfloat16><<<grid, XE_THREADS, 0, st>>>((const __nv_bfloat16*)logits, target, lse, grad_out,
-                                                                   (__nv_bfloat16*)dlogits, B, C);
-    else
-        xent_bwd_kernel<float><<<grid, XE_THREADS, 0, st>>>((const float*)logits, target, lse, grad_out,
-                                                           (float*)dlogits, B, C);
+    const bool smooth = eps != 0.f;
+    if (dtype == 0) {
+        auto k = smooth ? xent_bwd_kernel<__nv_bfloat16, true> : xent_bwd_kernel<__nv_bfloat16, false>;
+        k<<<grid, XE_THREADS, 0, st>>>((const __nv_bfloat16*)logits, target, lse, grad_out, (__nv_bfloat16*)dlogits,
+                                       B, C, eps);
+    } else {
+        auto k = smooth ? xent_bwd_kernel<float, true> : xent_bwd_kernel<float, false>;
+        k<<<grid, XE_THREADS, 0, st>>>((const float*)logits, target, lse, grad_out, (float*)dlogits, B, C, eps);
+    }
     return cudaGetLastError();
 }
 

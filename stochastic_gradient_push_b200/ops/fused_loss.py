@@ -13,6 +13,14 @@ without ever blocking the host (``parallel/trainer.py``).
 leaves ``criterion.metrics`` = device tensor ``[loss, prec@1 %, prec@5 %]``.
 CPU tensors / unsupported dtypes run the plain PyTorch composition, which is
 also the oracle in ``tests/test_fused_loss_gpu.py``.
+
+Label smoothing (``label_smoothing=eps``, in [0, 1]) follows
+``torch.nn.functional.cross_entropy(label_smoothing=eps)``:
+``loss_i = lse_i - (1 - eps) z_{i,t} - (eps / C) sum_j z_{i,j}``, averaged over the batch, and
+``metrics[0]`` is that smoothed loss (the one training minimises); prec@1 / prec@5 do not depend
+on eps.  The reference's KL divergence against the smoothed one-hot target would be lower by the
+constant entropy of that target, with the same gradient.  ``eps = 0`` runs exactly the
+unsmoothed kernels.
 """
 
 from __future__ import annotations
@@ -24,9 +32,18 @@ import torch.nn.functional as F
 from . import native
 
 
-def reference_loss_and_accuracy(logits: torch.Tensor, target: torch.Tensor):
-    """(loss, prec@1 %, prec@5 %) the way the reference's loop computes them."""
-    loss = F.cross_entropy(logits.float(), target)
+def check_label_smoothing(label_smoothing) -> float:
+    eps = float(label_smoothing)
+    if not 0.0 <= eps <= 1.0:
+        raise ValueError('label_smoothing must be in [0, 1], got %r' % (label_smoothing,))
+    return eps
+
+
+def reference_loss_and_accuracy(logits: torch.Tensor, target: torch.Tensor, label_smoothing: float = 0.0):
+    """(loss, prec@1 %, prec@5 %) the way the reference's loop computes them (loss with
+    ``F.cross_entropy(label_smoothing=...)``)."""
+    eps = check_label_smoothing(label_smoothing)
+    loss = F.cross_entropy(logits.float(), target, label_smoothing=eps)
     with torch.no_grad():
         k = min(5, logits.shape[1])
         _, pred = logits.float().topk(k, 1, True, True)
@@ -40,10 +57,11 @@ def reference_loss_and_accuracy(logits: torch.Tensor, target: torch.Tensor):
 class _FusedXent(torch.autograd.Function):
 
     @staticmethod
-    def forward(ctx, logits, target):
+    def forward(ctx, logits, target, label_smoothing):
         C = native.load()
-        metrics, lse = C.xent_forward(logits, target)
+        metrics, lse = C.xent_forward(logits, target, label_smoothing)
         ctx.save_for_backward(logits, target, lse)
+        ctx.label_smoothing = label_smoothing
         ctx.mark_non_differentiable(metrics)
         return metrics[0], metrics
 
@@ -52,27 +70,34 @@ class _FusedXent(torch.autograd.Function):
         C = native.load()
         logits, target, lse = ctx.saved_tensors
         g = g_loss.reshape(1).to(torch.float32)
-        return C.xent_backward(logits, target, lse, g), None
+        return C.xent_backward(logits, target, lse, g, ctx.label_smoothing), None, None
 
 
-def fused_cross_entropy(logits: torch.Tensor, target: torch.Tensor):
-    """Returns ``(loss, metrics)``; ``metrics = [loss, prec@1 %, prec@5 %]`` (fp32, detached)."""
+def fused_cross_entropy(logits: torch.Tensor, target: torch.Tensor, label_smoothing: float = 0.0):
+    """Returns ``(loss, metrics)``; ``metrics = [loss, prec@1 %, prec@5 %]`` (fp32, detached).
+    ``label_smoothing`` in [0, 1], as in ``F.cross_entropy``."""
+    eps = check_label_smoothing(label_smoothing)
     if logits.is_cuda and native.available():
         lg = logits if logits.is_contiguous() else logits.contiguous()
         if native.load().xent_can_fuse(lg, target):
-            loss, metrics = _FusedXent.apply(lg, target)
+            loss, metrics = _FusedXent.apply(lg, target, eps)
             return loss, metrics
-    loss, p1, p5 = reference_loss_and_accuracy(logits, target)
+    loss, p1, p5 = reference_loss_and_accuracy(logits, target, eps)
     return loss, torch.stack([loss.detach().float(), p1, p5])
 
 
 class FusedCrossEntropyWithAccuracy(nn.Module):
-    """Drop-in for ``nn.CrossEntropyLoss()`` (mean reduction) that also measures accuracy."""
+    """Drop-in for ``nn.CrossEntropyLoss(label_smoothing=label_smoothing)`` (mean reduction) that
+    also measures accuracy."""
 
-    def __init__(self):
+    def __init__(self, label_smoothing: float = 0.0):
         super().__init__()
+        self.label_smoothing = check_label_smoothing(label_smoothing)
         self.metrics = None
 
     def forward(self, logits, target):
-        loss, self.metrics = fused_cross_entropy(logits, target)
+        loss, self.metrics = fused_cross_entropy(logits, target, self.label_smoothing)
         return loss
+
+    def extra_repr(self):
+        return 'label_smoothing=%g' % self.label_smoothing if self.label_smoothing else ''

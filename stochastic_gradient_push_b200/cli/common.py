@@ -89,6 +89,17 @@ def build_parser(adpsgd: bool = False) -> argparse.ArgumentParser:
                    help='label smoothing eps in [0, 1] of the training loss (as in '
                         'torch.nn.CrossEntropyLoss(label_smoothing=eps); on the fused loss kernel with '
                         '--cuda_graph True); validation keeps the plain cross-entropy')
+    p.add_argument('--mixup_alpha', default=0.0, type=float,
+                   help='mixup (Zhang et al. 2018) on the training batch: lam ~ Beta(a, a), each image mixed '
+                        'with its partner in the flipped batch, two-target loss; 0 = off.  Fused into the '
+                        'input copy and the fused loss kernel with --cuda_graph True; validation is never mixed')
+    p.add_argument('--cutmix_alpha', default=0.0, type=float,
+                   help='CutMix (Yun et al. 2019): a box of area 1 - lam, lam ~ Beta(a, a), pasted from the '
+                        'partner image; 0 = off.  With --mixup_alpha too, one of the two per step')
+    p.add_argument('--mix_prob', default=1.0, type=float,
+                   help='probability that a training step is mixed (mixup or CutMix)')
+    p.add_argument('--mix_switch_prob', default=0.5, type=float,
+                   help='with both alphas > 0: probability that a mixed step uses CutMix rather than mixup')
     p.add_argument('--seed', default=47, type=int)
     p.add_argument('--resume', default=False, **B)
     p.add_argument('--backend', default='nccl', choices=['nccl', 'gloo', 'mpi'])
@@ -264,6 +275,7 @@ def finalize_args(args, adpsgd=False):
     check_schedule_args(args)
     if not 0.0 <= getattr(args, 'label_smoothing', 0.0) <= 1.0:
         raise ValueError('--label_smoothing must be in [0, 1], got %r' % (args.label_smoothing,))
+    check_mix_flags(args)
     args.consensus_fname = '{}{}consensus_r{}_n{}.csv'.format(args.checkpoint_dir, args.tag, args.rank,
                                                               args.world_size)
 
@@ -307,6 +319,18 @@ def finalize_args(args, adpsgd=False):
 # --------------------------------------------------------------------------- #
 # schedules
 # --------------------------------------------------------------------------- #
+def check_mix_flags(args):
+    """ValueError for mixup / CutMix flags out of range."""
+    for flag in ('mixup_alpha', 'cutmix_alpha'):
+        v = getattr(args, flag, 0.0)
+        if not 0.0 <= v < float('inf'):
+            raise ValueError('--%s must be a finite value >= 0, got %r' % (flag, v))
+    for flag in ('mix_prob', 'mix_switch_prob'):
+        v = getattr(args, flag, 0.0)
+        if not 0.0 <= v <= 1.0:
+            raise ValueError('--%s must be in [0, 1], got %r' % (flag, v))
+
+
 def check_schedule_args(args):
     """ValueError for learning-rate policy flags that contradict each other."""
     policy = getattr(args, 'lr_policy', 'step')
@@ -455,6 +479,34 @@ def device_batch(args, batch, train=True):
         from ..data import GpuAugment
         aug = args._gpu_augment = GpuAugment(out_size=args.image_size, seed=args.seed * 7919 + args.rank)
     return aug(batch.to(args.device, non_blocking=True), train=train)
+
+
+def make_batch_mix(args):
+    """The training batches' ``ops.batch_mix.BatchMix`` for --mixup_alpha / --cutmix_alpha (None
+    when both are 0): one draw per step, a pure function of (--seed, rank, iteration)."""
+    if not (getattr(args, 'mixup_alpha', 0.0) > 0 or getattr(args, 'cutmix_alpha', 0.0) > 0):
+        return None
+    from ..ops.batch_mix import BatchMix
+    return BatchMix(args.mixup_alpha, args.cutmix_alpha, args.mix_prob, args.mix_switch_prob,
+                    seed=args.seed, rank=args.rank)
+
+
+def mix_train_batch(args, batch_mix, batch, itr):
+    """Eager training loops: the batch of iteration ``itr`` mixed on ``args.device`` (the sm_90a
+    kernel on CUDA) and the mix state its loss needs."""
+    if batch.device.type != torch.device(args.device).type:
+        batch = batch.to(args.device, non_blocking=True)
+    batch_mix.iteration = itr
+    return batch_mix.apply(batch), batch_mix.state
+
+
+def train_loss(criterion, output, target, mix, label_smoothing):
+    """Training loss of the eager loops: ``criterion`` or, for a mixed batch, the two-target
+    cross-entropy (fused kernel on CUDA) with the same label smoothing."""
+    if mix is None:
+        return criterion(output.float(), target)
+    from ..ops.fused_loss import fused_cross_entropy
+    return fused_cross_entropy(output.float(), target, label_smoothing, mix=mix)[0]
 
 
 # --------------------------------------------------------------------------- #

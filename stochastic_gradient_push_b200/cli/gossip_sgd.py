@@ -130,6 +130,8 @@ def main(argv=None):
     # validation losses stay comparable across runs
     train_criterion = nn.CrossEntropyLoss(label_smoothing=args.label_smoothing)
     optimizer.zero_grad()
+    # --mixup_alpha / --cutmix_alpha: training batches only (validate() never mixes)
+    args._batch_mix = common.make_batch_mix(args)
     args._trainer = None
     if args.cuda_graph and not args.all_reduce and args.fused and getattr(model, '_kernel', None):
         from ..ops.fused_loss import FusedCrossEntropyWithAccuracy
@@ -138,7 +140,8 @@ def main(argv=None):
         # nn.CrossEntropyLoss(label_smoothing=...); tests/test_fused_loss_gpu.py)
         args._trainer = GossipTrainer(model, optimizer,
                                       FusedCrossEntropyWithAccuracy(label_smoothing=args.label_smoothing),
-                                      amp_dtype=torch.bfloat16 if args.amp else None)
+                                      amp_dtype=torch.bfloat16 if args.amp else None,
+                                      batch_mix=args._batch_mix)
 
     state = fresh_state(model.state_dict(), optimizer.state_dict())
     cmanager = ClusterManager(rank=args.rank, world_size=args.world_size, model_tag=args.tag,
@@ -235,6 +238,7 @@ def train(args, model, criterion, optimizer, batch_meter, data_meter, nn_meter, 
     # back once per print interval (the reference syncs 3x per iteration)
     pending = []
     trainer = getattr(args, '_trainer', None)
+    batch_mix = getattr(args, '_batch_mix', None)
     it = iter(loader)
     for _ in range(itr):            # resume mid-epoch: skip what was already consumed
         next(it, None)
@@ -256,6 +260,12 @@ def train(args, model, criterion, optimizer, batch_meter, data_meter, nn_meter, 
         # poly decays it every iteration (a device-resident value: no graph re-capture)
         if i % 100 == 0 or args.lr_policy == 'poly':
             update_learning_rate(args, optimizer, epoch, itr=i, itr_per_epoch=len(loader))
+        mix = None
+        if batch_mix is not None:               # this iteration's draw: resumes reproduce it
+            if trainer is not None:
+                batch_mix.iteration = epoch * len(loader) + i
+            else:
+                batch, mix = common.mix_train_batch(args, batch_mix, batch, epoch * len(loader) + i)
         if trainer is not None:
             # whole step = one CUDA-graph replay (forward+backward+fused gossip kernel);
             # the metrics are computed on the trainer's stream, before the next replay
@@ -268,7 +278,7 @@ def train(args, model, criterion, optimizer, batch_meter, data_meter, nn_meter, 
         else:
             with tracing.span('forward', itr=i), _autocast(args):
                 output = model(batch)
-                loss = criterion(output.float(), target)
+                loss = common.train_loss(criterion, output, target, mix, args.label_smoothing)
             with tracing.span('backward'):
                 loss.backward()
             with tracing.span('optimizer'):

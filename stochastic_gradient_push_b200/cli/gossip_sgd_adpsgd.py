@@ -32,7 +32,7 @@ from .common import (CSVLog, Meter, accuracy, build_parser, finalize_args, fresh
                      init_model, learning_rate_at, make_dataloader, update_state)
 from ..experiment import ClusterManager, make_logger
 from ..utils import tracing
-from .common import device_batch
+from .common import device_batch, make_batch_mix, mix_train_batch, train_loss
 
 
 def parse_args(argv=None):
@@ -96,6 +96,8 @@ def main(argv=None):
     optimizer = torch.optim.SGD(model.parameters(), lr=args.lr, momentum=args.momentum,
                                 weight_decay=args.weight_decay, nesterov=args.nesterov)
     optimizer.zero_grad(set_to_none=False)
+    # --mixup_alpha / --cutmix_alpha: training batches only (validate() never mixes)
+    args._batch_mix = make_batch_mix(args)
 
     state = fresh_state(model.state_dict(), optimizer.state_dict())
     cmanager = ClusterManager(rank=args.rank, world_size=args.world_size, model_tag=args.tag,
@@ -160,6 +162,7 @@ def train(args, model, criterion, optimizer, batch_meter, data_meter, nn_meter, 
     model.enable_gossip()
     dev = args.device
     amp = bool(args.amp and dev == 'cuda')
+    batch_mix = getattr(args, '_batch_mix', None)
     global_itr = update_global_iteration_counter(args, 0)
     since_sync = 0
     t_batch = time.time()
@@ -171,9 +174,12 @@ def train(args, model, criterion, optimizer, batch_meter, data_meter, nn_meter, 
         t_nn = time.time()
         if tracing.get_tracer().enabled and i >= args.trace_iters:
             log.info('trace written to %s' % tracing.disable().dump())
+        mix = None
+        if batch_mix is not None:            # keyed by this rank's own iteration count
+            batch, mix = mix_train_batch(args, batch_mix, batch, epoch * itr_per_epoch + i)
         with tracing.span('forward', itr=i), torch.autocast('cuda', dtype=torch.bfloat16, enabled=amp):
             output = model(batch)
-            loss = criterion(output.float(), target)
+            loss = train_loss(criterion, output, target, mix, args.label_smoothing)
         with tracing.span('backward+exchange'):
             loss.backward()      # end-of-backward hook: push grads, pull the gossip model
         with tracing.span('optimizer'):

@@ -561,9 +561,13 @@ static std::vector<torch::Tensor> conv1x1_bn_forward(torch::Tensor x, torch::Ten
 // ---------------------------------------------------------------------------
 extern "C" {
 cudaError_t xent_launch_fwd(int dtype, const void* logits, const long long* target, float* lse, float* out3, int B,
-                            int C, float eps, cudaStream_t st);
+                            int C, float eps, const float* mix, cudaStream_t st);
 cudaError_t xent_launch_bwd(int dtype, const void* logits, const long long* target, const float* lse,
-                            const float* grad_out, void* dlogits, int B, int C, float eps, cudaStream_t st);
+                            const float* grad_out, void* dlogits, int B, int C, float eps, const float* mix,
+                            cudaStream_t st);
+cudaError_t batch_mix_launch(int out_dtype, const float* src, void* dst, const float* mix, int B, int C, int H,
+                             int W, long long s_n, int s_c, int s_p, long long d_n, int d_c, int d_p,
+                             cudaStream_t st);
 }
 
 // torch.nn.functional.cross_entropy accepts label_smoothing in [0, 1]; so do the kernels
@@ -581,11 +585,25 @@ static bool xent_can_fuse(const torch::Tensor& logits, const torch::Tensor& targ
            target.size(0) == logits.size(0) && logits.size(0) > 0 && logits.size(1) > 0;
 }
 
-// returns (metrics[3] = mean loss (label-smoothed when label_smoothing > 0), prec@1 %, prec@5 %; lse[B])
-static std::vector<torch::Tensor> xent_forward(torch::Tensor logits, torch::Tensor target, double label_smoothing)
+// mixup / CutMix state (ops/batch_mix.py): fp32 [lam, mode, y0, y1, x0, x1] on the logits' device;
+// None = one target per row (the MIX = false kernels)
+static const float* xent_mix_ptr(const c10::optional<torch::Tensor>& mix, const torch::Tensor& logits)
+{
+    if (!mix.has_value() || !mix->defined()) return nullptr;
+    TORCH_CHECK(mix->is_cuda() && mix->get_device() == logits.get_device() && mix->scalar_type() == torch::kFloat32 &&
+                    mix->is_contiguous() && mix->numel() >= 6,
+                "mix must be the fp32 device mix state [lam, mode, y0, y1, x0, x1] on the logits' device");
+    return mix->data_ptr<float>();
+}
+
+// returns (metrics[3] = mean loss (label-smoothed when label_smoothing > 0), prec@1 %, prec@5 %; lse[B]);
+// with mix: the two-target loss lam CE(z_i, t_i) + (1 - lam) CE(z_i, t_{B-1-i})
+static std::vector<torch::Tensor> xent_forward(torch::Tensor logits, torch::Tensor target, double label_smoothing,
+                                               c10::optional<torch::Tensor> mix)
 {
     TORCH_CHECK(xent_can_fuse(logits, target), "xent_forward: unsupported tensors");
     const float eps = xent_check_smoothing(label_smoothing);
+    const float* mixp = xent_mix_ptr(mix, logits);
     c10::cuda::CUDAGuard guard(logits.get_device());
     auto st = at::cuda::getCurrentCUDAStream();
     auto fopt = torch::TensorOptions().dtype(torch::kFloat32).device(logits.device());
@@ -595,31 +613,68 @@ static std::vector<torch::Tensor> xent_forward(torch::Tensor logits, torch::Tens
     BN_CHECK(cudaMemsetAsync(out3.data_ptr(), 0, 3 * sizeof(float), st));
     BN_CHECK(xent_launch_fwd(dtype_code(logits), logits.data_ptr(),
                              reinterpret_cast<const long long*>(target.data_ptr<int64_t>()),
-                             lse.data_ptr<float>(), out3.data_ptr<float>(), B, C, eps, st));
+                             lse.data_ptr<float>(), out3.data_ptr<float>(), B, C, eps, mixp, st));
     return {out3, lse};
 }
 
 static torch::Tensor xent_backward(torch::Tensor logits, torch::Tensor target, torch::Tensor lse,
-                                   torch::Tensor grad_out, double label_smoothing)
+                                   torch::Tensor grad_out, double label_smoothing, c10::optional<torch::Tensor> mix)
 {
     TORCH_CHECK(xent_can_fuse(logits, target) && lse.is_cuda() && lse.scalar_type() == torch::kFloat32 &&
                 grad_out.is_cuda() && grad_out.scalar_type() == torch::kFloat32 && grad_out.numel() == 1);
     const float eps = xent_check_smoothing(label_smoothing);
+    const float* mixp = xent_mix_ptr(mix, logits);
     c10::cuda::CUDAGuard guard(logits.get_device());
     auto dl = torch::empty_like(logits);
     BN_CHECK(xent_launch_bwd(dtype_code(logits), logits.data_ptr(),
                              reinterpret_cast<const long long*>(target.data_ptr<int64_t>()), lse.data_ptr<float>(),
                              grad_out.data_ptr<float>(), dl.data_ptr(), (int)logits.size(0), (int)logits.size(1), eps,
-                             at::cuda::getCurrentCUDAStream()));
+                             mixp, at::cuda::getCurrentCUDAStream()));
     return dl;
+}
+
+// ---------------------------------------------------------------------------
+// mixup / CutMix inside the stage -> static input copy (csrc/mix_kernels.cu)
+// ---------------------------------------------------------------------------
+// NCHW or NHWC dense: pixel (h, w) at h * W * sp + w * sp
+static bool mix_layout_ok(const torch::Tensor& t)
+{
+    return t.dim() == 4 && (t.is_contiguous() || t.is_contiguous(at::MemoryFormat::ChannelsLast));
+}
+
+// out <- src with row i mixed with row B-1-i as the device mix state says (mode 0 = plain copy)
+static void batch_mix(torch::Tensor src, torch::Tensor out, torch::Tensor mix)
+{
+    TORCH_CHECK(src.is_cuda() && src.scalar_type() == torch::kFloat32 && mix_layout_ok(src),
+                "batch_mix: src must be a 4-d NCHW or NHWC fp32 CUDA tensor");
+    TORCH_CHECK(out.is_cuda() && out.get_device() == src.get_device() &&
+                    (out.scalar_type() == torch::kFloat32 || out.scalar_type() == torch::kBFloat16) &&
+                    mix_layout_ok(out) && out.sizes() == src.sizes(),
+                "batch_mix: out must be a 4-d NCHW or NHWC fp32 / bf16 tensor of src's shape on its device");
+    TORCH_CHECK(mix.is_cuda() && mix.get_device() == src.get_device() && mix.scalar_type() == torch::kFloat32 &&
+                    mix.is_contiguous() && mix.numel() >= 6,
+                "batch_mix: mix must be the fp32 device mix state [lam, mode, y0, y1, x0, x1]");
+    const long long B = src.size(0), C = src.size(1), H = src.size(2), W = src.size(3);
+    TORCH_CHECK(C * H * W < (1LL << 31), "batch_mix: one image must have fewer than 2^31 elements");
+    const char* s0 = (const char*)src.data_ptr();
+    const char* o0 = (const char*)out.data_ptr();
+    TORCH_CHECK(o0 + out.nbytes() <= s0 || s0 + src.nbytes() <= o0, "batch_mix: src and out must not overlap");
+    if (B == 0 || H * W == 0 || C == 0) return;
+    c10::cuda::CUDAGuard guard(src.get_device());
+    BN_CHECK(batch_mix_launch(dtype_code(out), src.data_ptr<float>(), out.data_ptr(), mix.data_ptr<float>(), (int)B,
+                              (int)C, (int)H, (int)W, src.stride(0), (int)src.stride(1), (int)src.stride(3),
+                              out.stride(0), (int)out.stride(1), (int)out.stride(3),
+                              at::cuda::getCurrentCUDAStream()));
 }
 
 void bind_bn(py::module& mod)
 {
     mod.def("xent_can_fuse", &xent_can_fuse);
-    mod.def("xent_forward", &xent_forward, py::arg("logits"), py::arg("target"), py::arg("label_smoothing") = 0.0);
+    mod.def("xent_forward", &xent_forward, py::arg("logits"), py::arg("target"), py::arg("label_smoothing") = 0.0,
+            py::arg("mix") = py::none());
     mod.def("xent_backward", &xent_backward, py::arg("logits"), py::arg("target"), py::arg("lse"),
-            py::arg("grad_out"), py::arg("label_smoothing") = 0.0);
+            py::arg("grad_out"), py::arg("label_smoothing") = 0.0, py::arg("mix") = py::none());
+    mod.def("batch_mix", &batch_mix, py::arg("src"), py::arg("out"), py::arg("mix"));
     mod.def("conv1x1_can_fuse", &conv1x1_can_fuse);
     mod.def("conv1x1_plan", &conv1x1_plan, py::arg("M"), py::arg("N"), py::arg("K"), py::arg("num_sms") = 132,
             py::arg("residual") = false, py::arg("f32") = false, py::arg("bn_reduce") = false);

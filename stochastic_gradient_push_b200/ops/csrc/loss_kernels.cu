@@ -19,6 +19,17 @@
 // SMOOTH is a template parameter: eps == 0 launches the SMOOTH = false kernels, whose code is the
 // unsmoothed kernels' instruction for instruction (no 0 * sum_j z_j, which is NaN for inf logits).
 // A row whose target is out of range adds no loss and gets a zero gradient either way.
+//
+// Two targets (mixup / CutMix, ops/batch_mix.py): row i's partner is row B-1-i (the flipped
+// batch), with target b = t_{B-1-i} and the mix weight lam read from the device mix state
+// (mix[0], written by an H2D copy each step: a captured graph never re-captures):
+//   forward : loss_i = lse_i - (1 - eps)(lam z_a + (1 - lam) z_b) - (eps / C) sum_j z_j
+//             (one more logit read per row); prec@1 / prec@5 count against the row's own target a
+//   backward: dz_ij = g * (exp(z_ij - lse_i) - (1 - eps)(lam [j == a] + (1 - lam)[j == b]) - eps / C) / B
+// MIX is a template parameter next to SMOOTH: without a mix state the MIX = false kernels run,
+// whose code is the one-target kernels' (the mix pointer is a trailing, unused argument).  A row
+// whose target or partner target is out of range adds no loss and gets a zero gradient; its
+// accuracy still counts against its own target.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -47,10 +58,10 @@ __device__ __forceinline__ float warp_sum(float v)
     return v;
 }
 
-template <typename T, bool SMOOTH>
+template <typename T, bool SMOOTH, bool MIX>
 __global__ void __launch_bounds__(XE_THREADS)
 xent_fwd_kernel(const T* __restrict__ logits, const long long* __restrict__ target, float* __restrict__ lse_out,
-                float* __restrict__ out3, int B, int C, float eps)
+                float* __restrict__ out3, int B, int C, float eps, const float* __restrict__ mix)
 {
     __shared__ float s_acc[3];
     if (threadIdx.x < 3) s_acc[threadIdx.x] = 0.f;
@@ -63,6 +74,14 @@ xent_fwd_kernel(const T* __restrict__ logits, const long long* __restrict__ targ
         const bool valid = t >= 0 && t < C;
         if (!valid) t = 0;
         const float zt = to_f<T>(z[t]);
+        float zb = 0.f;
+        bool valid_b = true;
+        if (MIX) {
+            long long tb = target[B - 1 - row];
+            valid_b = tb >= 0 && tb < C;
+            if (!valid_b) tb = 0;
+            zb = to_f<T>(z[tb]);
+        }
         // online softmax: one pass for max + sum, rank counted in the same pass
         float m = -INFINITY, s = 0.f, above = 0.f, sum_z = 0.f;
         for (int j = lane; j < C; j += 32) {
@@ -82,8 +101,15 @@ xent_fwd_kernel(const T* __restrict__ logits, const long long* __restrict__ targ
             lse_out[row] = lse;
             if (valid) {
                 const float inv_b = 1.f / (float)B;
-                const float loss = SMOOTH ? lse - (1.f - eps) * zt - eps * (sum_z / (float)C) : lse - zt;
-                atomicAdd(&s_acc[0], loss * inv_b);
+                if (MIX) {
+                    const float lam = mix[0];
+                    const float zm = lam * zt + (1.f - lam) * zb;
+                    const float loss = SMOOTH ? lse - (1.f - eps) * zm - eps * (sum_z / (float)C) : lse - zm;
+                    if (valid_b) atomicAdd(&s_acc[0], loss * inv_b);
+                } else {
+                    const float loss = SMOOTH ? lse - (1.f - eps) * zt - eps * (sum_z / (float)C) : lse - zt;
+                    atomicAdd(&s_acc[0], loss * inv_b);
+                }
                 if (above < 0.5f) atomicAdd(&s_acc[1], 100.f * inv_b);
                 if (above < 4.5f) atomicAdd(&s_acc[2], 100.f * inv_b);
             }
@@ -93,10 +119,11 @@ xent_fwd_kernel(const T* __restrict__ logits, const long long* __restrict__ targ
     if (threadIdx.x < 3) atomicAdd(out3 + threadIdx.x, s_acc[threadIdx.x]);
 }
 
-template <typename T, bool SMOOTH>
+template <typename T, bool SMOOTH, bool MIX>
 __global__ void __launch_bounds__(XE_THREADS)
 xent_bwd_kernel(const T* __restrict__ logits, const long long* __restrict__ target, const float* __restrict__ lse,
-                const float* __restrict__ grad_out, T* __restrict__ dlogits, int B, int C, float eps)
+                const float* __restrict__ grad_out, T* __restrict__ dlogits, int B, int C, float eps,
+                const float* __restrict__ mix)
 {
     const int lane = threadIdx.x & 31;
     const int row = blockIdx.x * (XE_THREADS / 32) + (threadIdx.x >> 5);
@@ -105,10 +132,25 @@ xent_bwd_kernel(const T* __restrict__ logits, const long long* __restrict__ targ
     const T* z = logits + (size_t)row * C;
     T* dz = dlogits + (size_t)row * C;
     const long long t = target[row];
-    const bool valid = t >= 0 && t < C;
+    bool valid = t >= 0 && t < C;
     const float l = lse[row];
     const float eps_c = SMOOTH ? eps / (float)C : 0.f;        // smoothed target mass of every class
     const float hit = SMOOTH ? 1.f - eps + eps_c : 1.f;       // ... and of the target class
+    if (MIX) {
+        const long long tb = target[B - 1 - row];
+        valid = valid && tb >= 0 && tb < C;
+        const float lam = mix[0];
+        const float wa = SMOOTH ? (1.f - eps) * lam : lam;                // target mass of class a
+        const float wb = SMOOTH ? (1.f - eps) * (1.f - lam) : 1.f - lam;  // ... and of class b
+        for (int j = lane; j < C; j += 32) {
+            float q = eps_c;
+            if (j == t) q += wa;
+            if (j == tb) q += wb;
+            const float p = __expf(to_f<T>(z[j]) - l) - q;
+            dz[j] = from_f<T>(valid ? g * p : 0.f);
+        }
+        return;
+    }
     for (int j = lane; j < C; j += 32) {
         float p = __expf(to_f<T>(z[j]) - l);
         if (j == t) p -= hit;
@@ -122,34 +164,40 @@ xent_bwd_kernel(const T* __restrict__ logits, const long long* __restrict__ targ
 extern "C" {
 
 // dtype: 0 = bf16 logits, 1 = fp32 logits; out3 must be zeroed by the caller (same stream);
-// eps = label smoothing in [0, 1] (checked by the caller), 0 = plain cross-entropy
+// eps = label smoothing in [0, 1] (checked by the caller), 0 = plain cross-entropy;
+// mix = device mix state (mix[0] = lam, partner row B-1-i), nullptr = one target per row
 cudaError_t xent_launch_fwd(int dtype, const void* logits, const long long* target, float* lse, float* out3, int B,
-                            int C, float eps, cudaStream_t st)
+                            int C, float eps, const float* mix, cudaStream_t st)
 {
     const int grid = (B + XE_THREADS / 32 - 1) / (XE_THREADS / 32);
     const bool smooth = eps != 0.f;
     if (dtype == 0) {
-        auto k = smooth ? xent_fwd_kernel<__nv_bfloat16, true> : xent_fwd_kernel<__nv_bfloat16, false>;
-        k<<<grid, XE_THREADS, 0, st>>>((const __nv_bfloat16*)logits, target, lse, out3, B, C, eps);
+        auto k = mix ? (smooth ? xent_fwd_kernel<__nv_bfloat16, true, true> : xent_fwd_kernel<__nv_bfloat16, false, true>)
+                     : (smooth ? xent_fwd_kernel<__nv_bfloat16, true, false> : xent_fwd_kernel<__nv_bfloat16, false, false>);
+        k<<<grid, XE_THREADS, 0, st>>>((const __nv_bfloat16*)logits, target, lse, out3, B, C, eps, mix);
     } else {
-        auto k = smooth ? xent_fwd_kernel<float, true> : xent_fwd_kernel<float, false>;
-        k<<<grid, XE_THREADS, 0, st>>>((const float*)logits, target, lse, out3, B, C, eps);
+        auto k = mix ? (smooth ? xent_fwd_kernel<float, true, true> : xent_fwd_kernel<float, false, true>)
+                     : (smooth ? xent_fwd_kernel<float, true, false> : xent_fwd_kernel<float, false, false>);
+        k<<<grid, XE_THREADS, 0, st>>>((const float*)logits, target, lse, out3, B, C, eps, mix);
     }
     return cudaGetLastError();
 }
 
 cudaError_t xent_launch_bwd(int dtype, const void* logits, const long long* target, const float* lse,
-                            const float* grad_out, void* dlogits, int B, int C, float eps, cudaStream_t st)
+                            const float* grad_out, void* dlogits, int B, int C, float eps, const float* mix,
+                            cudaStream_t st)
 {
     const int grid = (B + XE_THREADS / 32 - 1) / (XE_THREADS / 32);
     const bool smooth = eps != 0.f;
     if (dtype == 0) {
-        auto k = smooth ? xent_bwd_kernel<__nv_bfloat16, true> : xent_bwd_kernel<__nv_bfloat16, false>;
+        auto k = mix ? (smooth ? xent_bwd_kernel<__nv_bfloat16, true, true> : xent_bwd_kernel<__nv_bfloat16, false, true>)
+                     : (smooth ? xent_bwd_kernel<__nv_bfloat16, true, false> : xent_bwd_kernel<__nv_bfloat16, false, false>);
         k<<<grid, XE_THREADS, 0, st>>>((const __nv_bfloat16*)logits, target, lse, grad_out, (__nv_bfloat16*)dlogits,
-                                       B, C, eps);
+                                       B, C, eps, mix);
     } else {
-        auto k = smooth ? xent_bwd_kernel<float, true> : xent_bwd_kernel<float, false>;
-        k<<<grid, XE_THREADS, 0, st>>>((const float*)logits, target, lse, grad_out, (float*)dlogits, B, C, eps);
+        auto k = mix ? (smooth ? xent_bwd_kernel<float, true, true> : xent_bwd_kernel<float, false, true>)
+                     : (smooth ? xent_bwd_kernel<float, true, false> : xent_bwd_kernel<float, false, false>);
+        k<<<grid, XE_THREADS, 0, st>>>((const float*)logits, target, lse, grad_out, (float*)dlogits, B, C, eps, mix);
     }
     return cudaGetLastError();
 }

@@ -21,6 +21,12 @@ Label smoothing (``label_smoothing=eps``, in [0, 1]) follows
 on eps.  The reference's KL divergence against the smoothed one-hot target would be lower by the
 constant entropy of that target, with the same gradient.  ``eps = 0`` runs exactly the
 unsmoothed kernels.
+
+Mixup / CutMix (``mix=state``, the device mix state of ``batch_mix.BatchMix``): row ``i`` has two
+targets, its own ``t_i`` and its partner's ``t_{B-1-i}``, weighted ``lam`` and ``1 - lam`` (``lam``
+read by the kernels from ``state[0]``, so a captured graph follows each step's draw):
+``loss_i = lam CE_eps(z_i, t_i) + (1 - lam) CE_eps(z_i, t_{B-1-i})``.  prec@1 / prec@5 still count
+against each row's own target.  ``mix=None`` runs exactly the one-target kernels.
 """
 
 from __future__ import annotations
@@ -57,11 +63,12 @@ def reference_loss_and_accuracy(logits: torch.Tensor, target: torch.Tensor, labe
 class _FusedXent(torch.autograd.Function):
 
     @staticmethod
-    def forward(ctx, logits, target, label_smoothing):
+    def forward(ctx, logits, target, label_smoothing, mix):
         C = native.load()
-        metrics, lse = C.xent_forward(logits, target, label_smoothing)
+        metrics, lse = C.xent_forward(logits, target, label_smoothing, mix)
         ctx.save_for_backward(logits, target, lse)
         ctx.label_smoothing = label_smoothing
+        ctx.mix = mix
         ctx.mark_non_differentiable(metrics)
         return metrics[0], metrics
 
@@ -70,19 +77,25 @@ class _FusedXent(torch.autograd.Function):
         C = native.load()
         logits, target, lse = ctx.saved_tensors
         g = g_loss.reshape(1).to(torch.float32)
-        return C.xent_backward(logits, target, lse, g, ctx.label_smoothing), None, None
+        return C.xent_backward(logits, target, lse, g, ctx.label_smoothing, ctx.mix), None, None, None
 
 
-def fused_cross_entropy(logits: torch.Tensor, target: torch.Tensor, label_smoothing: float = 0.0):
+def fused_cross_entropy(logits: torch.Tensor, target: torch.Tensor, label_smoothing: float = 0.0,
+                        mix: torch.Tensor = None):
     """Returns ``(loss, metrics)``; ``metrics = [loss, prec@1 %, prec@5 %]`` (fp32, detached).
-    ``label_smoothing`` in [0, 1], as in ``F.cross_entropy``."""
+    ``label_smoothing`` in [0, 1], as in ``F.cross_entropy``.  ``mix``: the mix state of
+    ``batch_mix.BatchMix`` (two targets per row, see the module docstring), or None."""
     eps = check_label_smoothing(label_smoothing)
     if logits.is_cuda and native.available():
         lg = logits if logits.is_contiguous() else logits.contiguous()
         if native.load().xent_can_fuse(lg, target):
-            loss, metrics = _FusedXent.apply(lg, target, eps)
+            loss, metrics = _FusedXent.apply(lg, target, eps, mix)
             return loss, metrics
-    loss, p1, p5 = reference_loss_and_accuracy(logits, target, eps)
+    if mix is None:
+        loss, p1, p5 = reference_loss_and_accuracy(logits, target, eps)
+    else:
+        from .batch_mix import reference_mixed_loss_and_accuracy
+        loss, p1, p5 = reference_mixed_loss_and_accuracy(logits, target, mix[0], eps)
     return loss, torch.stack([loss.detach().float(), p1, p5])
 
 
@@ -95,8 +108,10 @@ class FusedCrossEntropyWithAccuracy(nn.Module):
         self.label_smoothing = check_label_smoothing(label_smoothing)
         self.metrics = None
 
-    def forward(self, logits, target):
-        loss, self.metrics = fused_cross_entropy(logits, target, self.label_smoothing)
+    def forward(self, logits, target, mix=None):
+        """``mix``: the device mix state of ``batch_mix.BatchMix`` for mixup / CutMix targets
+        (prec@1 / prec@5 then count against each row's own target), or None."""
+        loss, self.metrics = fused_cross_entropy(logits, target, self.label_smoothing, mix=mix)
         return loss
 
     def extra_repr(self):

@@ -584,12 +584,13 @@ class _BilatEngineShim(object):
 
 
 def make_bilat_trainer(model: BilatGossipDataParallel, lr, criterion=None, amp_dtype=None,
-                       use_cuda_graph=True, warmup_iters=3, channels_last=True, lars=False):
+                       use_cuda_graph=True, warmup_iters=3, channels_last=True, lars=False, batch_mix=None):
     """AD-PSGD counterpart of :class:`~.trainer.GossipTrainer`: forward + fused loss/accuracy +
     backward are captured ONCE as a CUDA graph; after every replay the gradients are handed to
     the gossip side with :meth:`BilatGossipDataParallel.handoff` (fused SGD on the gossip copy +
     model pull, enqueued on the daemon's stream under its lock).  The bilateral averaging itself
-    runs asynchronously on the native daemon's low-priority stream the whole time."""
+    runs asynchronously on the native daemon's low-priority stream the whole time.  ``batch_mix``:
+    mixup / CutMix as in ``GossipTrainer``."""
     if lars:
         raise ValueError('LARS is not supported with AD-PSGD: its SGD runs on the gossip daemon\'s '
                          'copy, outside FusedGossipSGD')
@@ -612,7 +613,7 @@ def make_bilat_trainer(model: BilatGossipDataParallel, lr, criterion=None, amp_d
             self.overlap = False
             self.gossip = False
             self._init_runtime(self.engine.device, criterion, amp_dtype, use_cuda_graph, warmup_iters,
-                               channels_last)
+                               channels_last, batch_mix)
 
         def _one_step(self, first=False):
             self._fwd_bwd()                      # the captured part

@@ -18,6 +18,10 @@ backward hooks + the gossip thread) with zero Python on the critical path:
 Modes: ``'sgp'`` (push-sum, directed graph), ``'dpsgd'`` (push-pull, symmetric
 graph) -- same kernel, the graph/mixing differ --, ``'osgp'`` (overlap), and
 ``'local'`` (world size 1 / gossip disabled).
+
+Mixup / CutMix (``batch_mix=ops.batch_mix.BatchMix(...)``): the stage -> static input copy becomes
+one launch of the batch-mix kernel (same bytes read and written), after an H2D copy of the step's
+draw into the device mix state; the captured fused cross-entropy reads ``lam`` from that state.
 """
 
 from __future__ import annotations
@@ -38,7 +42,9 @@ class GossipTrainer(object):
     def __init__(self, model: GossipDataParallel, optimizer: FusedGossipSGD,
                  criterion: Optional[Callable] = None, amp_dtype=torch.bfloat16,
                  use_cuda_graph: bool = True, warmup_iters: int = 3,
-                 channels_last: bool = True):
+                 channels_last: bool = True, batch_mix=None):
+        """``batch_mix``: an ``ops.batch_mix.BatchMix`` to train with mixup / CutMix (needs the
+        fused criterion; the draw of each step comes from ``batch_mix.iteration``), or None."""
         assert model._kernel is not None, 'GossipTrainer drives the nvlink kernel transport'
         self.model = model
         self.opt = optimizer
@@ -47,15 +53,22 @@ class GossipTrainer(object):
         self.overlap = model.overlap
         self.gossip = model.dist_config['world_size'] > 1
         self._init_runtime(self.engine.device, criterion, amp_dtype, use_cuda_graph, warmup_iters,
-                           channels_last)
+                           channels_last, batch_mix)
         self._slowmo_on = model.slowmo_frequency > 0      # step() runs the SlowMo step itself
 
-    def _init_runtime(self, device, criterion, amp_dtype, use_cuda_graph, warmup_iters, channels_last):
+    def _init_runtime(self, device, criterion, amp_dtype, use_cuda_graph, warmup_iters, channels_last,
+                      batch_mix=None):
         """state shared by every trainer flavour (gossip / all-reduce / bilateral)"""
         # default: fused softmax cross-entropy that also yields prec@1 / prec@5 (the reference loop
         # measures both every iteration, gossip_sgd.py:394-399) in the same launch
         self.criterion = criterion or FusedCrossEntropyWithAccuracy()
         self._fused_loss = isinstance(self.criterion, FusedCrossEntropyWithAccuracy)
+        if batch_mix is not None and not batch_mix.enabled:
+            batch_mix = None                     # both alphas 0: the plain copy and loss
+        if batch_mix is not None and not self._fused_loss:
+            raise ValueError('batch_mix needs the fused criterion (FusedCrossEntropyWithAccuracy): it '
+                             'carries the mixed targets into the loss')
+        self.batch_mix = batch_mix
         self.amp_dtype = amp_dtype
         self.use_graph = use_cuda_graph
         self.warmup_iters = warmup_iters
@@ -105,11 +118,11 @@ class GossipTrainer(object):
             net = twin[0]
             net.train(self.model.module.training)
             out = net(self.static_in)
-            loss = self.criterion(out if self._fused_loss else out.float(), self.static_tgt)
+            loss = self._loss(out)
         else:
             with self._autocast():
                 out = self.model.module(self.static_in)
-                loss = self.criterion(out if self._fused_loss else out.float(), self.static_tgt)
+                loss = self._loss(out)
         self._backward(loss, net if twin else self.model.module)
         metrics = getattr(self.criterion, 'metrics', None)
         if metrics is not None:
@@ -117,6 +130,11 @@ class GossipTrainer(object):
         else:
             self.static_metrics[0].copy_(loss.detach())
         self.static_out = out.detach()
+
+    def _loss(self, out):
+        if self.batch_mix is not None:            # two targets per row, lam from the device mix state
+            return self.criterion(out, self.static_tgt, mix=self.batch_mix.state)
+        return self.criterion(out if self._fused_loss else out.float(), self.static_tgt)
 
     def _backward(self, loss, net):
         """``loss.backward()`` without ~160 per-parameter accumulate kernels: the flat gradient
@@ -239,7 +257,11 @@ class GossipTrainer(object):
             self.prefetch(batch, target)
         main.wait_event(self._stage_ready)
         with torch.cuda.stream(main):
-            self.static_in.copy_(self._stage, non_blocking=True)
+            if self.batch_mix is not None:
+                # the same read and write of the batch, mixed with its flipped batch on the way
+                self.batch_mix.apply(self._stage, self.static_in)
+            else:
+                self.static_in.copy_(self._stage, non_blocking=True)
             self.static_tgt.copy_(self._stage_tgt, non_blocking=True)
             self._stage_free.record(main)
         self._prefetched = False

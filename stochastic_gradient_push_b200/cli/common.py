@@ -100,6 +100,13 @@ def build_parser(adpsgd: bool = False) -> argparse.ArgumentParser:
                    help='probability that a training step is mixed (mixup or CutMix)')
     p.add_argument('--mix_switch_prob', default=0.5, type=float,
                    help='with both alphas > 0: probability that a mixed step uses CutMix rather than mixup')
+    p.add_argument('--model_ema_decay', default=0.0, type=float,
+                   help='keep an exponential moving average of the weights and BatchNorm statistics '
+                        '(ops.model_ema.ModelEma) with this decay in [0, 1), updated after every step (inside '
+                        'the captured step with --cuda_graph True), validated at each epoch end and logged to '
+                        '<checkpoint_dir><tag>ema_r<rank>_n<world>.csv; 0 = off.  Not with AD-PSGD')
+    p.add_argument('--model_ema_warmup', default=False, **B,
+                   help='EMA decay warm-up: min(decay, (1 + t) / (10 + t)) after t updates')
     p.add_argument('--seed', default=47, type=int)
     p.add_argument('--resume', default=False, **B)
     p.add_argument('--backend', default='nccl', choices=['nccl', 'gloo', 'mpi'])
@@ -276,6 +283,8 @@ def finalize_args(args, adpsgd=False):
     if not 0.0 <= getattr(args, 'label_smoothing', 0.0) <= 1.0:
         raise ValueError('--label_smoothing must be in [0, 1], got %r' % (args.label_smoothing,))
     check_mix_flags(args)
+    check_ema_flags(args, adpsgd)
+    args.ema_fname = '{}{}ema_r{}_n{}.csv'.format(args.checkpoint_dir, args.tag, args.rank, args.world_size)
     args.consensus_fname = '{}{}consensus_r{}_n{}.csv'.format(args.checkpoint_dir, args.tag, args.rank,
                                                               args.world_size)
 
@@ -329,6 +338,24 @@ def check_mix_flags(args):
         v = getattr(args, flag, 0.0)
         if not 0.0 <= v <= 1.0:
             raise ValueError('--%s must be in [0, 1], got %r' % (flag, v))
+
+
+def check_ema_flags(args, adpsgd=False):
+    """ValueError for --model_ema_decay out of [0, 1) or with AD-PSGD."""
+    d = getattr(args, 'model_ema_decay', 0.0)
+    if not 0.0 <= d < 1.0:
+        raise ValueError('--model_ema_decay must be in [0, 1), got %r' % (d,))
+    if d > 0 and adpsgd:
+        raise ValueError('--model_ema_decay is not supported with AD-PSGD: its gossip daemon rewrites the '
+                         'parameters concurrently on another stream')
+
+
+def make_model_ema(args, model):
+    """The ``ops.model_ema.ModelEma`` of ``model`` for --model_ema_decay (None when it is 0)."""
+    if not getattr(args, 'model_ema_decay', 0.0) > 0:
+        return None
+    from ..ops.model_ema import ModelEma
+    return ModelEma(model, decay=args.model_ema_decay, warmup=args.model_ema_warmup)
 
 
 def check_schedule_args(args):
@@ -563,6 +590,22 @@ class ConsensusLog(object):
             print('{},{},{!r},{!r},{!r},{}'.format(epoch, itr, stats.distance_sq, stats.average_norm_sq,
                                                     stats.relative, '' if avg_prec1 is None else avg_prec1),
                   file=f)
+
+
+class EmaLog(object):
+    """``--model_ema_decay``: one row per validation of the EMA model."""
+
+    COLUMNS = 'epoch,num_updates,prec1,prec5'
+
+    def __init__(self, fname):
+        self.fname = fname
+        if not os.path.exists(fname):
+            with open(fname, 'w') as f:
+                print(self.COLUMNS, file=f)
+
+    def row(self, epoch, num_updates, prec1, prec5):
+        with open(self.fname, 'a') as f:
+            print('{},{},{!r},{!r}'.format(epoch, num_updates, prec1, prec5), file=f)
 
 
 def update_state(state, update_dict):

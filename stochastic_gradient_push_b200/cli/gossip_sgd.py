@@ -132,6 +132,9 @@ def main(argv=None):
     optimizer.zero_grad()
     # --mixup_alpha / --cutmix_alpha: training batches only (validate() never mixes)
     args._batch_mix = common.make_batch_mix(args)
+    # --model_ema_decay: weight EMA, updated after every step (the last launch of the captured step)
+    args._ema = common.make_model_ema(args, model)
+    args._ema_due = False
     args._trainer = None
     if args.cuda_graph and not args.all_reduce and args.fused and getattr(model, '_kernel', None):
         from ..ops.fused_loss import FusedCrossEntropyWithAccuracy
@@ -141,9 +144,11 @@ def main(argv=None):
         args._trainer = GossipTrainer(model, optimizer,
                                       FusedCrossEntropyWithAccuracy(label_smoothing=args.label_smoothing),
                                       amp_dtype=torch.bfloat16 if args.amp else None,
-                                      batch_mix=args._batch_mix)
+                                      batch_mix=args._batch_mix, ema=args._ema)
 
     state = fresh_state(model.state_dict(), optimizer.state_dict())
+    if args._ema is not None:
+        state['model_ema'] = args._ema.state_dict()
     cmanager = ClusterManager(rank=args.rank, world_size=args.world_size, model_tag=args.tag,
                               state=state, all_workers=args.checkpoint_all)
     if args.resume and os.path.isfile(cmanager.checkpoint_fpath):
@@ -155,6 +160,13 @@ def main(argv=None):
         state['is_best'] = False
         model.load_state_dict(ckpt['state_dict'])
         optimizer.load_state_dict(ckpt['optimizer'])
+        if args._ema is not None:
+            if 'model_ema' in ckpt:
+                args._ema.load_state_dict(ckpt['model_ema'])
+                state['model_ema'] = ckpt['model_ema']
+            else:
+                log.warning('checkpoint has no model_ema: the EMA starts again from the loaded model')
+                args._ema.reset()
         log.info("=> loaded checkpoint (epoch {}; itr {})".format(ckpt['epoch'], ckpt['itr']))
     elif args.resume:
         log.info("=> no checkpoint found at '{}'".format(cmanager.checkpoint_fpath))
@@ -165,6 +177,7 @@ def main(argv=None):
     csv = CSVLog(args.out_fname, args.world_size, args.num_dataloader_workers, args.batch_size)
     args._consensus_log = (ConsensusLog(args.consensus_fname)
                            if args.consensus_freq > 0 or args.validate_average else None)
+    args._ema_log = common.EmaLog(args.ema_fname) if args._ema is not None else None
 
     loader, sampler = make_dataloader(args, train=True)
     val_loader = None if args.train_fast else make_dataloader(args, train=False)
@@ -188,8 +201,12 @@ def main(argv=None):
                 'state_dict': model.state_dict(), 'optimizer': optimizer.state_dict(),
                 'elapsed_time': elapsed_time, 'batch_meter': batch_meter.__dict__,
                 'data_meter': data_meter.__dict__, 'nn_meter': nn_meter.__dict__})
+            if args._ema is not None:
+                state['model_ema'] = args._ema.state_dict()
             prec1 = validate(args, val_loader, model, criterion, log)
             csv.val_row(epoch, batch_meter, nn_meter, data_meter, prec1)
+            if args._ema is not None:
+                validate_ema(args, val_loader, model, criterion, log, epoch)
             if prec1 > best_val_prec1:
                 update_state(state, {'is_best': True, 'best_prec1': prec1})
                 best_val_prec1 = prec1
@@ -203,6 +220,8 @@ def main(argv=None):
         val_loader = make_dataloader(args, train=False)
         prec1 = validate(args, val_loader, model, criterion, log)
         log.info('Test accuracy: {}'.format(prec1))
+        if args._ema is not None:
+            validate_ema(args, val_loader, model, criterion, log, args.num_epochs - 1)
     log.info('elapsed_time {0}'.format(time.time() - begin_time))
     if tracing.get_tracer().enabled:            # shorter run than --trace_iters
         log.info('trace written to %s' % tracing.disable().dump())
@@ -239,6 +258,7 @@ def train(args, model, criterion, optimizer, batch_meter, data_meter, nn_meter, 
     pending = []
     trainer = getattr(args, '_trainer', None)
     batch_mix = getattr(args, '_batch_mix', None)
+    ema = getattr(args, '_ema', None) if trainer is None else None    # (the trainer updates its own)
     it = iter(loader)
     for _ in range(itr):            # resume mid-epoch: skip what was already consumed
         next(it, None)
@@ -279,6 +299,11 @@ def train(args, model, criterion, optimizer, batch_meter, data_meter, nn_meter, 
             with tracing.span('forward', itr=i), _autocast(args):
                 output = model(batch)
                 loss = common.train_loss(criterion, output, target, mix, args.label_smoothing)
+            if ema is not None and args._ema_due:
+                # c10d plane: the previous step's gossip was received and de-biased by the forward
+                # pre-hook just now; the EMA takes those parameters (and this forward's BN statistics)
+                ema.update()
+                args._ema_due = False
             with tracing.span('backward'):
                 loss.backward()
             with tracing.span('optimizer'):
@@ -288,6 +313,11 @@ def train(args, model, criterion, optimizer, batch_meter, data_meter, nn_meter, 
                 model.transfer_params()
             if getattr(args, 'slowmo_frequency', 0):
                 model.perform_slowmo(optimizer)        # (the trainer path runs it inside step())
+            if ema is not None:
+                if getattr(model, 'is_ps_numerator', False):
+                    args._ema_due = True               # gossip in flight: after the next forward pre-hook
+                else:
+                    ema.update()
             with torch.no_grad():
                 p1, p5 = accuracy(output, target, topk=(1, 5))
                 pending.append((torch.stack([loss.detach().float().reshape(()), p1[0], p5[0]]),
@@ -366,7 +396,22 @@ def epoch_end_consensus(args, model, criterion, val_loader, epoch, log):
     log_consensus(args, stats, epoch, -1, log, avg_prec1=prec1)
 
 
+def validate_ema(args, val_loader, model, criterion, log, epoch):
+    """Validate the EMA weights and BatchNorm statistics (``ModelEma.applied``, restored afterwards)
+    and log their prec@1 / prec@5 to stdout and the EMA CSV."""
+    ema = args._ema
+    with ema.applied():
+        prec1, prec5 = evaluate(args, val_loader, model, criterion, log, label='EMA ')
+    args._ema_log.row(epoch, ema.num_updates, prec1, prec5)
+    return prec1
+
+
 def validate(args, val_loader, model, criterion, log):
+    return evaluate(args, val_loader, model, criterion, log)[0]
+
+
+def evaluate(args, val_loader, model, criterion, log, label=''):
+    """(prec@1, prec@5) over the validation set, logged as `` * <label>Prec@1 .. Prec@5 ..``"""
     losses, top1, top5 = Meter(ptag='Loss'), Meter(ptag='Prec@1'), Meter(ptag='Prec@5')
     model.eval()
     dev = args.device
@@ -384,8 +429,8 @@ def validate(args, val_loader, model, criterion, log):
             losses.update(loss.item(), n)
             top1.update(p1.item(), n)
             top5.update(p5.item(), n)
-    log.info(' * Prec@1 {top1.avg:.3f} Prec@5 {top5.avg:.3f}'.format(top1=top1, top5=top5))
-    return top1.avg
+    log.info(' * {label}Prec@1 {top1.avg:.3f} Prec@5 {top5.avg:.3f}'.format(label=label, top1=top1, top5=top5))
+    return top1.avg, top5.avg
 
 
 if __name__ == '__main__':

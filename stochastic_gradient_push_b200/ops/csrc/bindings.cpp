@@ -858,6 +858,35 @@ static void zero_(torch::Tensor x)
     SGP_CUDA_CHECK(sgp_launch_zero(x.data_ptr(), bytes, at::cuda::getCurrentCUDAStream()));
 }
 
+// ---------------------------------------------------------------------------
+// model weight EMA (csrc/ema_kernels.cu, ops/model_ema.py)
+// ---------------------------------------------------------------------------
+extern "C" {
+int sgp_ema_chunk();
+cudaError_t sgp_launch_ema_update(const void* segs, const void* items, int nitems, float* ema, void* state,
+                                  int num_sms, cudaStream_t stream);
+}
+
+// ema: flat fp32 EMA buffer; segs: int64 [nseg, 4] (src address, numel, offset, bf16); items: int32
+// [nitems, 2] (segment, chunk); state: fp32 [4] decay row.  One launch on the current stream.
+static void ema_update(torch::Tensor ema, torch::Tensor segs, torch::Tensor items, torch::Tensor state)
+{
+    TORCH_CHECK(ema.is_cuda() && ema.scalar_type() == torch::kFloat32 && ema.is_contiguous(), "ema: fp32 CUDA");
+    TORCH_CHECK(segs.is_cuda() && segs.scalar_type() == torch::kInt64 && segs.is_contiguous() && segs.dim() == 2 &&
+                segs.size(1) == 4, "segs: int64 [nseg, 4] on the device");
+    TORCH_CHECK(items.is_cuda() && items.scalar_type() == torch::kInt32 && items.is_contiguous() &&
+                items.dim() == 2 && items.size(1) == 2, "items: int32 [nitems, 2] on the device");
+    TORCH_CHECK(state.is_cuda() && state.scalar_type() == torch::kFloat32 && state.is_contiguous() &&
+                state.numel() == 4, "state: fp32 [4] on the device");
+    TORCH_CHECK(segs.get_device() == ema.get_device() && items.get_device() == ema.get_device() &&
+                state.get_device() == ema.get_device(), "EMA tensors on different devices");
+    c10::cuda::CUDAGuard guard(ema.get_device());
+    const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
+    SGP_CUDA_CHECK(sgp_launch_ema_update(segs.data_ptr(), items.data_ptr(), (int)items.size(0),
+                                         ema.data_ptr<float>(), state.data_ptr(), sms,
+                                         at::cuda::getCurrentCUDAStream()));
+}
+
 void bind_bn(py::module& mod);   // bn_bindings.cpp
 void bind_vmm(py::module& mod);  // vmm_symm.cpp
 void bind_data(py::module& mod); // data_loader.cpp
@@ -884,6 +913,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, mod)
     mod.def("launch_count", []() { return (long long)g_sgp_kernel_launches.load(); },
             "kernels of this extension launched (or captured) so far by this process");
     mod.def("max_resident_ctas", &sgp_max_resident_ctas);
+    mod.def("ema_update", &ema_update, py::arg("ema"), py::arg("segs"), py::arg("items"), py::arg("state"),
+            "e <- fmaf(1 - d_t, s - e, e) over every segment in one launch; advances the device counter");
+    mod.attr("EMA_CHUNK") = sgp_ema_chunk();
 
     mod.attr("CHUNK") = (int)SGP_CHUNK;
     mod.attr("MAX_PEERS") = (int)SGP_MAX_PEERS;

@@ -584,13 +584,18 @@ class _BilatEngineShim(object):
 
 
 def make_bilat_trainer(model: BilatGossipDataParallel, lr, criterion=None, amp_dtype=None,
-                       use_cuda_graph=True, warmup_iters=3, channels_last=True, lars=False, batch_mix=None):
+                       use_cuda_graph=True, warmup_iters=3, channels_last=True, lars=False, batch_mix=None,
+                       ema=None):
     """AD-PSGD counterpart of :class:`~.trainer.GossipTrainer`: forward + fused loss/accuracy +
     backward are captured ONCE as a CUDA graph; after every replay the gradients are handed to
     the gossip side with :meth:`BilatGossipDataParallel.handoff` (fused SGD on the gossip copy +
     model pull, enqueued on the daemon's stream under its lock).  The bilateral averaging itself
     runs asynchronously on the native daemon's low-priority stream the whole time.  ``batch_mix``:
-    mixup / CutMix as in ``GossipTrainer``."""
+    mixup / CutMix as in ``GossipTrainer``.  ``ema`` must be None: a weight EMA is not supported,
+    the gossip daemon rewrites the parameters concurrently on its own stream."""
+    if ema is not None:
+        raise ValueError('ModelEma is not supported with AD-PSGD: its gossip daemon rewrites the parameters '
+                         'concurrently on another stream, so no launch sees a settled model')
     if lars:
         raise ValueError('LARS is not supported with AD-PSGD: its SGD runs on the gossip daemon\'s '
                          'copy, outside FusedGossipSGD')

@@ -188,7 +188,7 @@ class ARTrainer(GossipTrainer):
 
     def __init__(self, model: AllReduceDataParallel, lr, momentum=0.9, weight_decay=1e-4,
                  nesterov=True, criterion=None, amp_dtype=torch.bfloat16, use_cuda_graph=True,
-                 warmup_iters=3, channels_last=True, lars=False, batch_mix=None):
+                 warmup_iters=3, channels_last=True, lars=False, batch_mix=None, ema=None):
         if lars:
             raise ValueError('LARS is not supported by the all-reduce optimizer: its sharded fused step '
                              'holds 1/n of each tensor, so no rank sees a whole tensor\'s norm')
@@ -205,7 +205,7 @@ class ARTrainer(GossipTrainer):
         self.overlap = False
         self.gossip = False
         self._init_runtime(model.device, criterion, amp_dtype, use_cuda_graph, warmup_iters, channels_last,
-                           batch_mix)
+                           batch_mix, ema)
 
     def _one_step(self, first=False):
         self._fwd_bwd()

@@ -22,6 +22,14 @@ graph) -- same kernel, the graph/mixing differ --, ``'osgp'`` (overlap), and
 Mixup / CutMix (``batch_mix=ops.batch_mix.BatchMix(...)``): the stage -> static input copy becomes
 one launch of the batch-mix kernel (same bytes read and written), after an H2D copy of the step's
 draw into the device mix state; the captured fused cross-entropy reads ``lam`` from that state.
+
+Weight EMA (``ema=ops.model_ema.ModelEma(model, ...)``): ``ema.update()`` is the LAST launch of every
+step, eager warm-up steps and captured graph alike, on the trainer's stream after the forward pass
+(which updated the BatchNorm running statistics) and after the gossip / SGD launch -- under
+Overlap-SGP after ``publish`` and the join with the gossip stream.  The EMA therefore follows the
+parameters exactly as the next forward pass sees them: under Overlap-SGP the residual gathered during
+step k is folded in at the next publish, so it reaches the EMA one step later, and a SlowMo step
+(enqueued after the replay) reaches it at the next step.
 """
 
 from __future__ import annotations
@@ -42,9 +50,10 @@ class GossipTrainer(object):
     def __init__(self, model: GossipDataParallel, optimizer: FusedGossipSGD,
                  criterion: Optional[Callable] = None, amp_dtype=torch.bfloat16,
                  use_cuda_graph: bool = True, warmup_iters: int = 3,
-                 channels_last: bool = True, batch_mix=None):
+                 channels_last: bool = True, batch_mix=None, ema=None):
         """``batch_mix``: an ``ops.batch_mix.BatchMix`` to train with mixup / CutMix (needs the
-        fused criterion; the draw of each step comes from ``batch_mix.iteration``), or None."""
+        fused criterion; the draw of each step comes from ``batch_mix.iteration``), or None.
+        ``ema``: an ``ops.model_ema.ModelEma`` of ``model`` updated at the end of every step, or None."""
         assert model._kernel is not None, 'GossipTrainer drives the nvlink kernel transport'
         self.model = model
         self.opt = optimizer
@@ -53,11 +62,11 @@ class GossipTrainer(object):
         self.overlap = model.overlap
         self.gossip = model.dist_config['world_size'] > 1
         self._init_runtime(self.engine.device, criterion, amp_dtype, use_cuda_graph, warmup_iters,
-                           channels_last, batch_mix)
+                           channels_last, batch_mix, ema)
         self._slowmo_on = model.slowmo_frequency > 0      # step() runs the SlowMo step itself
 
     def _init_runtime(self, device, criterion, amp_dtype, use_cuda_graph, warmup_iters, channels_last,
-                      batch_mix=None):
+                      batch_mix=None, ema=None):
         """state shared by every trainer flavour (gossip / all-reduce / bilateral)"""
         # default: fused softmax cross-entropy that also yields prec@1 / prec@5 (the reference loop
         # measures both every iteration, gossip_sgd.py:394-399) in the same launch
@@ -88,6 +97,9 @@ class GossipTrainer(object):
         # AccumulateGrad nodes are then created on the stream the graph is captured on
         self.stream = torch.cuda.Stream(device=self.device)
         self.stream.wait_stream(torch.cuda.current_stream(self.device))
+        self.ema = ema
+        if ema is not None:
+            ema._stream = self.stream          # set_decay() / the counter read order with the step
         self._copy_stream = torch.cuda.Stream(device=self.device)
         self._stage = None
         self._stage_tgt = None
@@ -191,6 +203,12 @@ class GossipTrainer(object):
             join.record(side)
         self._fwd_bwd()
         main.wait_event(join)
+
+    def _full_step(self, first=False):
+        """the step of every trainer flavour (its ``_one_step``), then the EMA update as its last launch"""
+        self._one_step(first)
+        if self.ema is not None:
+            self.ema.update()
 
     def _one_step(self, first=False):
         if self.overlap and self.gossip and self.model.gossip_enable:
@@ -331,7 +349,7 @@ class GossipTrainer(object):
             self._after_replay()
         else:
             c0 = self.engine.C.launch_count()
-            self._one_step(first=(self._eager_steps == 0))
+            self._full_step(first=(self._eager_steps == 0))
             self.own_launches_per_step = self.engine.C.launch_count() - c0
             self._eager_steps += 1
 
@@ -358,7 +376,7 @@ class GossipTrainer(object):
         c0 = self.engine.C.launch_count()
         with torch.cuda.graph(self.graph, stream=self.stream, capture_error_mode='thread_local',
                               pool=self._pool):
-            self._one_step(first=False)
+            self._full_step(first=False)
         self.own_launches_per_step = self.engine.C.launch_count() - c0
         if key is not None:
             self._graphs[key] = self.graph

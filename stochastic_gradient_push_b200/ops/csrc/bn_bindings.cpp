@@ -445,10 +445,14 @@ static py::dict conv1x1_plan(long long M, int N, int K, int num_sms, bool residu
 
 static int sm_count() { return at::cuda::getCurrentDeviceProperties()->multiProcessorCount; }
 
+// num_sms: the SM count the persistent grid is planned for; <= 0 is the device's own.  A smaller value
+// gives every CTA more row tiles (tests of the cross-tile state reach it at small M).
+static int plan_sms(int num_sms) { return num_sms > 0 ? num_sms : sm_count(); }
+
 // y = x . w^T [+ residual] (residual: same shape / layout as y, added in fp32 in the epilogue).
 // with_stats: also run the statistics epilogue into a scratch buffer (benchmarking the GEMM alone)
 static torch::Tensor conv1x1_forward(torch::Tensor x, torch::Tensor w, bool with_stats,
-                                     c10::optional<torch::Tensor> residual)
+                                     c10::optional<torch::Tensor> residual, int num_sms)
 {
     TORCH_CHECK(conv1x1_can_fuse(x, w), "conv1x1_forward: unsupported tensors");
     const int K = (int)x.size(1), N = (int)w.size(0);
@@ -463,13 +467,14 @@ static torch::Tensor conv1x1_forward(torch::Tensor x, torch::Tensor w, bool with
                     residual->sizes() == y.sizes() && residual->strides() == y.strides() &&
                     (reinterpret_cast<uintptr_t>(residual->data_ptr()) & 15) == 0,
                     "conv1x1_forward: residual must match the output's shape and layout");
+    const int sms = plan_sms(num_sms);
     torch::Tensor partial;
     if (with_stats)
-        partial = torch::empty({c1_partial_rows(M, N, K, sm_count(), 0, f32), 3, N},
+        partial = torch::empty({c1_partial_rows(M, N, K, sms, 0, f32), 3, N},
                                torch::TensorOptions().dtype(torch::kFloat32).device(x.device()));
     BN_CHECK(c1_launch_gemm(x.data_ptr(), w.data_ptr(), y.data_ptr(), M, N, K,
                             with_stats ? partial.data_ptr<float>() : nullptr,
-                            has_res ? residual->data_ptr() : nullptr, nullptr, nullptr, nullptr, sm_count(), f32,
+                            has_res ? residual->data_ptr() : nullptr, nullptr, nullptr, nullptr, sms, f32,
                             at::cuda::getCurrentCUDAStream()));
     return y;
 }
@@ -478,7 +483,8 @@ static torch::Tensor conv1x1_forward(torch::Tensor x, torch::Tensor w, bool with
 // + ReLU) whose input was bn_x, output mask `mask` ([M, N/8] uint8) and coefficients `coef` ([4, N]:
 // mean, invstd, scale, shift).  Returns (dz, partial[R][2][N]) for bn_backward_from_partials.
 static std::vector<torch::Tensor> conv1x1_dgrad_bn_reduce(torch::Tensor x, torch::Tensor w, torch::Tensor residual,
-                                                          torch::Tensor bn_x, torch::Tensor coef, torch::Tensor mask)
+                                                          torch::Tensor bn_x, torch::Tensor coef, torch::Tensor mask,
+                                                          int num_sms)
 {
     TORCH_CHECK(conv1x1_can_fuse(x, w), "conv1x1_dgrad_bn_reduce: unsupported tensors");
     const int K = (int)x.size(1), N = (int)w.size(0);
@@ -495,11 +501,12 @@ static std::vector<torch::Tensor> conv1x1_dgrad_bn_reduce(torch::Tensor x, torch
                 mask.numel() == M * (N / 8) && (reinterpret_cast<uintptr_t>(mask.data_ptr()) & 15) == 0,
                 "conv1x1_dgrad_bn_reduce: mask must be [M, N/8] uint8");
     const int f32 = x.scalar_type() == torch::kFloat32 ? 1 : 0;
-    auto partial = torch::empty({c1_partial_rows(M, N, K, sm_count(), 1, f32), 2, N},
+    const int sms = plan_sms(num_sms);
+    auto partial = torch::empty({c1_partial_rows(M, N, K, sms, 1, f32), 2, N},
                                 torch::TensorOptions().dtype(torch::kFloat32).device(x.device()));
     BN_CHECK(c1_launch_gemm(x.data_ptr(), w.data_ptr(), y.data_ptr(), M, N, K, partial.data_ptr<float>(),
                             residual.data_ptr(), bn_x.data_ptr(), coef.data_ptr<float>(), mask.data_ptr<uint8_t>(),
-                            sm_count(), f32, at::cuda::getCurrentCUDAStream()));
+                            sms, f32, at::cuda::getCurrentCUDAStream()));
     return {y, partial};
 }
 
@@ -512,7 +519,7 @@ static std::vector<torch::Tensor> conv1x1_bn_forward(torch::Tensor x, torch::Ten
                                                      c10::optional<torch::Tensor> running_var,
                                                      c10::optional<torch::Tensor> num_batches_tracked,
                                                      double momentum, double eps, bool relu,
-                                                     c10::optional<torch::Tensor> mask)
+                                                     c10::optional<torch::Tensor> mask, int num_sms)
 {
     TORCH_CHECK(conv1x1_can_fuse(x, w), "conv1x1_bn_forward: unsupported tensors");
     const int K = (int)x.size(1), N = (int)w.size(0);
@@ -526,7 +533,7 @@ static std::vector<torch::Tensor> conv1x1_bn_forward(torch::Tensor x, torch::Ten
     const bool has_res = residual.has_value() && residual->defined();
     if (has_res) TORCH_CHECK(residual->sizes() == yraw.sizes() && residual->scalar_type() == yraw.scalar_type()
                              && residual->strides() == yraw.strides());
-    const int sms = sm_count();
+    const int sms = plan_sms(num_sms);
     const int f32 = x.scalar_type() == torch::kFloat32 ? 1 : 0;
     const bool has_mask = mask.has_value() && mask->defined();
     if (has_mask)
@@ -679,12 +686,13 @@ void bind_bn(py::module& mod)
     mod.def("conv1x1_plan", &conv1x1_plan, py::arg("M"), py::arg("N"), py::arg("K"), py::arg("num_sms") = 132,
             py::arg("residual") = false, py::arg("f32") = false, py::arg("bn_reduce") = false);
     mod.def("conv1x1_forward", &conv1x1_forward, py::arg("x"), py::arg("w"), py::arg("with_stats") = false,
-            py::arg("residual") = py::none());
+            py::arg("residual") = py::none(), py::kw_only(), py::arg("num_sms") = 0);
     mod.def("conv1x1_bn_forward", &conv1x1_bn_forward, py::arg("x"), py::arg("w"), py::arg("residual"),
             py::arg("gamma"), py::arg("beta"), py::arg("running_mean"), py::arg("running_var"),
             py::arg("num_batches_tracked"), py::arg("momentum"), py::arg("eps"), py::arg("relu"),
-            py::arg("mask") = py::none());
-    mod.def("conv1x1_dgrad_bn_reduce", &conv1x1_dgrad_bn_reduce);
+            py::arg("mask") = py::none(), py::kw_only(), py::arg("num_sms") = 0);
+    mod.def("conv1x1_dgrad_bn_reduce", &conv1x1_dgrad_bn_reduce, py::arg("x"), py::arg("w"), py::arg("residual"),
+            py::arg("bn_x"), py::arg("coef"), py::arg("mask"), py::kw_only(), py::arg("num_sms") = 0);
     mod.def("stem_can_fuse", &stem_can_fuse);
     mod.def("stem_forward", &stem_forward);
     mod.def("stem_wgrad", &stem_wgrad);

@@ -66,6 +66,14 @@ def build_parser(adpsgd: bool = False) -> argparse.ArgumentParser:
                         'optim.lars_groups (no decay and no LARS for ndim <= 1 parameters).  --fused True '
                         'with SGP / OSGP / D-PSGD only')
     p.add_argument('--lars_trust', default=0.001, type=float, help='LARS trust coefficient eta')
+    p.add_argument('--clip_grad_norm', default=0.0, type=float,
+                   help='clip each rank\'s gradient to this global 2-norm inside the fused gossip step '
+                        '(FusedGossipSGD(max_grad_norm=...), torch.nn.utils.clip_grad_norm_ semantics); '
+                        '0 = off.  --fused True with SGP / OSGP / D-PSGD only')
+    p.add_argument('--skip_nonfinite', default=False, **B,
+                   help='skip the SGD of a step whose gradient norm is inf or NaN on that rank (the rank '
+                        'keeps gossiping; FusedGossipSGD(skip_nonfinite=True)).  --fused True with SGP / '
+                        'OSGP / D-PSGD only')
     p.add_argument('--push_sum', default=True, **B, help='push-sum (SGP) or push-pull (D-PSGD)')
     p.add_argument('--graph_type', default=5, type=int, choices=list(GRAPH_TOPOLOGIES))
     p.add_argument('--mixing_strategy', default=0, type=int, choices=list(MIXING_STRATEGIES))
@@ -271,6 +279,7 @@ def finalize_args(args, adpsgd=False):
                              'step (FusedGossipSGD) for SGP, OSGP and D-PSGD' % unsupported)
         if not args.lars_trust > 0:
             raise ValueError('--lars_trust must be > 0')
+    check_grad_clip_flags(args, adpsgd)
     if getattr(args, 'slowmo_frequency', 0):
         unsupported = ('AD-PSGD' if adpsgd else '--all_reduce' if args.all_reduce else
                        '--nprocs_per_node > 1' if getattr(args, 'nprocs_per_node', 1) > 1 else None)
@@ -338,6 +347,23 @@ def check_mix_flags(args):
         v = getattr(args, flag, 0.0)
         if not 0.0 <= v <= 1.0:
             raise ValueError('--%s must be in [0, 1], got %r' % (flag, v))
+
+
+def check_grad_clip_flags(args, adpsgd=False):
+    """ValueError for --clip_grad_norm / --skip_nonfinite outside the fused gossip step, or for a
+    negative or non-finite --clip_grad_norm."""
+    clip = getattr(args, 'clip_grad_norm', 0.0)
+    if not (clip >= 0 and clip != float('inf')):
+        raise ValueError('--clip_grad_norm must be a finite number >= 0 (0 = off), got %r' % (clip,))
+    for flag, on in (('--clip_grad_norm', clip > 0), ('--skip_nonfinite', getattr(args, 'skip_nonfinite', False))):
+        if not on:
+            continue
+        unsupported = ('AD-PSGD' if adpsgd else '--all_reduce' if args.all_reduce else
+                       '--fused False' if not getattr(args, 'fused', True) else None)
+        if unsupported:
+            raise ValueError('%s is not supported with %s: gradient clipping and non-finite step skipping '
+                             'are implemented in the fused gossip step (FusedGossipSGD) for SGP, OSGP and '
+                             'D-PSGD' % (flag, unsupported))
 
 
 def check_ema_flags(args, adpsgd=False):

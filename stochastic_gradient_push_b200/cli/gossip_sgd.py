@@ -78,7 +78,9 @@ def build_model_and_optimizer(args, log):
     if args.fused:
         optimizer = FusedGossipSGD(model, lr=args.lr, momentum=args.momentum,
                                    weight_decay=args.weight_decay, nesterov=args.nesterov,
-                                   param_groups=groups, lars=args.lars, trust_coefficient=args.lars_trust)
+                                   param_groups=groups, lars=args.lars, trust_coefficient=args.lars_trust,
+                                   max_grad_norm=args.clip_grad_norm if args.clip_grad_norm > 0 else None,
+                                   skip_nonfinite=args.skip_nonfinite)
     else:
         optimizer = torch.optim.SGD(groups if groups is not None else model.parameters(), lr=args.lr,
                                     momentum=args.momentum, weight_decay=args.weight_decay,
@@ -359,6 +361,10 @@ def train(args, model, criterion, optimizer, batch_meter, data_meter, nn_meter, 
             top1.update(a1, n)
             top5.update(a5, n)
     csv.train_row(epoch, i, batch_meter, nn_meter, data_meter, losses, top1, top5)
+    grad_norm = getattr(optimizer, 'grad_norm', None)       # (--clip_grad_norm / --skip_nonfinite)
+    if grad_norm is not None:
+        log.info('epoch {} last gradient norm {:.6e} non-finite steps skipped {}'.format(
+            epoch, float(grad_norm), optimizer.nonfinite_steps))
     return losses.avg
 
 

@@ -272,87 +272,40 @@ public:
 
     // LARS (SGP_F_LARS on every SGD launch of step(), which then enqueues norms -> trust -> step).
     // `offsets` / `numels`: int64 CPU tensors, the arena layout (every offset a multiple of 64,
-    // ascending); `enabled`: uint8 / bool CPU tensor, one per tensor.  Builds the block -> tensor
-    // map, the tile table and every buffer the two LARS kernels use here, once: a captured launch
-    // allocates nothing.  `offsets` undefined: LARS off.
+    // ascending); `enabled`: uint8 / bool CPU tensor, one per tensor.  Builds the norm plan (see
+    // set_norm_plan) and the LARS buffers here, once: a captured launch allocates nothing.
+    // `offsets` undefined: LARS off.
     void set_lars(c10::optional<torch::Tensor> offsets, c10::optional<torch::Tensor> numels,
                   c10::optional<torch::Tensor> enabled, double eta, double eps)
     {
         if (!(offsets.has_value() && offsets->defined())) {
-            args_.block_tensor = nullptr;
             args_.lars_trust = nullptr;
             args_.lars_enabled = nullptr;
-            args_.lars_tiles = nullptr;
-            args_.lars_tile_first = nullptr;
-            args_.lars_partials = nullptr;
             args_.lars_sumsq = nullptr;
-            args_.lars_tensors = args_.lars_ntiles = 0;
             lars_keep_ = {};
             lars_trust_ = lars_sumsq_ = torch::Tensor();
+            if (!args_.clip) set_norm_plan(torch::Tensor(), torch::Tensor(), "LARS", false);
             return;
         }
         TORCH_CHECK(numels.has_value() && numels->defined() && enabled.has_value() && enabled->defined(),
                     "set_lars takes offsets, numels and enabled together");
-        const torch::Tensor off = offsets->to(torch::kCPU, torch::kInt64).contiguous();
-        const torch::Tensor num = numels->to(torch::kCPU, torch::kInt64).contiguous();
         const torch::Tensor en = enabled->to(torch::kCPU, torch::kUInt8).contiguous();
-        const int64_t T = off.numel();
-        TORCH_CHECK(T >= 1 && T <= SGP_LARS_MAX_TENSORS, "LARS supports 1 to ", SGP_LARS_MAX_TENSORS,
-                    " tensors in the fp32 arena, got ", T);
-        TORCH_CHECK(num.numel() == T && en.numel() == T, "offsets, numels and enabled differ in length");
         TORCH_CHECK(eta > 0.0 && eps >= 0.0, "LARS needs trust_coefficient > 0 and eps >= 0");
-        const int64_t* po = off.data_ptr<int64_t>();
-        const int64_t* pn = num.data_ptr<int64_t>();
-        const int64_t nblocks = args_.n / SGP_GROUP_BLOCK;
-        auto cpu16 = torch::TensorOptions().dtype(torch::kInt16);
-        torch::Tensor bt = torch::zeros({nblocks}, cpu16);       // (uint16 bits in int16 storage)
-        uint16_t* pbt = reinterpret_cast<uint16_t*>(bt.data_ptr<int16_t>());
-        std::vector<int64_t> tiles;                              // start, tensor | count << 32
-        std::vector<int32_t> first(T + 1, 0);
-        int64_t prev_end = 0;
-        for (int64_t t = 0; t < T; ++t) {
-            TORCH_CHECK(po[t] % SGP_GROUP_BLOCK == 0 && pn[t] >= 1 && po[t] >= prev_end &&
-                        po[t] + pn[t] <= args_.n,
-                        "LARS tensor ", t, " is not a 64-aligned, ascending slice of the arena");
-            prev_end = po[t] + pn[t];
-            for (int64_t b = po[t] / SGP_GROUP_BLOCK; b < (prev_end + SGP_GROUP_BLOCK - 1) / SGP_GROUP_BLOCK; ++b)
-                pbt[b] = (uint16_t)t;
-            first[t] = (int32_t)(tiles.size() / 2);
-            for (int64_t s = 0; s < pn[t]; s += SGP_LARS_TILE) {
-                const int64_t cnt = std::min<int64_t>(SGP_LARS_TILE, pn[t] - s);
-                tiles.push_back(po[t] + s);
-                tiles.push_back(t | (cnt << 32));
-            }
-        }
-        const int64_t ntiles = (int64_t)tiles.size() / 2;
-        first[T] = (int32_t)ntiles;
-        TORCH_CHECK(ntiles < (1ll << 31), "too many LARS tiles");
-        static_assert(sizeof(SgpLarsTile) == 16, "SgpLarsTile is {int64 start; int32 tensor; int32 count}");
+        TORCH_CHECK(en.numel() == offsets->numel(), "offsets, numels and enabled differ in length");
+        set_norm_plan(*offsets, *numels, "LARS", args_.clip != nullptr);
+        const int64_t T = args_.lars_tensors;
         const auto dev = torch::TensorOptions().device(torch::kCUDA, device_);
-        torch::Tensor tiles_t = torch::from_blob(tiles.data(), {ntiles, 2}, torch::kInt64).to(dev.dtype(torch::kInt64));
-        torch::Tensor first_t = torch::from_blob(first.data(), {T + 1}, torch::kInt32).to(dev.dtype(torch::kInt32));
-        torch::Tensor bt_d = bt.to(dev.dtype(torch::kInt16));
         torch::Tensor en_d = en.to(dev.dtype(torch::kUInt8));
         lars_trust_ = torch::ones({T}, dev.dtype(torch::kFloat32));
         lars_sumsq_ = torch::zeros({T, 2}, dev.dtype(torch::kFloat64));
-        torch::Tensor partials = torch::zeros({ntiles, 2}, dev.dtype(torch::kFloat64));
-        args_.block_tensor = reinterpret_cast<const uint16_t*>(bt_d.data_ptr<int16_t>());
         args_.lars_trust = lars_trust_.data_ptr<float>();
         args_.lars_enabled = en_d.data_ptr<uint8_t>();
-        args_.lars_tiles = reinterpret_cast<const SgpLarsTile*>(tiles_t.data_ptr<int64_t>());
-        args_.lars_tile_first = first_t.data_ptr<int32_t>();
-        args_.lars_partials = partials.data_ptr<double>();
         args_.lars_sumsq = lars_sumsq_.data_ptr<double>();
-        args_.lars_tensors = (int)T;
-        args_.lars_ntiles = (int)ntiles;
         args_.lars_eta = (float)eta;
         args_.lars_eps = (float)eps;
-        lars_keep_ = {bt_d, en_d, tiles_t, first_t, partials};
-        int sms = 0;
-        SGP_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device_));
-        lars_grid_ = (int)std::max<int64_t>(1, std::min<int64_t>(ntiles, 8ll * std::max(sms, 1)));
+        lars_keep_ = {en_d};
     }
-    bool lars() const { return args_.lars_tensors > 0; }
+    bool lars() const { return args_.lars_trust != nullptr; }
     int lars_tiles() const { return args_.lars_ntiles; }
     int lars_grid() const { return lars_grid_; }
     void set_lars_grid(int grid) { TORCH_CHECK(grid >= 1, "grid >= 1"); lars_grid_ = grid; }
@@ -362,11 +315,54 @@ public:
     // the norm and trust kernels alone, as the next SGD launch would run them (benchmarks, tests)
     void lars_update()
     {
-        TORCH_CHECK(args_.lars_tensors > 0 && args_.groups > 0 && args_.g, "LARS is not configured");
+        TORCH_CHECK(args_.lars_trust && args_.groups > 0 && args_.g, "LARS is not configured");
         SgpArgs a = prepare(SGP_F_SGD | SGP_F_GROUPS | SGP_F_LARS);
         c10::cuda::CUDAGuard guard(device_);
         SGP_CUDA_CHECK(sgp_launch_lars_norms(&a, lars_grid_, at::cuda::getCurrentCUDAStream()));
         SGP_CUDA_CHECK(sgp_launch_lars_trust(&a, at::cuda::getCurrentCUDAStream()));
+    }
+
+    // Gradient-norm clipping and non-finite step skipping (SGP_F_CLIP on every SGD launch of step(),
+    // which then enqueues norms -> clip finalize [-> LARS trust] -> step).  `offsets` / `numels` as in
+    // set_lars (the same norm plan serves both); `state`: a device buffer of at least
+    // sizeof(SgpClipState) bytes that the finalize kernel writes (the caller keeps it, so the skip
+    // counter outlives a reconfiguration).  `clip_norm`: clip to max_grad_norm = hyper[6]; `skip`:
+    // skip the SGD of a launch whose gradient norm is not finite.  `offsets` undefined: off.
+    void set_grad_clip(c10::optional<torch::Tensor> offsets, c10::optional<torch::Tensor> numels,
+                       c10::optional<torch::Tensor> state, bool clip_norm, bool skip)
+    {
+        if (!(offsets.has_value() && offsets->defined())) {
+            args_.clip = nullptr;
+            args_.clip_norm = args_.clip_skip = 0;
+            clip_keep_ = torch::Tensor();
+            if (!args_.lars_trust) set_norm_plan(torch::Tensor(), torch::Tensor(), "clipping", false);
+            return;
+        }
+        TORCH_CHECK(numels.has_value() && numels->defined() && state.has_value() && state->defined(),
+                    "set_grad_clip takes offsets, numels and state together");
+        const torch::Tensor& st = *state;
+        TORCH_CHECK(st.is_cuda() && st.get_device() == device_ && st.is_contiguous() &&
+                    st.numel() * st.element_size() >= (int64_t)sizeof(SgpClipState) &&
+                    reinterpret_cast<uintptr_t>(st.data_ptr()) % alignof(SgpClipState) == 0,
+                    "the clip state must be a contiguous, 16-byte aligned device buffer of at least ",
+                    sizeof(SgpClipState), " bytes on the arena's device");
+        TORCH_CHECK(clip_norm || skip, "set_grad_clip needs clipping or skipping (or offsets=None)");
+        set_norm_plan(*offsets, *numels, "clipping", args_.lars_trust != nullptr);
+        args_.clip = reinterpret_cast<SgpClipState*>(st.data_ptr());
+        args_.clip_norm = clip_norm ? 1 : 0;
+        args_.clip_skip = skip ? 1 : 0;
+        clip_keep_ = st;
+    }
+    bool grad_clip() const { return args_.clip != nullptr; }
+    // the norm and clip kernels alone, as the next SGD launch would run them (benchmarks, tests);
+    // like an SGD launch, they leave the state alone while hyper do_sgd is 0
+    void clip_update()
+    {
+        TORCH_CHECK(args_.clip && args_.g, "gradient clipping is not configured");
+        SgpArgs a = prepare(SGP_F_SGD | SGP_F_CLIP);
+        c10::cuda::CUDAGuard guard(device_);
+        SGP_CUDA_CHECK(sgp_launch_lars_norms(&a, lars_grid_, at::cuda::getCurrentCUDAStream()));
+        SGP_CUDA_CHECK(sgp_launch_grad_clip(&a, at::cuda::getCurrentCUDAStream()));
     }
 
     void step(unsigned int flags, int grid)
@@ -382,19 +378,21 @@ public:
         }
         if (a.flags & SGP_F_SGD) TORCH_CHECK(a.g && a.m, "SGD needs grad + momentum buffers");
         if ((a.flags & SGP_F_SGD) && a.groups > 0) a.flags |= SGP_F_GROUPS;
-        if ((a.flags & SGP_F_SGD) && a.lars_tensors > 0) {
+        if ((a.flags & SGP_F_SGD) && a.lars_trust) {
             TORCH_CHECK(a.flags & SGP_F_GROUPS, "LARS needs the parameter-group block map (set_param_groups)");
             a.flags |= SGP_F_LARS;
         }
+        if ((a.flags & SGP_F_SGD) && a.clip) a.flags |= SGP_F_CLIP;
         if (a.flags & SGP_F_FOLD_RES) TORCH_CHECK(a.residual, "fold needs a residual buffer");
         if (a.flags & SGP_F_PUBLISH) TORCH_CHECK(a.outboxes, "publish needs outboxes");
         if (a.flags & SGP_F_PHASE2) TORCH_CHECK(a.flags & SGP_F_PUBLISH, "phase 2 needs publish");
         c10::cuda::CUDAGuard guard(device_);
-        if (a.flags & SGP_F_LARS) {
-            // norms of the x and g^ this launch's phase 1 sees, then the trust ratios, on the same stream
+        // norms of the x and g^ this launch's phase 1 sees, then the clip coefficient and the trust
+        // ratios (which read it), all on the same stream
+        if (a.flags & (SGP_F_LARS | SGP_F_CLIP))
             SGP_CUDA_CHECK(sgp_launch_lars_norms(&a, lars_grid_, at::cuda::getCurrentCUDAStream()));
-            SGP_CUDA_CHECK(sgp_launch_lars_trust(&a, at::cuda::getCurrentCUDAStream()));
-        }
+        if (a.flags & SGP_F_CLIP) SGP_CUDA_CHECK(sgp_launch_grad_clip(&a, at::cuda::getCurrentCUDAStream()));
+        if (a.flags & SGP_F_LARS) SGP_CUDA_CHECK(sgp_launch_lars_trust(&a, at::cuda::getCurrentCUDAStream()));
         const unsigned int full = SGP_F_PHASE1 | SGP_F_PUBLISH | SGP_F_PHASE2;
         const unsigned int not_piped = SGP_F_FOLD_RES | SGP_F_NO_ROTATE | SGP_F_KEEP_Z | SGP_F_SELF_FROM_Z;
         if (use_pipe_ && (a.flags & full) == full && (a.flags & not_piped) == 0)
@@ -582,6 +580,77 @@ public:
     int segments() const { return args_.segments; }
 
 private:
+    // The norm plan of LARS and clipping: the block -> tensor map, the tile table (tiles never cross
+    // a tensor boundary) and the partials buffer.  It depends on the arena layout only, so it is
+    // built once and kept while either feature uses it; a second caller with the same layout reuses
+    // it (`other_on`: the other feature uses the plan, so the layout may not change).  Undefined
+    // offsets drop it.
+    void set_norm_plan(const torch::Tensor& offsets, const torch::Tensor& numels, const char* what, bool other_on)
+    {
+        if (!offsets.defined()) {
+            args_.block_tensor = nullptr;
+            args_.lars_tiles = nullptr;
+            args_.lars_tile_first = nullptr;
+            args_.lars_partials = nullptr;
+            args_.lars_tensors = args_.lars_ntiles = 0;
+            plan_keep_ = {};
+            plan_offsets_ = plan_numels_ = torch::Tensor();
+            return;
+        }
+        const torch::Tensor off = offsets.to(torch::kCPU, torch::kInt64).contiguous();
+        const torch::Tensor num = numels.to(torch::kCPU, torch::kInt64).contiguous();
+        if (plan_offsets_.defined() && plan_offsets_.equal(off) && plan_numels_.equal(num)) return;
+        TORCH_CHECK(!other_on, "LARS and gradient clipping must describe the same arena layout");
+        const int64_t T = off.numel();
+        TORCH_CHECK(T >= 1 && T <= SGP_LARS_MAX_TENSORS, what, " supports 1 to ", SGP_LARS_MAX_TENSORS,
+                    " tensors in the fp32 arena, got ", T);
+        TORCH_CHECK(num.numel() == T, "offsets and numels differ in length");
+        const int64_t* po = off.data_ptr<int64_t>();
+        const int64_t* pn = num.data_ptr<int64_t>();
+        const int64_t nblocks = args_.n / SGP_GROUP_BLOCK;
+        auto cpu16 = torch::TensorOptions().dtype(torch::kInt16);
+        torch::Tensor bt = torch::zeros({nblocks}, cpu16);       // (uint16 bits in int16 storage)
+        uint16_t* pbt = reinterpret_cast<uint16_t*>(bt.data_ptr<int16_t>());
+        std::vector<int64_t> tiles;                              // start, tensor | count << 32
+        std::vector<int32_t> first(T + 1, 0);
+        int64_t prev_end = 0;
+        for (int64_t t = 0; t < T; ++t) {
+            TORCH_CHECK(po[t] % SGP_GROUP_BLOCK == 0 && pn[t] >= 1 && po[t] >= prev_end &&
+                        po[t] + pn[t] <= args_.n,
+                        what, " tensor ", t, " is not a 64-aligned, ascending slice of the arena");
+            prev_end = po[t] + pn[t];
+            for (int64_t b = po[t] / SGP_GROUP_BLOCK; b < (prev_end + SGP_GROUP_BLOCK - 1) / SGP_GROUP_BLOCK; ++b)
+                pbt[b] = (uint16_t)t;
+            first[t] = (int32_t)(tiles.size() / 2);
+            for (int64_t s = 0; s < pn[t]; s += SGP_LARS_TILE) {
+                const int64_t cnt = std::min<int64_t>(SGP_LARS_TILE, pn[t] - s);
+                tiles.push_back(po[t] + s);
+                tiles.push_back(t | (cnt << 32));
+            }
+        }
+        const int64_t ntiles = (int64_t)tiles.size() / 2;
+        first[T] = (int32_t)ntiles;
+        TORCH_CHECK(ntiles < (1ll << 31), "too many norm tiles");
+        static_assert(sizeof(SgpLarsTile) == 16, "SgpLarsTile is {int64 start; int32 tensor; int32 count}");
+        const auto dev = torch::TensorOptions().device(torch::kCUDA, device_);
+        torch::Tensor tiles_t = torch::from_blob(tiles.data(), {ntiles, 2}, torch::kInt64).to(dev.dtype(torch::kInt64));
+        torch::Tensor first_t = torch::from_blob(first.data(), {T + 1}, torch::kInt32).to(dev.dtype(torch::kInt32));
+        torch::Tensor bt_d = bt.to(dev.dtype(torch::kInt16));
+        torch::Tensor partials = torch::zeros({ntiles, 2}, dev.dtype(torch::kFloat64));
+        args_.block_tensor = reinterpret_cast<const uint16_t*>(bt_d.data_ptr<int16_t>());
+        args_.lars_tiles = reinterpret_cast<const SgpLarsTile*>(tiles_t.data_ptr<int64_t>());
+        args_.lars_tile_first = first_t.data_ptr<int32_t>();
+        args_.lars_partials = partials.data_ptr<double>();
+        args_.lars_tensors = (int)T;
+        args_.lars_ntiles = (int)ntiles;
+        plan_keep_ = {bt_d, tiles_t, first_t, partials};
+        plan_offsets_ = off.clone();
+        plan_numels_ = num.clone();
+        int sms = 0;
+        SGP_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device_));
+        lars_grid_ = (int)std::max<int64_t>(1, std::min<int64_t>(ntiles, 8ll * std::max(sms, 1)));
+    }
+
     SgpArgs prepare(unsigned int flags) const
     {
         SgpArgs a = args_;
@@ -615,7 +684,10 @@ private:
     torch::Tensor grad2_keep_;
     torch::Tensor mom_keep_;
     std::vector<torch::Tensor> groups_keep_;
+    std::vector<torch::Tensor> plan_keep_;
+    torch::Tensor plan_offsets_, plan_numels_;
     std::vector<torch::Tensor> lars_keep_;
+    torch::Tensor clip_keep_;
     torch::Tensor lars_trust_;
     torch::Tensor lars_sumsq_;
     int lars_grid_ = 1;
@@ -951,6 +1023,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, mod)
     mod.attr("F_LARS") = (unsigned)SGP_F_LARS;
     mod.attr("LARS_TILE") = (int)SGP_LARS_TILE;
     mod.attr("LARS_MAX_TENSORS") = (int)SGP_LARS_MAX_TENSORS;
+    mod.attr("F_CLIP") = (unsigned)SGP_F_CLIP;
+    mod.attr("CLIP_STATE_BYTES") = (int)sizeof(SgpClipState);
+    mod.attr("CLIP_OFF_SUMSQ") = (int)offsetof(SgpClipState, sumsq);
+    mod.attr("CLIP_OFF_TOTAL") = (int)offsetof(SgpClipState, total);
+    mod.attr("CLIP_OFF_COEF") = (int)offsetof(SgpClipState, coef);
+    mod.attr("CLIP_OFF_SKIP") = (int)offsetof(SgpClipState, skip);
+    mod.attr("CLIP_OFF_SKIPPED") = (int)offsetof(SgpClipState, skipped);
 
     py::class_<BilatDaemon>(mod, "BilatDaemon")
         .def(py::init<std::shared_ptr<GossipContext>, int, bool, double, int, double>(), py::arg("ctx"),
@@ -999,6 +1078,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, mod)
         .def("lars_trust", &GossipContext::lars_trust)
         .def("lars_sumsq", &GossipContext::lars_sumsq)
         .def("lars_update", &GossipContext::lars_update)
+        .def("set_grad_clip", &GossipContext::set_grad_clip, py::arg("offsets"), py::arg("numels"),
+             py::arg("state"), py::arg("clip_norm"), py::arg("skip"))
+        .def("grad_clip", &GossipContext::grad_clip)
+        .def("clip_update", &GossipContext::clip_update)
         .def("set_timeout", &GossipContext::set_timeout)
         .def("set_segments", &GossipContext::set_segments)
         .def("bilat_decide", &GossipContext::bilat_decide, py::arg("pub_grid"), py::arg("passive"),

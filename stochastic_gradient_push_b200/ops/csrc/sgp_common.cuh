@@ -91,7 +91,7 @@ struct SgpHyper {
     float nesterov;      // 0 / 1
     float do_sgd;        // 0 / 1  (first overlap step has no gradient yet)
     float grad_scale;    // multiplies the gradient (1/nprocs, loss-scale^-1 ...)
-    float _pad[2];
+    float _pad[2];       // _pad[0]: max_grad_norm of SGP_F_CLIP (read by sgp_grad_clip_kernel)
 };
 
 // kernel mode bits
@@ -125,12 +125,27 @@ struct SgpHyper {
 #define SGP_F_LARS       (1u << 15)
 #define SGP_LARS_TILE    4096   // elements per norm tile (a tile never crosses a tensor boundary)
 #define SGP_LARS_MAX_TENSORS 65535
+// gradient-norm clipping / non-finite step skipping (SGD modes): sgp_lars_norms_kernel and
+// sgp_grad_clip_kernel run right before the step on the same stream and leave the clip
+// coefficient and the skip flag in *clip; phase 1 scales g^ by the coefficient, or, under skip,
+// leaves x and m alone and only clears the gradient.  Needs neither SGP_F_GROUPS nor SGP_F_LARS
+#define SGP_F_CLIP       (1u << 16)
 
 // one norm tile: `count` elements of tensor `tensor` from arena element `start` (a multiple of 64)
 struct SgpLarsTile {
     long long start;
     int       tensor;
     int       count;
+};
+
+// device clip state (SGP_F_CLIP), written by sgp_grad_clip_kernel at every SGD launch
+struct __align__(16) SgpClipState {
+    double   sumsq;      // sum of g^2 over every tensor of the norm plan, g = grad_scale * (g [+ g2])
+    float    total;      // sqrt(sumsq), rounded to fp32: the norm before clipping
+    float    coef;       // min(max_grad_norm / (total + 1e-6), 1) (NaN stays NaN); 1 without clipping
+    uint32_t skip;       // 1: skip_nonfinite and total is not finite: this launch skips its SGD
+    uint32_t skipped;    // SGD launches skipped so far
+    uint32_t _pad[2];
 };
 
 struct SgpArgs {
@@ -176,6 +191,11 @@ struct SgpArgs {
     int                  lars_ntiles;
     float                lars_eta;       // trust coefficient
     float                lars_eps;
+    // SGP_F_CLIP (appended after the LARS fields; the norm plan above -- tiles, tile_first,
+    // partials, tensors, ntiles -- serves LARS and clipping alike)
+    SgpClipState*        clip;           // device clip state
+    int                  clip_norm;      // 1: clip to hyper->_pad[0]; 0: coef stays 1 (skip only)
+    int                  clip_skip;      // 1: skip the SGD of a launch whose norm is not finite
 };
 
 #ifdef __CUDACC__
@@ -314,6 +334,7 @@ cudaError_t sgp_launch_step_pipe(const SgpArgs* args, int grid, cudaStream_t str
 int sgp_max_resident_ctas_pipe(int device);
 cudaError_t sgp_launch_lars_norms(const SgpArgs* args, int grid, cudaStream_t stream);
 cudaError_t sgp_launch_lars_trust(const SgpArgs* args, cudaStream_t stream);
+cudaError_t sgp_launch_grad_clip(const SgpArgs* args, cudaStream_t stream);
 cudaError_t sgp_launch_gather(const SgpArgs* args, int grid, int pub_grid, cudaStream_t stream);
 cudaError_t sgp_launch_gather_tma(const SgpArgs* args, int grid, int pub_grid, cudaStream_t stream);
 cudaError_t sgp_launch_probe(const SgpArgs* args, int pub_grid, uint32_t* host_flag,

@@ -23,7 +23,9 @@
 //   sgp_snapshot_kernel, sgp_consensus_kernel, sgp_consensus_finalize_kernel
 //                      consensus distance and the push-sum average model
 //   sgp_slowmo_kernel  SlowMo: exact average + slow-momentum update
-//   sgp_lars_norms_kernel, sgp_lars_trust_kernel   LARS trust ratios for the step kernels
+//   sgp_lars_norms_kernel  per-tile norms of the norm plan (LARS and gradient clipping)
+//   sgp_lars_trust_kernel  LARS trust ratios for the step kernels
+//   sgp_grad_clip_kernel   global gradient norm, clip coefficient and non-finite skip flag
 //
 // What several kernels share is written once, ahead of the kernels:
 //   phase1_chunk       phase 1 of both step kernels for one chunk (sgd4, store_z)
@@ -136,9 +138,30 @@ __device__ __forceinline__ void store_z(const SgpArgs& a, uint32_t flags, long l
     if (flags & SGP_F_SHADOW) st_u2(reinterpret_cast<uint2*>(a.shadow + i), f4_to_bf16x4(zv));
 }
 
+// What phase 1 does with the gradient, read once per CTA.  sgd: the launch applies SGD (SGP_F_SGD
+// and hyper->do_sgd).  With SGP_F_CLIP the clip state that sgp_grad_clip_kernel wrote earlier on
+// the stream folds the coefficient into the scale (exact when it is 1) and, under skip, turns the
+// update off but keeps clearing the gradient
+struct SgdControls {
+    float gscale;
+    bool  do_sgd;      // apply the update to x and m
+    bool  clear_g;     // clear the gradient (SGP_F_ZERO_GRAD)
+};
+__device__ __forceinline__ SgdControls sgd_controls(const SgpArgs& a, uint32_t flags, const SgpHyper& hp) {
+    const bool sgd = (flags & SGP_F_SGD) && (hp.do_sgd != 0.f);
+    SgdControls c{hp.grad_scale, sgd, sgd && (flags & SGP_F_ZERO_GRAD) != 0u};
+    if (sgd && (flags & SGP_F_CLIP)) {
+        c.gscale = hp.grad_scale * a.clip->coef;
+        c.do_sgd = a.clip->skip == 0u;
+    }
+    return c;
+}
+
 // ---- phase 1 of the step kernels, one chunk -----------------------------------
-// All SGP_UNROLL loads first, then per access: x = z * wmul ; SGD (clearing the gradient with
-// SGP_F_ZERO_GRAD) ; + rscale * residual ; publish ; z = x / w1.
+// All SGP_UNROLL loads first, then per access: x = z * wmul ; SGD with g^ = gscale * g (do_sgd) ;
+// clear the gradient (clear_g) ; + rscale * residual ; publish ; z = x / w1.
+// gscale = grad_scale * clip coefficient and do_sgd / clear_g come from sgd_controls: a step that
+// SGP_F_CLIP skips has do_sgd false and clear_g true, so x and m keep their bits.
 // MSG_BF16: publish Q(x) = bf16(x) and keep what was not sent, c = x - (1 - self_w) Q(x), in z.
 // FULL_STEP (sgp_step_pipe_kernel: always PHASE1 | PUBLISH | PHASE2, never FOLD_RES) compiles the
 // residual fold, the test of SGP_F_PUBLISH and the z store out; rscale, inv_w1 and write_z are
@@ -146,7 +169,8 @@ __device__ __forceinline__ void store_z(const SgpArgs& a, uint32_t flags, long l
 template <bool MSG_BF16, bool GROUPS, bool LARS, bool FULL_STEP>
 __device__ __forceinline__ void phase1_chunk(
     const SgpArgs& a, const uint32_t flags, const long long c, const int tid, const SgpHyper& hp,
-    const bool do_sgd, const float4* s_rows, const float wmul, const float self_w,
+    const float gscale, const bool do_sgd, const bool clear_g, const float4* s_rows, const float wmul,
+    const float self_w,
     typename std::conditional<MSG_BF16, __nv_bfloat16, float>::type* my_out, const uint64_t pol_first,
     const uint64_t pol_last, const float rscale, const float inv_w1, const bool write_z)
 {
@@ -181,23 +205,23 @@ __device__ __forceinline__ void phase1_chunk(
         const long long i = chunk_elem(base, u);
         float4 xv = mul4(x[u], wmul);               // numerator (exact if w == 1)
         if (do_sgd) {
-            const float4 gv = mul4(g[u], hp.grad_scale);
+            const float4 gv = mul4(g[u], gscale);
             float4 mv = m[u];
             float t = 1.f;
             if constexpr (LARS) t = tr[u];
             if constexpr (GROUPS) sgd4<LARS>(xv, gv, mv, s_rows[grp[u]], t);
             else                  sgd4<LARS>(xv, gv, mv, hyper_row(hp), t);
             st_f4(reinterpret_cast<float4*>(a.m + i), mv);
-            if (flags & SGP_F_ZERO_GRAD) {
-                if (flags & SGP_F_GRAD_BF16)
-                    st_u2(reinterpret_cast<uint2*>(
-                              reinterpret_cast<__nv_bfloat16*>(a.g) + i), make_uint2(0u, 0u));
-                else
-                    st_f4(reinterpret_cast<float4*>(reinterpret_cast<float*>(a.g) + i),
-                          make_float4(0.f, 0.f, 0.f, 0.f));
-                if (a.g2 != nullptr)
-                    st_f4(reinterpret_cast<float4*>(a.g2 + i), make_float4(0.f, 0.f, 0.f, 0.f));
-            }
+        }
+        if (clear_g) {
+            if (flags & SGP_F_GRAD_BF16)
+                st_u2(reinterpret_cast<uint2*>(
+                          reinterpret_cast<__nv_bfloat16*>(a.g) + i), make_uint2(0u, 0u));
+            else
+                st_f4(reinterpret_cast<float4*>(reinterpret_cast<float*>(a.g) + i),
+                      make_float4(0.f, 0.f, 0.f, 0.f));
+            if (a.g2 != nullptr)
+                st_f4(reinterpret_cast<float4*>(a.g2 + i), make_float4(0.f, 0.f, 0.f, 0.f));
         }
         if (fold)      // (rscale: 1 after a gather kernel, the edge weight after a DMA gather)
             xv = fma4(r[u], rscale, xv);
@@ -453,7 +477,7 @@ sgp_step_kernel(const SgpArgs a)
     const SgpHyper hp = *a.hyper;
     const uint64_t pol_first = l2_evict_first_policy();
     const uint64_t pol_last = l2_evict_last_policy();
-    const bool do_sgd = (flags & SGP_F_SGD) && (hp.do_sgd != 0.f);
+    const SgdControls sc = sgd_controls(a, flags, hp);
     const float4* s_rows = nullptr;
     if constexpr (GROUPS) {
         __shared__ float4 s_group_rows[SGP_MAX_GROUPS];
@@ -499,9 +523,9 @@ sgp_step_kernel(const SgpArgs a)
         // ---------------- phase 1: local update + publish ------------------
         if (flags & SGP_F_PHASE1) {
             for (long long it = it_lo; it < it_hi; ++it)
-                phase1_chunk<MSG_BF16, GROUPS, LARS, false>(a, flags, b + it * gridDim.x, tid, hp, do_sgd, s_rows,
-                                                            wmul, row.self_w, my_out, pol_first, pol_last,
-                                                            rscale, inv_w1, write_z);
+                phase1_chunk<MSG_BF16, GROUPS, LARS, false>(a, flags, b + it * gridDim.x, tid, hp, sc.gscale,
+                                                            sc.do_sgd, sc.clear_g, s_rows, wmul, row.self_w,
+                                                            my_out, pol_first, pol_last, rscale, inv_w1, write_z);
             if (flags & SGP_F_PUBLISH) {
                 __syncthreads();
                 if (tid == 0) {
@@ -888,7 +912,7 @@ sgp_step_pipe_kernel(const SgpArgs a)
         const SgpHyper hp = *a.hyper;
         const uint64_t pol_first = l2_evict_first_policy();
         const uint64_t pol_last = l2_evict_last_policy();
-        const bool do_sgd = (flags & SGP_F_SGD) && (hp.do_sgd != 0.f);
+        const SgdControls sc = sgd_controls(a, flags, hp);
         const int lane = tid & 31;
 
         if (outbox_was_read(a, step)) {
@@ -906,9 +930,9 @@ sgp_step_pipe_kernel(const SgpArgs a)
             if (seg < K) {
                 const long long it_lo = my_chunks * seg / K, it_hi = my_chunks * (seg + 1) / K;
                 for (long long it = it_lo; it < it_hi; ++it)
-                    phase1_chunk<MSG_BF16, GROUPS, LARS, true>(a, flags, b + it * gridDim.x, tid, hp, do_sgd, s_rows,
-                                                               wmul, row.self_w, my_out, pol_first, pol_last,
-                                                               1.f, inv_w1, false);
+                    phase1_chunk<MSG_BF16, GROUPS, LARS, true>(a, flags, b + it * gridDim.x, tid, hp, sc.gscale,
+                                                               sc.do_sgd, sc.clear_g, s_rows, wmul, row.self_w,
+                                                               my_out, pol_first, pol_last, 1.f, inv_w1, false);
                 asm volatile("bar.sync 1, %0;" :: "n"(PIPE_CONSUMERS) : "memory");
                 if (tid == 0) {
                     if (seg == 0) st_relaxed_sys_f32(&mypad->psw[parity], w1);
@@ -1572,14 +1596,16 @@ sgp_slowmo_kernel(const SgpArgs a, float* u, float* x_prev, float lr, float alph
 }
 
 // ---------------------------------------------------------------------------
-// LARS (SGP_F_LARS): per-tensor trust ratios, computed right before each SGD launch.
+// The norm plan: LARS (SGP_F_LARS) per-tensor trust ratios and gradient clipping (SGP_F_CLIP),
+// computed right before each SGD launch.
 //
 // sgp_lars_norms_kernel: grid-stride over the host-built tile table.  A tile is <= SGP_LARS_TILE
 // elements of ONE tensor; the CTA reads its x = z * wmul and g^ = grad_scale * (g [+ g2]) exactly
 // as phase 1 of the step kernels does (same fp32 operations), and writes the tile's sum x^2 and
 // sum g^2 in fp64 to lars_partials[tile].  Each thread owns fixed elements of the tile, the warps
 // reduce with a fixed shuffle tree and thread 0 adds the warps in order: no atomics, so the
-// partials -- and the trust ratios -- are bit-identical from run to run and for any grid.
+// partials -- and the trust ratios and the clip coefficient -- are bit-identical from run to run
+// and for any grid.  Without SGP_F_LARS (clipping alone) x is not read and sum x^2 stays 0.
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(SGP_THREADS)
 sgp_lars_norms_kernel(const SgpArgs a)
@@ -1591,6 +1617,7 @@ sgp_lars_norms_kernel(const SgpArgs a)
     const float wmul = (a.flags & SGP_F_IN_NUMER) ? 1.f : w0;    // as phase 1
     const float gscale = a.hyper->grad_scale;
     const bool g_bf16 = (a.flags & SGP_F_GRAD_BF16) != 0;
+    const bool with_x = (a.flags & SGP_F_LARS) != 0;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     static_assert(SGP_LARS_TILE == SGP_THREADS * SGP_VEC * SGP_UNROLL, "one pass per tile");
 
@@ -1606,7 +1633,7 @@ sgp_lars_norms_kernel(const SgpArgs a)
             xv[u] = make_float4(0.f, 0.f, 0.f, 0.f);
             gv[u] = xv[u];
             if (j < tile.count) {
-                xv[u] = __ldg(reinterpret_cast<const float4*>(a.z + i));
+                if (with_x) xv[u] = __ldg(reinterpret_cast<const float4*>(a.z + i));
                 if (g_bf16)
                     gv[u] = bf16x4_to_f4(__ldg(reinterpret_cast<const uint2*>(
                                 reinterpret_cast<const __nv_bfloat16*>(a.g) + i)));
@@ -1653,10 +1680,12 @@ sgp_lars_norms_kernel(const SgpArgs a)
 // sgp_lars_trust_kernel: one warp per tensor.  Lane l adds the tensor's tile partials l, l+32, ...
 // in order and a fixed shuffle tree combines the lanes (deterministic); lane 0 writes the sums to
 // lars_sumsq and the trust ratio
-//     t = eta |x| / (|g^| + wd |x| + eps)   if LARS is on for the tensor and |x| > 0 and |g^| > 0,
-//     t = 1                                 otherwise,
+//     t = eta |x| / (c |g^| + wd |x| + eps)   if LARS is on for the tensor and |x| > 0 and |g^| > 0,
+//     t = 1                                   otherwise,
 // in fp64, rounded once to fp32.  wd is the weight decay of the tensor's group, read from the
-// device rows at every launch (so a change reaches a captured graph).
+// device rows at every launch (so a change reaches a captured graph).  c is the clip coefficient
+// sgp_grad_clip_kernel wrote just before (SGP_F_CLIP; 1 otherwise, exactly): LARS sees the clipped
+// gradient, |c g^| = c |g^|, and lars_sumsq keeps the sums before clipping.
 __global__ void __launch_bounds__(SGP_THREADS)
 sgp_lars_trust_kernel(const SgpArgs a)
 {
@@ -1682,9 +1711,51 @@ sgp_lars_trust_kernel(const SgpArgs a)
             const double nx = sqrt(sx), ng = sqrt(sg);
             const int grp = a.block_group[a.lars_tiles[k0].start / SGP_GROUP_BLOCK];
             const double wd = (double)a.hyper_groups[grp].weight_decay;
-            tr = (float)((double)a.lars_eta * nx / (ng + wd * nx + (double)a.lars_eps));
+            const double c = (a.flags & SGP_F_CLIP) ? (double)a.clip->coef : 1.0;
+            tr = (float)((double)a.lars_eta * nx / (c * ng + wd * nx + (double)a.lars_eps));
         }
         a.lars_trust[t] = tr;
+    }
+}
+
+// sgp_grad_clip_kernel: one CTA.  Thread i adds the sum g^2 of tiles i, i + 256, ... in order, a
+// fixed tree combines the threads, so the total is bit-identical for any norm-kernel grid.  Thread 0
+// then writes the clip state (torch.nn.utils.clip_grad_norm_ with norm type 2, in fp64):
+//     total = sqrt(sum g^2) ; coef = max_grad_norm / (total + 1e-6) clamped at 1 as torch.clamp
+//     does it (a NaN stays NaN) ; skip = skip_nonfinite and total is inf / NaN.
+// A launch that applies no SGD (hyper->do_sgd == 0: the first Overlap-SGP publish, or the one
+// after finish()) leaves the state alone, so `total` stays that of the last SGD launch and
+// nothing is counted.
+__global__ void __launch_bounds__(SGP_THREADS)
+sgp_grad_clip_kernel(const SgpArgs a)
+{
+    __shared__ double s_g[SGP_THREADS];
+    const int tid = threadIdx.x;
+    if (a.hyper->do_sgd == 0.f) return;                // (uniform over the CTA)
+    double sg = 0.0;
+    for (int k = tid; k < a.lars_ntiles; k += SGP_THREADS) sg += a.lars_partials[2 * (long long)k + 1];
+    s_g[tid] = sg;
+    __syncthreads();
+#pragma unroll
+    for (int w = SGP_THREADS / 2; w > 0; w >>= 1) {
+        if (tid < w) s_g[tid] += s_g[tid + w];
+        __syncthreads();
+    }
+    if (tid == 0) {
+        const double sumsq = s_g[0];
+        const double total = sqrt(sumsq);
+        float coef = 1.f;
+        if (a.clip_norm) {
+            const double c = (double)a.hyper->_pad[0] / (total + 1e-6);
+            coef = (c > 1.0) ? 1.f : (float)c;         // NaN > 1 is false: the NaN is kept
+        }
+        const bool skip = a.clip_skip && !isfinite(total);
+        SgpClipState* cs = a.clip;
+        cs->sumsq = sumsq;
+        cs->total = (float)total;
+        cs->coef = coef;
+        cs->skip = skip ? 1u : 0u;
+        if (skip) cs->skipped += 1u;
     }
 }
 
@@ -1790,21 +1861,34 @@ static bool groups_ok(const SgpArgs* args)
     return args->hyper_groups && args->block_group && args->groups >= 1 && args->groups <= SGP_MAX_GROUPS;
 }
 
+// the norm plan shared by LARS and clipping: tile table and partials
+static bool norm_plan_ok(const SgpArgs* args)
+{
+    return args->lars_tiles && args->lars_tile_first && args->lars_partials && args->lars_tensors >= 1 &&
+           args->lars_tensors <= SGP_LARS_MAX_TENSORS && args->lars_ntiles >= args->lars_tensors;
+}
+
 // SGP_F_LARS needs SGP_F_GROUPS (the rows give each tensor's weight decay) and every LARS buffer
 static bool lars_ok(const SgpArgs* args)
 {
     if (!(args->flags & SGP_F_LARS)) return true;
-    return (args->flags & SGP_F_GROUPS) && groups_ok(args) && args->block_tensor && args->lars_trust &&
-           args->lars_enabled && args->lars_tiles && args->lars_tile_first && args->lars_partials &&
-           args->lars_sumsq && args->lars_tensors >= 1 && args->lars_tensors <= SGP_LARS_MAX_TENSORS &&
-           args->lars_ntiles >= args->lars_tensors;
+    return (args->flags & SGP_F_GROUPS) && groups_ok(args) && norm_plan_ok(args) && args->block_tensor &&
+           args->lars_trust && args->lars_enabled && args->lars_sumsq;
+}
+
+// SGP_F_CLIP needs the norm plan and the clip state
+static bool clip_ok(const SgpArgs* args)
+{
+    if (!(args->flags & SGP_F_CLIP)) return true;
+    return norm_plan_ok(args) && args->clip;
 }
 
 extern "C" {
 
 cudaError_t sgp_launch_step(const SgpArgs* args, int grid, cudaStream_t stream)
 {
-    if (!msg_bf16_mode_ok(args->flags) || !groups_ok(args) || !lars_ok(args)) return cudaErrorInvalidValue;
+    if (!msg_bf16_mode_ok(args->flags) || !groups_ok(args) || !lars_ok(args) || !clip_ok(args))
+        return cudaErrorInvalidValue;
     return with_step_variant(args->flags, [&](auto v) {
         v.step<<<grid, SGP_THREADS, 0, stream>>>(*args);
         return cudaGetLastError();
@@ -1813,7 +1897,8 @@ cudaError_t sgp_launch_step(const SgpArgs* args, int grid, cudaStream_t stream)
 
 cudaError_t sgp_launch_step_pipe(const SgpArgs* args, int grid, cudaStream_t stream)
 {
-    if (!msg_bf16_mode_ok(args->flags) || !groups_ok(args) || !lars_ok(args)) return cudaErrorInvalidValue;
+    if (!msg_bf16_mode_ok(args->flags) || !groups_ok(args) || !lars_ok(args) || !clip_ok(args))
+        return cudaErrorInvalidValue;
     return with_step_variant(args->flags, [&](auto v) {
         const cudaError_t e = ensure_dynamic_smem<v.pipe>(PIPE_SMEM, true);
         if (e != cudaSuccess) return e;
@@ -1825,20 +1910,28 @@ cudaError_t sgp_launch_step_pipe(const SgpArgs* args, int grid, cudaStream_t str
 int sgp_max_resident_ctas_pipe(int device) { return step_resident_ctas(device, true); }
 int sgp_max_resident_ctas(int device) { return step_resident_ctas(device, false); }
 
-// the two LARS kernels (see sgp_lars_norms_kernel): any grid >= 1 gives the same bits
+// the norm-plan kernels (see sgp_lars_norms_kernel): any grid >= 1 gives the same bits
 cudaError_t sgp_launch_lars_norms(const SgpArgs* args, int grid, cudaStream_t stream)
 {
-    if (!lars_ok(args) || !(args->flags & SGP_F_LARS) || grid < 1) return cudaErrorInvalidValue;
+    if (!lars_ok(args) || !clip_ok(args) || !(args->flags & (SGP_F_LARS | SGP_F_CLIP)) || grid < 1)
+        return cudaErrorInvalidValue;
     sgp_lars_norms_kernel<<<grid, SGP_THREADS, 0, stream>>>(*args);
     return cudaGetLastError();
 }
 
 cudaError_t sgp_launch_lars_trust(const SgpArgs* args, cudaStream_t stream)
 {
-    if (!lars_ok(args) || !(args->flags & SGP_F_LARS)) return cudaErrorInvalidValue;
+    if (!lars_ok(args) || !clip_ok(args) || !(args->flags & SGP_F_LARS)) return cudaErrorInvalidValue;
     const int warps_per_cta = SGP_THREADS / 32;
     const int grid = (args->lars_tensors + warps_per_cta - 1) / warps_per_cta;
     sgp_lars_trust_kernel<<<grid, SGP_THREADS, 0, stream>>>(*args);
+    return cudaGetLastError();
+}
+
+cudaError_t sgp_launch_grad_clip(const SgpArgs* args, cudaStream_t stream)
+{
+    if (!clip_ok(args) || !(args->flags & SGP_F_CLIP)) return cudaErrorInvalidValue;
+    sgp_grad_clip_kernel<<<1, SGP_THREADS, 0, stream>>>(*args);
     return cudaGetLastError();
 }
 
@@ -1983,7 +2076,7 @@ cudaError_t sgp_preload_kernels()
     for_each_step_variant([&](auto v) { load((const void*)v.step); load((const void*)v.pipe); });
     const void* kernels[] = {
         (const void*)sgp_gather_kernel, (const void*)sgp_gather_tma_kernel,
-        (const void*)sgp_lars_norms_kernel, (const void*)sgp_lars_trust_kernel,
+        (const void*)sgp_lars_norms_kernel, (const void*)sgp_lars_trust_kernel, (const void*)sgp_grad_clip_kernel,
         (const void*)sgp_probe_kernel, (const void*)sgp_gather_wait_kernel,
         (const void*)sgp_gather_ack_kernel, (const void*)sgp_bilat_decide_kernel, (const void*)sgp_bilat_ctl_kernel,
         (const void*)sgp_allreduce_sgd_kernel, (const void*)sgp_zero_kernel, (const void*)sgp_barrier_kernel,

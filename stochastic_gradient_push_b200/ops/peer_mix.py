@@ -158,13 +158,15 @@ class GossipEngine(object):
         world.barrier()
 
     # -- configuration ------------------------------------------------------ #
-    def set_hyper(self, lr, momentum, weight_decay, nesterov, do_sgd=True, grad_scale=1.0, groups=None):
+    def set_hyper(self, lr, momentum, weight_decay, nesterov, do_sgd=True, grad_scale=1.0, groups=None,
+                  max_grad_norm=None):
         """Stage the SGD hyper-parameters for the next launches (device resident: a captured graph
         reads the new values).  ``groups``: with :meth:`set_param_groups`, one
         ``(lr, momentum, weight_decay, nesterov)`` per parameter group; ``do_sgd`` and
-        ``grad_scale`` apply to every group."""
+        ``grad_scale`` apply to every group.  ``max_grad_norm``: the clipping threshold of
+        :meth:`set_grad_clip` (ignored while clipping is off)."""
         key = (float(lr), float(momentum), float(weight_decay), bool(nesterov),
-               bool(do_sgd), float(grad_scale))
+               bool(do_sgd), float(grad_scale), 0.0 if max_grad_norm is None else float(max_grad_norm))
         if groups is not None:
             if len(groups) != self.groups:
                 raise ValueError('set_hyper got %d group rows, set_param_groups configured %d'
@@ -183,11 +185,12 @@ class GossipEngine(object):
         h[3] = 1.0 if key[3] else 0.0
         h[4] = 1.0 if key[4] else 0.0
         h[5] = key[5]
+        h[6] = key[6]
         if groups is None:
             self.hyper.copy_(h, non_blocking=True)
         else:
             rows = self._hyper_host[slot][:1 + len(groups)]
-            for r, (g_lr, g_mu, g_wd, g_nest) in zip(rows[1:], key[6:]):
+            for r, (g_lr, g_mu, g_wd, g_nest) in zip(rows[1:], key[7:]):
                 r[0], r[1], r[2], r[3] = g_lr, g_mu, g_wd, 1.0 if g_nest else 0.0
             self._hyper_rows[:1 + len(groups)].copy_(rows, non_blocking=True)
         ev = self._hyper_events[slot] = torch.cuda.Event()
@@ -233,6 +236,75 @@ class GossipEngine(object):
     def lars_sumsq(self) -> Optional[torch.Tensor]:
         """fp64 [tensors, 2]: sum x^2 and sum g^2 per tensor as the last SGD launch saw them"""
         return self.ctx.lars_sumsq() if self.ctx.lars() else None
+
+    def set_grad_clip(self, offsets=None, numels=None, enabled=True, skip_nonfinite=False):
+        """Gradient-norm clipping and non-finite step skipping on every SGD launch.  The arena holds
+        tensors at ``offsets`` (64-element aligned, ascending) of ``numels`` elements -- the layout
+        :meth:`set_lars` takes; both share one norm plan.  Each SGD launch then first computes, in
+        fp64, ``total = |g^|_2`` over those tensors with ``g^ = grad_scale * (g [+ g2])``:
+
+        * ``enabled``: phase 1 applies ``coef * g^`` with ``coef = min(max_grad_norm / (total + 1e-6),
+          1)`` (``torch.nn.utils.clip_grad_norm_``; a NaN total gives a NaN coef), ``max_grad_norm``
+          staged by :meth:`set_hyper`;
+        * ``skip_nonfinite``: a launch whose total is inf or NaN leaves x and the momentum alone (the
+          gradient is still cleared, the publish and mix run as usual) and counts in
+          :attr:`nonfinite_steps`.
+
+        ``offsets=None`` turns both off.  Turning them on or off changes the launch sequence: a
+        captured CUDA graph has to be captured again.  The skip count survives reconfiguration."""
+        if offsets is None or not (enabled or skip_nonfinite):
+            self.ctx.set_grad_clip(None, None, None, False, False)
+            return
+        as_t = lambda v: torch.as_tensor(v, dtype=torch.int64, device='cpu')
+        self.ctx.set_grad_clip(as_t(offsets), as_t(numels), self._ensure_clip_state(), bool(enabled),
+                               bool(skip_nonfinite))
+
+    def _ensure_clip_state(self):
+        if getattr(self, '_clip_state', None) is None:
+            C = self.C
+            self._clip_state = torch.zeros(C.CLIP_STATE_BYTES // 4, dtype=torch.float32, device=self.device)
+            self._clip_state[C.CLIP_OFF_COEF // 4] = 1.0
+        return self._clip_state
+
+    @property
+    def grad_clip(self) -> bool:
+        return self.ctx.grad_clip()
+
+    def _clip_word(self, off, dtype=torch.float32):
+        if not self.ctx.grad_clip():
+            return None
+        return self._clip_state.view(dtype)[off // dtype.itemsize]
+
+    @property
+    def grad_norm(self) -> Optional[torch.Tensor]:
+        """0-dim fp32 device tensor: the gradient norm (before clipping) of the last SGD launch,
+        rewritten by the next one; None while clipping and skipping are off.  No synchronisation"""
+        return self._clip_word(self.C.CLIP_OFF_TOTAL)
+
+    @property
+    def clip_coef(self) -> Optional[torch.Tensor]:
+        """0-dim fp32 device tensor: the clip coefficient of the last SGD launch (1 when not clipped)"""
+        return self._clip_word(self.C.CLIP_OFF_COEF)
+
+    @property
+    def grad_sumsq(self) -> Optional[torch.Tensor]:
+        """0-dim fp64 device tensor: sum of g^2 of the last SGD launch"""
+        return self._clip_word(self.C.CLIP_OFF_SUMSQ, torch.float64)
+
+    @property
+    def nonfinite_steps(self) -> int:
+        """SGD launches skipped for a non-finite gradient norm so far (synchronises)"""
+        if getattr(self, '_clip_state', None) is None:
+            return 0
+        return int(self._clip_state.view(torch.int32)[self.C.CLIP_OFF_SKIPPED // 4].item())
+
+    @nonfinite_steps.setter
+    def nonfinite_steps(self, v: int):
+        self._ensure_clip_state().view(torch.int32)[self.C.CLIP_OFF_SKIPPED // 4] = int(v)
+
+    def clip_update(self):
+        """the norm and clip kernels alone, as the next SGD launch would run them (tests, benchmarks)"""
+        self.ctx.clip_update()
 
     def set_schedule(self, graph=None, mixing=None):
         """Re-emit the device tables (e.g. after ``peers_per_itr`` changed).

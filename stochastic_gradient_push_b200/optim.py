@@ -34,6 +34,12 @@ such a group takes
 
 with x the push-sum numerator the step acts on.  The kernels compute the norms and t on the device
 before every SGD launch (DESIGN.md 2.0.4); :func:`lars_groups` is the MLPerf ResNet-50 recipe.
+
+``max_grad_norm`` clips the gradient the update consumes, g^ = grad_scale * g, as
+``torch.nn.utils.clip_grad_norm_(params, max_grad_norm)`` would (norm type 2, over every parameter
+of every group, in fp64); LARS then sees the clipped gradient.  ``skip_nonfinite=True`` skips the
+SGD of a step whose gradient norm is inf or NaN: x and the momentum keep their bits, the gradient is
+still cleared, and the rank keeps gossiping (DESIGN.md 2.0.6).
 """
 
 from __future__ import annotations
@@ -69,13 +75,30 @@ def lars_groups(module, weight_decay):
 class FusedGossipSGD(object):
 
     def __init__(self, model, lr=0.1, momentum=0.0, weight_decay=0.0, nesterov=False,
-                 grad_scale=1.0, param_groups=None, lars=False, trust_coefficient=0.001, lars_eps=1e-8):
+                 grad_scale=1.0, param_groups=None, lars=False, trust_coefficient=0.001, lars_eps=1e-8,
+                 max_grad_norm=None, skip_nonfinite=False):
+        """``max_grad_norm``: a float > 0 clips the gradient of every step to that global 2-norm
+        (``torch.nn.utils.clip_grad_norm_`` semantics); None: off.  ``skip_nonfinite``: a step whose
+        gradient norm is inf or NaN leaves the parameters and the momentum unchanged, clears the
+        gradient and counts in :attr:`nonfinite_steps`; without it such a norm propagates into the
+        update as in torch (a NaN coefficient, or 0 for an infinite norm).
+
+        Both act per rank, on the gradient the update consumes: gossip has no global gradient, and
+        in hierarchical mode (``nprocs_per_node > 1``) the backward hook has already averaged it over
+        the node, so every rank of a node clips the same node gradient.  BatchNorm running statistics
+        are not protected: a NaN that the forward pass produces reaches them before any check.
+
+        Turning either option on or off changes the kernel launches of a step, so a captured CUDA
+        graph (GossipTrainer) has to be captured again; ``max_grad_norm`` itself lives in device
+        memory, and a new value reaches a captured graph."""
         from .parallel.distributed import GossipDataParallel
         assert isinstance(model, GossipDataParallel)
         if nesterov and momentum <= 0:
             raise ValueError('Nesterov momentum requires a momentum')
         if not trust_coefficient > 0 or not lars_eps >= 0:
             raise ValueError('LARS needs trust_coefficient > 0 and lars_eps >= 0')
+        self._max_grad_norm = self._check_max_grad_norm(max_grad_norm)
+        self.skip_nonfinite = bool(skip_nonfinite)
         self.model = model
         self.defaults = dict(lr=lr, momentum=momentum, weight_decay=weight_decay,
                              nesterov=nesterov, dampening=0, lars=bool(lars))
@@ -122,6 +145,8 @@ class FusedGossipSGD(object):
         self._steps = 0
         if self._grouped:
             self._setup_groups()
+        self._clip_flags = None
+        self._setup_clip()
 
     @staticmethod
     def _partition(model, param_groups, defaults):
@@ -235,6 +260,102 @@ class FusedGossipSGD(object):
                         torch.ones_like(nx))
         return torch.cat([t, t.new_ones(1)]).to(x.dtype)[idx]
 
+    @staticmethod
+    def _check_max_grad_norm(v):
+        if v is None:
+            return None
+        try:
+            v = float(v)
+        except (TypeError, ValueError):
+            raise ValueError('max_grad_norm must be a finite number > 0 or None, got %r' % (v,))
+        if not (v > 0 and v != float('inf')):
+            raise ValueError('max_grad_norm must be a finite number > 0 or None, got %r' % (v,))
+        return v
+
+    @property
+    def max_grad_norm(self):
+        """the clipping threshold (None: off).  A new value reaches the next step, a captured CUDA graph
+        included; switching between None and a number re-plans the launches (re-capture needed)"""
+        return self._max_grad_norm
+
+    @max_grad_norm.setter
+    def max_grad_norm(self, v):
+        self._max_grad_norm = self._check_max_grad_norm(v)
+        if self._clip_flags is not None and (self._max_grad_norm is not None, self.skip_nonfinite) != self._clip_flags:
+            self._setup_clip()
+
+    def _clip_on(self):
+        return self.max_grad_norm is not None or self.skip_nonfinite
+
+    def _setup_clip(self):
+        """hand the fp32 arena's layout to the engine (kernel plane; it shares the LARS norm plan),
+        or mark each arena's tensor elements, padding excluded (c10d plane)"""
+        m = self.model
+        self._clip_flags = (self.max_grad_norm is not None, self.skip_nonfinite)
+        self._elem_valid = {}
+        if not hasattr(self, '_nonfinite'):
+            dev = self._arenas[next(iter(self._arenas))].device
+            self._nonfinite = torch.zeros((), dtype=torch.int64, device=dev)     # c10d plane
+            self._grad_norm = torch.zeros((), dtype=torch.float32, device=dev)
+        k = m._kernel
+        if k is not None:
+            if not self._clip_on():
+                k.engine.set_grad_clip(None)
+                return
+            arena = self._arenas[torch.float32]
+            k.engine.set_grad_clip(arena.offsets, arena.numels, enabled=self.max_grad_norm is not None,
+                                   skip_nonfinite=self.skip_nonfinite)
+            return
+        if self._clip_on():
+            for dtype, arena in self._arenas.items():
+                valid = torch.zeros(arena.total, dtype=torch.bool)
+                for off, n in zip(arena.offsets, arena.numels):
+                    valid[off:off + n] = True
+                self._elem_valid[dtype] = valid.to(arena.device)
+
+    def _c10d_clip(self, grads):
+        """(coef or None, skip) of the c10d plane: the fp64 2-norm of every arena's scaled gradient,
+        coef = max_grad_norm / (total + 1e-6) clamped at 1 (torch.clamp keeps a NaN), and whether
+        skip_nonfinite skips this step (a 0-dim bool tensor, so no synchronisation)"""
+        sumsq = None
+        for dtype, g in grads.items():
+            s = g.double()[self._elem_valid[dtype].to(g.device)].square().sum()
+            sumsq = s if sumsq is None else sumsq + s.to(sumsq.device)
+        total = sumsq.sqrt()
+        self._grad_norm.copy_(total)
+        coef = None
+        if self.max_grad_norm is not None:
+            coef = torch.clamp(self.max_grad_norm / (total + 1e-6), max=1.0).float()
+        skip = None
+        if self.skip_nonfinite:
+            skip = ~torch.isfinite(total)
+            self._nonfinite += skip.to(self._nonfinite.device)
+        return coef, skip
+
+    @property
+    def grad_norm(self):
+        """0-dim fp32 device tensor: the gradient norm before clipping of the last SGD step, rewritten
+        by the next (None while clipping and skipping are off).  Reading it does not synchronise."""
+        if not self._clip_on():
+            return None
+        k = self.model._kernel
+        return k.engine.grad_norm if k is not None else self._grad_norm
+
+    @property
+    def nonfinite_steps(self) -> int:
+        """steps skipped for a non-finite gradient norm so far (synchronises)"""
+        k = self.model._kernel
+        if k is not None:
+            return k.engine.nonfinite_steps
+        return int(self._nonfinite.item())
+
+    def _set_nonfinite_steps(self, n):
+        k = self.model._kernel
+        if k is not None:
+            k.engine.nonfinite_steps = n
+        else:
+            self._nonfinite.fill_(int(n))
+
     # -- torch.optim-like surface -------------------------------------------- #
     def _hyper(self):
         g = self.param_groups[0]
@@ -251,7 +372,8 @@ class FusedGossipSGD(object):
         this before each replay, so per-group lr changes reach a captured graph)"""
         lr, mu, wd, nest = self._hyper()
         engine.set_hyper(lr, mu, wd, nest, do_sgd=do_sgd, grad_scale=self.grad_scale,
-                         groups=self._group_rows() if self._grouped else None)
+                         groups=self._group_rows() if self._grouped else None,
+                         max_grad_norm=self.max_grad_norm)
 
     def _c10d_vectors(self, dtype, rows):
         """per-element (lr, momentum, weight_decay, nesterov) of one arena, rebuilt only when a
@@ -280,16 +402,23 @@ class FusedGossipSGD(object):
             m = self.model
             m.ps_numerator()                       # step the numerator (reference :564)
             rows = self._group_rows() if self._grouped else None
-            for dtype, arena in self._arenas.items():
+            grads = {}
+            for dtype in self._arenas:
                 g = self.grad_flat[dtype]
-                if self.grad_scale != 1.0:
-                    g = g * self.grad_scale
+                grads[dtype] = g * self.grad_scale if self.grad_scale != 1.0 else g
+            coef, skip = self._c10d_clip(grads) if self._clip_on() else (None, None)
+            for dtype, arena in self._arenas.items():
+                g = grads[dtype] if coef is None else grads[dtype] * coef.to(grads[dtype].device)
                 if rows is not None:
                     lr, mu, wd, nest = self._c10d_vectors(dtype, rows)
                 trust = self._c10d_trust(dtype, arena.flat, g) if self._lars_flags and any(self._lars_flags) \
                     else None
                 x, mom = oracle.sgd_momentum(arena.flat, g, self.momentum_flat[dtype],
                                              lr, mu, wd, nest, trust=trust)
+                if skip is not None:              # a skipped step keeps the numerator and momentum bits
+                    keep = skip.to(x.device)
+                    x = torch.where(keep, arena.flat, x)
+                    mom = torch.where(keep, self.momentum_flat[dtype], mom)
                 arena.flat.copy_(x)
                 self.momentum_flat[dtype].copy_(mom)
         self._steps += 1
@@ -311,6 +440,8 @@ class FusedGossipSGD(object):
         groups = [{k: v for k, v in g.items() if k != 'params'} for g in self.param_groups]
         return {'param_groups': groups, 'steps': self._steps,
                 'lars': {'trust_coefficient': self.trust_coefficient, 'eps': self.lars_eps},
+                'grad_clip': {'max_grad_norm': self.max_grad_norm, 'skip_nonfinite': self.skip_nonfinite,
+                              'nonfinite_steps': self.nonfinite_steps},
                 'momentum': {str(dt): m.detach().cpu().clone()
                              for dt, m in self.momentum_flat.items()}}
 
@@ -319,7 +450,8 @@ class FusedGossipSGD(object):
         loads into a grouped one: its lr (the schedule's state) goes to every group, and each group
         keeps its own momentum, weight decay and nesterov.  The groups' ``lars`` flags, the trust
         coefficient and eps are restored too; if they change, the LARS maps are rebuilt (a CUDA graph
-        captured before then has to be captured again)."""
+        captured before then has to be captured again).  So are ``max_grad_norm``, ``skip_nonfinite``
+        and the count of skipped steps; a checkpoint without them keeps the constructor's values."""
         saved = sd['param_groups']
         before = (tuple(bool(g['lars']) for g in self.param_groups), self.trust_coefficient, self.lars_eps)
         if 'lars' in sd:
@@ -342,6 +474,13 @@ class FusedGossipSGD(object):
             else:
                 self._grouped = True
                 self._setup_groups()
+        clip = sd.get('grad_clip')
+        if clip is not None:
+            self._max_grad_norm = self._check_max_grad_norm(clip['max_grad_norm'])
+            self.skip_nonfinite = bool(clip['skip_nonfinite'])
+            if (self._max_grad_norm is not None, self.skip_nonfinite) != self._clip_flags:
+                self._setup_clip()
+            self._set_nonfinite_steps(int(clip.get('nonfinite_steps', 0)))
         self._steps = sd.get('steps', 0)
         for dt, m in self.momentum_flat.items():
             m.copy_(sd['momentum'][str(dt)])

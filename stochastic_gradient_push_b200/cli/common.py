@@ -366,6 +366,29 @@ def check_grad_clip_flags(args, adpsgd=False):
                              'D-PSGD' % (flag, unsupported))
 
 
+def check_accumulation_flags(args):
+    """ValueError for --accumulation_steps < 1, for K > 1 outside the captured fused gossip step
+    (GossipTrainer), and for a --batch_size that K does not divide."""
+    k = args.accumulation_steps
+    if k < 1:
+        raise ValueError('--accumulation_steps must be >= 1, got %r' % (k,))
+    if k == 1:
+        return
+    unsupported = ('--all_reduce' if args.all_reduce else
+                   '--fused False' if not args.fused else
+                   '--cuda_graph False' if not args.cuda_graph else
+                   '--transport c10d' if args.transport == 'c10d' else
+                   '--device cpu' if args.device == 'cpu' else
+                   '--nprocs_per_node > 1' if args.nprocs_per_node > 1 else None)
+    if unsupported:
+        raise ValueError('--accumulation_steps > 1 is not supported with %s: gradient accumulation is '
+                         'implemented in the captured fused gossip step (--cuda_graph True --fused True) for '
+                         'SGP, OSGP and D-PSGD' % unsupported)
+    if args.batch_size % k:
+        raise ValueError('--batch_size %d is not divisible by --accumulation_steps %d'
+                         % (args.batch_size, k))
+
+
 def check_ema_flags(args, adpsgd=False):
     """ValueError for --model_ema_decay out of [0, 1) or with AD-PSGD."""
     d = getattr(args, 'model_ema_decay', 0.0)

@@ -42,7 +42,14 @@ def parse_args(argv=None):
     parser = build_parser(adpsgd=False)
     parser.add_argument('--cuda_graph', default=False, type=common.str2bool, nargs='?', const=True,
                         help='capture forward+backward+gossip once and replay (fused path only)')
+    parser.add_argument('--accumulation_steps', default=1, type=int,
+                        help='gradient accumulation: K forward/backward passes of batch_size / K rows each per '
+                             'step, their gradients summed in fp32 before the one gossip / SGD step '
+                             '(GossipTrainer(accumulation_steps=K)); --batch_size stays the per-rank step batch '
+                             'and must be divisible by K.  BatchNorm statistics are per micro-batch.  SGP / OSGP '
+                             '/ D-PSGD with --cuda_graph True --fused True and --nprocs_per_node 1')
     args = parser.parse_args(argv)
+    common.check_accumulation_flags(args)
     return finalize_args(args, adpsgd=False)
 
 
@@ -146,7 +153,11 @@ def main(argv=None):
         args._trainer = GossipTrainer(model, optimizer,
                                       FusedCrossEntropyWithAccuracy(label_smoothing=args.label_smoothing),
                                       amp_dtype=torch.bfloat16 if args.amp else None,
-                                      batch_mix=args._batch_mix, ema=args._ema)
+                                      batch_mix=args._batch_mix, ema=args._ema,
+                                      accumulation_steps=args.accumulation_steps)
+    if args.accumulation_steps > 1 and args._trainer is None:
+        raise ValueError('--accumulation_steps > 1 needs the captured GossipTrainer step, which runs on the '
+                         'CUDA kernel transport only (got device %s, transport %s)' % (args.device, model.transport))
 
     state = fresh_state(model.state_dict(), optimizer.state_dict())
     if args._ema is not None:
@@ -361,6 +372,10 @@ def train(args, model, criterion, optimizer, batch_meter, data_meter, nn_meter, 
             top1.update(a1, n)
             top5.update(a5, n)
     csv.train_row(epoch, i, batch_meter, nn_meter, data_meter, losses, top1, top5)
+    k = getattr(args, 'accumulation_steps', 1)
+    if k > 1:
+        log.info('epoch {} gradient accumulation: {} micro-batches of {} rows per step of {} rows'.format(
+            epoch, k, args.batch_size // k, args.batch_size))
     grad_norm = getattr(optimizer, 'grad_norm', None)       # (--clip_grad_norm / --skip_nonfinite)
     if grad_norm is not None:
         log.info('epoch {} last gradient norm {:.6e} non-finite steps skipped {}'.format(

@@ -214,13 +214,23 @@ class BatchMix(object):
         return self.state
 
     # -- mixing ------------------------------------------------------------------------------- #
-    def apply(self, src: torch.Tensor, out: torch.Tensor = None, params: MixParams = None) -> torch.Tensor:
+    def apply(self, src: torch.Tensor, out: torch.Tensor = None, params: MixParams = None,
+              micro_batches: int = 1) -> torch.Tensor:
         """``out`` <- ``src`` mixed with its flipped batch.  ``params`` default: the next draw
         (:meth:`sample`).  CUDA: one launch of the sm_90a kernel (``src`` fp32, NCHW or NHWC;
         ``out`` NCHW or NHWC, fp32 or bf16; a missing extension is an error).  CPU: the plain torch
-        composition :func:`reference_batch_mix`."""
+        composition :func:`reference_batch_mix`.
+
+        ``micro_batches = k > 1`` (gradient accumulation): the batch is k equal row slices, each mixed
+        with its own flipped slice -- row i of slice j pairs with row m-1-i of that slice, as the fused
+        two-target loss of that micro-batch pairs them --, under ONE draw staged once: k launches that
+        move the same bytes as one."""
         if src.dim() != 4:
             raise ValueError('BatchMix.apply takes a 4-d image batch, got shape %s' % (tuple(src.shape),))
+        k = int(micro_batches)
+        if k < 1 or src.shape[0] % k:
+            raise ValueError('micro_batches must be >= 1 and divide the batch of %d rows, got %r'
+                             % (src.shape[0], micro_batches))
         if params is None:
             params = self.sample(src.shape[2], src.shape[3])
         if out is None:
@@ -228,9 +238,12 @@ class BatchMix(object):
                                           and not src.is_contiguous()) else torch.contiguous_format
             out = torch.empty(src.shape, dtype=torch.float32, device=src.device).contiguous(memory_format=fmt)
         state = self.stage(params, src.device)
-        if src.is_cuda:
-            native.load().batch_mix(src, out, state)
-        else:
-            out.copy_(reference_batch_mix(src, params))
+        m = src.shape[0] // k
+        for j in range(k):
+            s, o = (src, out) if k == 1 else (src[j * m:(j + 1) * m], out[j * m:(j + 1) * m])
+            if src.is_cuda:
+                native.load().batch_mix(s, o, state)
+            else:
+                o.copy_(reference_batch_mix(s, params))
         self.last = params
         return out

@@ -959,6 +959,60 @@ static void ema_update(torch::Tensor ema, torch::Tensor segs, torch::Tensor item
                                          at::cuda::getCurrentCUDAStream()));
 }
 
+// ---------------------------------------------------------------------------
+// gradient accumulation (csrc/accum_kernels.cu, parallel/trainer.py)
+// ---------------------------------------------------------------------------
+extern "C" {
+int sgp_accum_chunk();
+int sgp_accum_max_segs();
+cudaError_t sgp_launch_grad_accumulate(const long long* rows, int nseg, int num_sms, cudaStream_t stream);
+}
+
+// dst[i] += float(src[i]) for every pair: dst fp32, src fp32 or bf16, both non-overlapping and dense with
+// identical shapes and strides, size-1 dims aside (the kernel walks both in memory order).  One launch per ACCUM_MAX_SEGS pairs with
+// elements, on the current stream; an empty list launches nothing.
+static void grad_accumulate(const std::vector<torch::Tensor>& dst, const std::vector<torch::Tensor>& src)
+{
+    // (std::runtime_error with a std::string message: a TORCH_CHECK with formatted arguments thrown from
+    // here ended the process instead of raising)
+    auto fail = [](size_t i, const char* what) {
+        throw std::runtime_error("grad_accumulate: pair " + std::to_string(i) + ": " + what);
+    };
+    if (dst.size() != src.size())
+        throw std::runtime_error("grad_accumulate: " + std::to_string(dst.size()) + " dst tensors but " +
+                                 std::to_string(src.size()) + " src tensors");
+    if (dst.empty()) return;
+    const auto device = dst[0].device();
+    std::vector<long long> rows;
+    rows.reserve(4 * dst.size());
+    for (size_t i = 0; i < dst.size(); ++i) {
+        const torch::Tensor& d = dst[i];
+        const torch::Tensor& s = src[i];
+        if (!(d.is_cuda() && s.is_cuda() && d.device() == device && s.device() == device))
+            fail(i, "every tensor must be a CUDA tensor on the first dst's device");
+        if (d.scalar_type() != torch::kFloat32) fail(i, "dst must be fp32");
+        if (s.scalar_type() != torch::kFloat32 && s.scalar_type() != torch::kBFloat16)
+            fail(i, "src must be fp32 or bf16");
+        if (d.numel() != s.numel()) fail(i, "dst and src must have the same numel");
+        bool same = d.dim() == s.dim() && d.sizes() == s.sizes();
+        for (int64_t k = 0; same && k < d.dim(); ++k)      // (a size-1 dim's stride addresses nothing)
+            same = d.size(k) == 1 || d.stride(k) == s.stride(k);
+        if (!(d.is_non_overlapping_and_dense() && s.is_non_overlapping_and_dense() && same))
+            fail(i, "dst and src must be non-overlapping and dense with identical shapes and strides");
+        const auto d0 = reinterpret_cast<uintptr_t>(d.data_ptr()), s0 = reinterpret_cast<uintptr_t>(s.data_ptr());
+        if (d.numel() == 0) continue;
+        if (!(d0 + d.nbytes() <= s0 || s0 + s.nbytes() <= d0)) fail(i, "dst and src must not overlap");
+        rows.insert(rows.end(), {(long long)d0, (long long)s0, (long long)d.numel(),
+                                 s.scalar_type() == torch::kBFloat16 ? 1LL : 0LL});
+    }
+    c10::cuda::CUDAGuard guard(device);
+    const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
+    const auto stream = at::cuda::getCurrentCUDAStream();
+    const long long nseg = (long long)rows.size() / 4, per = sgp_accum_max_segs();
+    for (long long b = 0; b < nseg; b += per)
+        SGP_CUDA_CHECK(sgp_launch_grad_accumulate(rows.data() + 4 * b, (int)std::min(per, nseg - b), sms, stream));
+}
+
 void bind_bn(py::module& mod);   // bn_bindings.cpp
 void bind_vmm(py::module& mod);  // vmm_symm.cpp
 void bind_data(py::module& mod); // data_loader.cpp
@@ -988,6 +1042,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, mod)
     mod.def("ema_update", &ema_update, py::arg("ema"), py::arg("segs"), py::arg("items"), py::arg("state"),
             "e <- fmaf(1 - d_t, s - e, e) over every segment in one launch; advances the device counter");
     mod.attr("EMA_CHUNK") = sgp_ema_chunk();
+    mod.def("grad_accumulate", &grad_accumulate, py::arg("dst"), py::arg("src"),
+            "dst[i] += float(src[i]) over every (fp32 dst, fp32 / bf16 src) pair: one launch per ACCUM_MAX_SEGS "
+            "pairs, none for an empty list");
+    mod.attr("ACCUM_CHUNK") = sgp_accum_chunk();
+    mod.attr("ACCUM_MAX_SEGS") = sgp_accum_max_segs();
 
     mod.attr("CHUNK") = (int)SGP_CHUNK;
     mod.attr("MAX_PEERS") = (int)SGP_MAX_PEERS;

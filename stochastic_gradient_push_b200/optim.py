@@ -367,11 +367,15 @@ class FusedGossipSGD(object):
                 raise ValueError('Nesterov momentum requires a momentum')
         return [tuple(g[k] for k in _HYPER_KEYS) for g in self.param_groups]
 
-    def set_engine_hyper(self, engine, do_sgd=True):
+    def set_engine_hyper(self, engine, do_sgd=True, micro_batches=1):
         """Stage every group's current values into the engine's device table (GossipTrainer calls
-        this before each replay, so per-group lr changes reach a captured graph)"""
+        this before each replay, so per-group lr changes reach a captured graph).  ``micro_batches``:
+        the gradient is the sum of that many micro-batch gradients (gradient accumulation), so the
+        kernel scales it by ``fp32(grad_scale / micro_batches)`` (divided in fp64, rounded once);
+        :attr:`grad_scale` itself does not change."""
         lr, mu, wd, nest = self._hyper()
-        engine.set_hyper(lr, mu, wd, nest, do_sgd=do_sgd, grad_scale=self.grad_scale,
+        grad_scale = self.grad_scale if micro_batches == 1 else self.grad_scale / micro_batches
+        engine.set_hyper(lr, mu, wd, nest, do_sgd=do_sgd, grad_scale=grad_scale,
                          groups=self._group_rows() if self._grouped else None,
                          max_grad_norm=self.max_grad_norm)
 

@@ -30,11 +30,24 @@ Overlap-SGP after ``publish`` and the join with the gossip stream.  The EMA ther
 parameters exactly as the next forward pass sees them: under Overlap-SGP the residual gathered during
 step k is folded in at the next publish, so it reaches the EMA one step later, and a SlowMo step
 (enqueued after the replay) reaches it at the next step.
+
+Gradient accumulation (``accumulation_steps=k``): ``step()`` still takes the whole step batch of B
+rows (one H2D copy); the step runs k forward/backward passes on the row slices
+``static_in[j m:(j+1) m]``, m = B / k, then ONE gossip / SGD launch and one EMA update.  Micro-batch 0
+writes its gradients into the arena as a k = 1 step does; each later one adds its fresh gradients with
+one ``grad_accumulate`` launch (fp32 sums; with the bf16 twin into the fp32 ``g2`` buffer, which the
+step kernel adds to the bf16 one).  The kernel scales the sum by ``fp32(grad_scale / k)``: the gradient
+of the mean loss over the B rows, with BatchNorm statistics taken per micro-batch as in torch.  So
+BatchNorm running statistics are updated k times per step (momentum applied each time) and
+``num_batches_tracked`` grows by k; the metrics row is the mean of the k micro-batches' ``[loss,
+prec@1, prec@5]``; ``static_out`` holds the LAST micro-batch's logits.  With ``batch_mix`` one draw
+serves the step and each micro-batch is mixed with its own flipped micro-batch.
 """
 
 from __future__ import annotations
 
 import contextlib
+import numbers
 import os
 from typing import Callable, Optional
 
@@ -45,15 +58,29 @@ from ..optim import FusedGossipSGD
 from .distributed import GossipDataParallel
 
 
+def check_accumulation_steps(k) -> int:
+    """``k`` as an int; ValueError unless it is an integer >= 1 (not a bool)."""
+    if isinstance(k, bool) or not isinstance(k, numbers.Integral) or k < 1:
+        raise ValueError('accumulation_steps must be an integer >= 1, got %r' % (k,))
+    return int(k)
+
+
 class GossipTrainer(object):
 
     def __init__(self, model: GossipDataParallel, optimizer: FusedGossipSGD,
                  criterion: Optional[Callable] = None, amp_dtype=torch.bfloat16,
                  use_cuda_graph: bool = True, warmup_iters: int = 3,
-                 channels_last: bool = True, batch_mix=None, ema=None):
+                 channels_last: bool = True, batch_mix=None, ema=None, accumulation_steps: int = 1):
         """``batch_mix``: an ``ops.batch_mix.BatchMix`` to train with mixup / CutMix (needs the
         fused criterion; the draw of each step comes from ``batch_mix.iteration``), or None.
-        ``ema``: an ``ops.model_ema.ModelEma`` of ``model`` updated at the end of every step, or None."""
+        ``ema``: an ``ops.model_ema.ModelEma`` of ``model`` updated at the end of every step, or None.
+        ``accumulation_steps``: k >= 1 forward/backward passes per step over equal row slices of the
+        step batch, whose size must be divisible by k (see the module docstring); not with
+        ``nprocs_per_node > 1``."""
+        accumulation_steps = check_accumulation_steps(accumulation_steps)
+        if accumulation_steps > 1 and getattr(model, 'nprocs_per_node', 1) > 1:
+            raise ValueError('accumulation_steps > 1 is not supported with nprocs_per_node > 1 (hierarchical '
+                             'mode averages the gradient inside the node at every backward pass)')
         assert model._kernel is not None, 'GossipTrainer drives the nvlink kernel transport'
         self.model = model
         self.opt = optimizer
@@ -64,6 +91,10 @@ class GossipTrainer(object):
         self._init_runtime(self.engine.device, criterion, amp_dtype, use_cuda_graph, warmup_iters,
                            channels_last, batch_mix, ema)
         self._slowmo_on = model.slowmo_frequency > 0      # step() runs the SlowMo step itself
+        self.accumulation_steps = accumulation_steps
+        if accumulation_steps > 1 and not self.batched_grad_copy and getattr(model, '_twin', None):
+            raise ValueError('accumulation_steps > 1 with the bf16 compute twin needs the batched gradient '
+                             'copy (SGP_B200_BATCHED_GRAD_COPY=0 would sum its gradients in bf16)')
 
     def _init_runtime(self, device, criterion, amp_dtype, use_cuda_graph, warmup_iters, channels_last,
                       batch_mix=None, ema=None):
@@ -93,6 +124,12 @@ class GossipTrainer(object):
         # see _backward(); SGP_B200_BATCHED_GRAD_COPY=0 restores per-parameter accumulation
         self.batched_grad_copy = os.environ.get('SGP_B200_BATCHED_GRAD_COPY', '1') != '0'
         self._grad_slots = None
+        self.accumulation_steps = 1          # (GossipTrainer(accumulation_steps=k) sets k)
+        self._accum_dst = None               # per grad slot: the fp32 view micro-batches 1..k-1 add into
+        self._micro = None                   # [(input slice, target slice)] of the k micro-batches
+        self._micro_metrics = None           # [k, 3]: [loss, prec@1, prec@5] of each micro-batch
+        # slots whose fresh gradient had a foreign dtype, shape or strides and were added with add_()
+        self.accum_fallbacks = 0
         # every launch of the step runs on ONE dedicated side stream: autograd's
         # AccumulateGrad nodes are then created on the stream the graph is captured on
         self.stream = torch.cuda.Stream(device=self.device)
@@ -123,39 +160,53 @@ class GossipTrainer(object):
         return torch.autocast('cuda', dtype=self.amp_dtype)
 
     def _fwd_bwd(self):
+        if self.accumulation_steps == 1:
+            out = self._fwd_bwd_one(self.static_in, self.static_tgt, self.static_metrics, accumulate=False)
+        else:
+            for j, (x, t) in enumerate(self._micro):
+                out = self._fwd_bwd_one(x, t, self._micro_metrics[j], accumulate=j > 0)
+            torch.mean(self._micro_metrics, 0, out=self.static_metrics)
+        self.static_out = out.detach()
+
+    def _fwd_bwd_one(self, x, tgt, metrics_out, accumulate):
+        """forward + loss + backward of one (micro-)batch; its ``[loss, prec@1 %, prec@5 %]`` go to
+        ``metrics_out``.  ``accumulate``: add the gradients to the arena instead of writing them."""
         twin = getattr(self.model, '_twin', None)
         net = None
         if twin:
             # bf16 twin: weights already live in bf16 (shadow arena), input buffer is bf16
             net = twin[0]
             net.train(self.model.module.training)
-            out = net(self.static_in)
-            loss = self._loss(out)
+            out = net(x)
+            loss = self._loss(out, tgt)
         else:
             with self._autocast():
-                out = self.model.module(self.static_in)
-                loss = self._loss(out)
-        self._backward(loss, net if twin else self.model.module)
+                out = self.model.module(x)
+                loss = self._loss(out, tgt)
+        self._backward(loss, net if twin else self.model.module, accumulate)
         metrics = getattr(self.criterion, 'metrics', None)
         if metrics is not None:
-            self.static_metrics.copy_(metrics)          # [loss, prec@1 %, prec@5 %]
+            metrics_out.copy_(metrics)                  # [loss, prec@1 %, prec@5 %]
         else:
-            self.static_metrics[0].copy_(loss.detach())
-        self.static_out = out.detach()
+            metrics_out[0].copy_(loss.detach())
+        return out
 
-    def _loss(self, out):
+    def _loss(self, out, tgt):
         if self.batch_mix is not None:            # two targets per row, lam from the device mix state
-            return self.criterion(out, self.static_tgt, mix=self.batch_mix.state)
-        return self.criterion(out if self._fused_loss else out.float(), self.static_tgt)
+            return self.criterion(out, tgt, mix=self.batch_mix.state)
+        return self.criterion(out if self._fused_loss else out.float(), tgt)
 
-    def _backward(self, loss, net):
+    def _backward(self, loss, net, accumulate=False):
         """``loss.backward()`` without ~160 per-parameter accumulate kernels: the flat gradient
         buffers are zero at this point (the fused SGD kernel clears them), so instead of letting
         autograd run ``p.grad += g`` once per parameter, the ``.grad`` views are detached for
         the backward pass (autograd then just keeps each fresh gradient) and the results are
-        written into the arena with one multi-tensor copy per dtype."""
+        written into the arena with one multi-tensor copy per dtype.
+
+        ``accumulate`` (micro-batches 1 .. k-1 of gradient accumulation): the fresh gradients are
+        added in fp32 to :meth:`_accum_views` by one ``grad_accumulate`` launch instead."""
         if not self.batched_grad_copy:
-            loss.backward()
+            loss.backward()                                # (autograd accumulates into the views)
             return
         if self._grad_slots is None:
             self._grad_slots = [(p, p.grad) for p in net.parameters()
@@ -163,6 +214,9 @@ class GossipTrainer(object):
         for p, _ in self._grad_slots:
             p.grad = None
         loss.backward()
+        if accumulate:
+            self._accumulate_grads(net)
+            return
         by_dtype = {}
         for p, view in self._grad_slots:
             g = p.grad
@@ -177,6 +231,39 @@ class GossipTrainer(object):
             src.append(g)
         for dst, src in by_dtype.values():
             torch._foreach_copy_(dst, src)
+
+    def _accum_views(self, net):
+        """per grad slot, the fp32 view the later micro-batches add into: the slot's own view for an
+        fp32 model; with the bf16 twin the parameter's view in the fp32 ``g2`` buffer (``lo`` keeps
+        micro-batch 0 in bf16, the step kernel reads ``g + g2`` and clears both)"""
+        if self._accum_dst is None:
+            if getattr(self.model, '_twin', None):
+                hi = self.opt._arenas[torch.float32].views_of(self.opt.grad_flat[torch.float32])
+                by_param = {id(p): v for p, v in zip(net.parameters(), hi)}
+                self._accum_dst = [by_param[id(p)] for p, _ in self._grad_slots]
+            else:
+                self._accum_dst = [view for _, view in self._grad_slots]
+        return self._accum_dst
+
+    def _accumulate_grads(self, net):
+        dst, src = [], []
+        for (p, view), acc in zip(self._grad_slots, self._accum_views(net)):
+            g = p.grad
+            p.grad = view
+            if g is None:
+                continue
+            # (a size-1 dim's stride addresses nothing: a 1x1 conv's fresh gradient may come
+            # channels_last-strided while its arena view is contiguous, with the same memory order)
+            if (acc.dtype == torch.float32 and g.dtype in (torch.float32, torch.bfloat16)
+                    and g.shape == acc.shape
+                    and all(n == 1 or a == b for n, a, b in zip(g.shape, g.stride(), acc.stride()))):
+                dst.append(acc)
+                src.append(g)
+            else:
+                acc.add_(g)                                # foreign layout / dtype: plain add
+                self.accum_fallbacks += 1
+        if dst:
+            self.engine.C.grad_accumulate(dst, src)
 
     def _step_sync(self):
         """forward/backward, then ONE kernel: SGD + publish + pull + mix + de-bias
@@ -220,6 +307,10 @@ class GossipTrainer(object):
     def _ensure_static(self, batch, target):
         if self.static_in is not None:
             return
+        k = self.accumulation_steps
+        if batch.shape[0] % k:
+            raise ValueError('the step batch of %d rows is not divisible by accumulation_steps=%d'
+                             % (batch.shape[0], k))
         fmt = torch.channels_last if (self.channels_last and batch.dim() == 4) \
             else torch.contiguous_format
         in_dtype = torch.bfloat16 if getattr(self.model, '_twin', None) else batch.dtype
@@ -232,6 +323,12 @@ class GossipTrainer(object):
         self._stage_tgt = torch.empty_like(self.static_tgt)
         self.static_metrics = torch.full((3,), float('nan'), dtype=torch.float32, device=self.device)
         self.static_loss = self.static_metrics[0]
+        if k > 1:
+            # dim-0 slices: an NHWC slice is itself channels_last-contiguous, so no copy
+            m = batch.shape[0] // k
+            self._micro = [(self.static_in[j * m:(j + 1) * m], self.static_tgt[j * m:(j + 1) * m])
+                           for j in range(k)]
+            self._micro_metrics = torch.full((k, 3), float('nan'), dtype=torch.float32, device=self.device)
         self._metrics_ring = torch.zeros(1024, 3, dtype=torch.float32).pin_memory()
         self._loss_ring = self._metrics_ring[:, 0]
         self.stream.wait_stream(torch.cuda.current_stream(self.device))
@@ -245,7 +342,7 @@ class GossipTrainer(object):
         do_sgd = not self._skip_next_sgd
         self._skip_next_sgd = False
         if isinstance(self.opt, FusedGossipSGD):
-            self.opt.set_engine_hyper(self.engine, do_sgd=do_sgd)
+            self.opt.set_engine_hyper(self.engine, do_sgd=do_sgd, micro_batches=self.accumulation_steps)
             return
         g = self.opt.param_groups[0]          # (the all-reduce / AD-PSGD trainers' one-group facades)
         self.engine.set_hyper(g['lr'], g['momentum'], g['weight_decay'], g['nesterov'],
@@ -277,7 +374,8 @@ class GossipTrainer(object):
         with torch.cuda.stream(main):
             if self.batch_mix is not None:
                 # the same read and write of the batch, mixed with its flipped batch on the way
-                self.batch_mix.apply(self._stage, self.static_in)
+                # (with accumulation: each micro-batch with its own flipped micro-batch, one draw)
+                self.batch_mix.apply(self._stage, self.static_in, micro_batches=self.accumulation_steps)
             else:
                 self.static_in.copy_(self._stage, non_blocking=True)
             self.static_tgt.copy_(self._stage_tgt, non_blocking=True)

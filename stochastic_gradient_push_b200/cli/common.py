@@ -148,6 +148,15 @@ def build_parser(adpsgd: bool = False) -> argparse.ArgumentParser:
                         "shards: pre-decoded uint8 shards under DATASET_DIR/{train,val} (python -m "
                         "stochastic_gradient_push_b200.data.make_shards) gathered by a background thread, "
                         "crop / flip / normalisation on the GPU (data/shards.py)")
+    p.add_argument('--auto_augment', default='none', choices=['none', 'ta_wide'],
+                   help='ta_wide: TrivialAugmentWide on the training images (torchvision\'s ResNet-50 recipe); '
+                        'with --data_format shards inside the GPU augment kernel (data.GpuAugment), with '
+                        '--data_format folder transforms.TrivialAugmentWide() after the flip.  Not with '
+                        'synthetic data')
+    p.add_argument('--random_erase', default=0.0, type=float,
+                   help='probability p in [0, 1] of RandomErasing(p, value=0) after the normalisation of each '
+                        'training image (GPU augment kernel with --data_format shards, '
+                        'transforms.RandomErasing(p) with --data_format folder); 0 = off.  Not with synthetic data')
     p.add_argument('--fused', default=True, **B, help='FusedGossipSGD (SGD inside the gossip kernel)')
     p.add_argument('--amp', default=True, **B, help='bf16 autocast for forward/backward')
     p.add_argument('--channels_last', default=True, **B)
@@ -292,6 +301,7 @@ def finalize_args(args, adpsgd=False):
     if not 0.0 <= getattr(args, 'label_smoothing', 0.0) <= 1.0:
         raise ValueError('--label_smoothing must be in [0, 1], got %r' % (args.label_smoothing,))
     check_mix_flags(args)
+    check_augment_flags(args)
     check_ema_flags(args, adpsgd)
     args.ema_fname = '{}{}ema_r{}_n{}.csv'.format(args.checkpoint_dir, args.tag, args.rank, args.world_size)
     args.consensus_fname = '{}{}consensus_r{}_n{}.csv'.format(args.checkpoint_dir, args.tag, args.rank,
@@ -347,6 +357,17 @@ def check_mix_flags(args):
         v = getattr(args, flag, 0.0)
         if not 0.0 <= v <= 1.0:
             raise ValueError('--%s must be in [0, 1], got %r' % (flag, v))
+
+
+def check_augment_flags(args):
+    """ValueError for --random_erase outside [0, 1], and for --auto_augment / --random_erase with
+    synthetic data (there are no images to augment)."""
+    p = getattr(args, 'random_erase', 0.0)
+    if not 0.0 <= p <= 1.0:
+        raise ValueError('--random_erase must be in [0, 1], got %r' % (p,))
+    if (getattr(args, 'auto_augment', 'none') != 'none' or p > 0) and args.synthetic:
+        raise ValueError('--auto_augment / --random_erase need image data (--dataset_dir); synthetic data '
+                         'has no images to augment')
 
 
 def check_grad_clip_flags(args, adpsgd=False):
@@ -525,12 +546,8 @@ def make_dataloader(args, train=True):
         return ShardLoader(os.path.join(args.dataset_dir, 'val'), args.batch_size, 1, 0, shuffle=False,
                            drop_last=False, seed=args.seed)
     import torchvision.datasets as datasets
-    import torchvision.transforms as transforms
-    norm = transforms.Normalize(mean=[0.485, 0.456, 0.406], std=[0.229, 0.224, 0.225])
     if train:
-        ds = datasets.ImageFolder(os.path.join(args.dataset_dir, 'train'), transforms.Compose([
-            transforms.RandomResizedCrop(args.image_size), transforms.RandomHorizontalFlip(),
-            transforms.ToTensor(), norm]))
+        ds = datasets.ImageFolder(os.path.join(args.dataset_dir, 'train'), folder_transforms(args, train=True))
         sampler = torch.utils.data.distributed.DistributedSampler(
             ds, num_replicas=args.world_size, rank=args.rank)
         loader = torch.utils.data.DataLoader(
@@ -538,22 +555,42 @@ def make_dataloader(args, train=True):
             num_workers=args.num_dataloader_workers, pin_memory=True, drop_last=True,
             persistent_workers=args.num_dataloader_workers > 0)
         return loader, sampler
-    ds = datasets.ImageFolder(os.path.join(args.dataset_dir, 'val'), transforms.Compose([
-        transforms.Resize(int(args.image_size * 256 / 224)), transforms.CenterCrop(args.image_size),
-        transforms.ToTensor(), norm]))
+    ds = datasets.ImageFolder(os.path.join(args.dataset_dir, 'val'), folder_transforms(args, train=False))
     return torch.utils.data.DataLoader(ds, batch_size=args.batch_size, shuffle=False,
                                        num_workers=args.num_dataloader_workers, pin_memory=True)
 
 
+def folder_transforms(args, train=True):
+    """The ``--data_format folder`` pipeline: RandomResizedCrop, flip, [TrivialAugmentWide],
+    ToTensor, Normalize, [RandomErasing] for training (torchvision's recipe order), Resize +
+    CenterCrop for validation, which never augments."""
+    import torchvision.transforms as transforms
+    norm = transforms.Normalize(mean=[0.485, 0.456, 0.406], std=[0.229, 0.224, 0.225])
+    if not train:
+        return transforms.Compose([transforms.Resize(int(args.image_size * 256 / 224)),
+                                   transforms.CenterCrop(args.image_size), transforms.ToTensor(), norm])
+    steps = [transforms.RandomResizedCrop(args.image_size), transforms.RandomHorizontalFlip()]
+    if getattr(args, 'auto_augment', 'none') == 'ta_wide':
+        steps.append(transforms.TrivialAugmentWide())
+    steps += [transforms.ToTensor(), norm]
+    if getattr(args, 'random_erase', 0.0) > 0:
+        steps.append(transforms.RandomErasing(p=args.random_erase))
+    return transforms.Compose(steps)
+
+
 def device_batch(args, batch, train=True):
     """uint8 shard batches (``--data_format shards``): copy the bytes to the device and run the
-    crop / flip / normalisation there (``data.GpuAugment``); anything else passes through."""
+    crop / flip / normalisation, and --auto_augment / --random_erase on training batches, there
+    (``data.GpuAugment``); anything else passes through."""
     if batch.dtype != torch.uint8:
         return batch
     aug = getattr(args, '_gpu_augment', None)
     if aug is None:
         from ..data import GpuAugment
-        aug = args._gpu_augment = GpuAugment(out_size=args.image_size, seed=args.seed * 7919 + args.rank)
+        ta = getattr(args, 'auto_augment', 'none')
+        aug = args._gpu_augment = GpuAugment(out_size=args.image_size, seed=args.seed * 7919 + args.rank,
+                                             auto_augment=None if ta == 'none' else ta,
+                                             random_erase=getattr(args, 'random_erase', 0.0))
     return aug(batch.to(args.device, non_blocking=True), train=train)
 
 

@@ -30,7 +30,7 @@ import math
 import os
 import queue
 import threading
-from typing import List, Optional, Sequence
+from typing import List, NamedTuple, Optional, Sequence
 
 import numpy as np
 import torch
@@ -38,6 +38,7 @@ import torch.nn.functional as F
 
 IMAGENET_MEAN = (0.485, 0.456, 0.406)
 IMAGENET_STD = (0.229, 0.224, 0.225)
+RING_SLOTS = 8                  # pinned staging slots of the augment kernel's per-image rows
 
 
 # --------------------------------------------------------------------------- #
@@ -237,17 +238,114 @@ class ShardLoader(object):
 # --------------------------------------------------------------------------- #
 # GPU-side augmentation
 # --------------------------------------------------------------------------- #
+# TrivialAugmentWide (Mueller & Hutter 2021) as torchvision.transforms.v2.TrivialAugmentWide draws it:
+# one op uniform over these 14, one of 31 magnitude bins, a random sign for the signed ops
+TA_WIDE_OPS = ('Identity', 'ShearX', 'ShearY', 'TranslateX', 'TranslateY', 'Rotate', 'Brightness', 'Color',
+               'Contrast', 'Sharpness', 'Posterize', 'Solarize', 'AutoContrast', 'Equalize')
+TA_WIDE_SIGNED = frozenset(TA_WIDE_OPS[1:10])
+TA_WIDE_BINS = 31
+GEOMETRIC_OPS = frozenset(TA_WIDE_OPS[1:6])
+ERASE_SCALE = (0.02, 0.33)
+ERASE_RATIO = (0.3, 3.3)
+ERASE_ATTEMPTS = 10
+# dynamic shared memory one CTA may use on sm_90 (227 KB); the augment kernel keeps the whole
+# out x out x 3 uint8 crop there plus its per-op tables
+SM90_SMEM_PER_CTA = 232448
+AUGMENT_ROW = 24
+
+
+def ta_wide_magnitudes(num_bins: int = TA_WIDE_BINS) -> dict:
+    """op name -> magnitude per bin (fp32 values as torchvision's v2 tables hold them; None for
+    the ops without a magnitude)."""
+    lin = lambda hi: torch.linspace(0.0, hi, num_bins)  # noqa: E731
+    return {
+        'Identity': None, 'ShearX': lin(0.99), 'ShearY': lin(0.99), 'TranslateX': lin(32.0),
+        'TranslateY': lin(32.0), 'Rotate': lin(135.0), 'Brightness': lin(0.99), 'Color': lin(0.99),
+        'Contrast': lin(0.99), 'Sharpness': lin(0.99),
+        'Posterize': (8 - (torch.arange(num_bins) / ((num_bins - 1) / 6))).round().int(),
+        'Solarize': torch.linspace(1.0, 0.0, num_bins), 'AutoContrast': None, 'Equalize': None,
+    }
+
+
+def augment_smem_bytes(out: int) -> int:
+    """Shared memory of one augment-kernel CTA for ``out x out`` output images (the kernel's
+    ``aug_smem_bytes``)."""
+    return (3 * out * out + 15) // 16 * 16 + (3 * 256 + 16) * 4
+
+
+class AugmentParams(NamedTuple):
+    """Per-sample parameters of one training batch (CPU tensors, ``n`` rows each).
+
+    ``cx, cy, w, h, flip``: the RandomResizedCrop box as fractions of the stored image and the flip
+    sign (fp32, :meth:`GpuAugment.sample_boxes`); ``op``: int64 index into :data:`TA_WIDE_OPS`;
+    ``magnitude``: float64, the signed magnitude torchvision would pass to the op (0 for the ops
+    without one); ``erase``: int64 ``[n, 4]`` box ``(top, left, height, width)`` in output pixels,
+    height 0 = no box."""
+    cx: torch.Tensor
+    cy: torch.Tensor
+    w: torch.Tensor
+    h: torch.Tensor
+    flip: torch.Tensor
+    op: torch.Tensor
+    magnitude: torch.Tensor
+    erase: torch.Tensor
+
+
+def inverse_affine_matrix(center, angle: float, translate, shear) -> List[float]:
+    """Inverse of ``T C R(angle) Sh(shear) C^-1`` (scale 1) as the 2 x 3 row-major list that maps
+    output pixels to input pixels, in coordinates relative to the image centre: the matrix
+    torchvision's ``affine`` / ``rotate`` sample through.  Angles in degrees."""
+    rot = math.radians(angle)
+    sx, sy = math.radians(shear[0]), math.radians(shear[1])
+    cx, cy = center
+    tx, ty = translate
+    # R S the forward rotation-shear block [[a, b], [c, d]] (determinant 1)
+    a = math.cos(rot - sy) / math.cos(sy)
+    b = -(a * math.tan(sx) + math.sin(rot))
+    c = math.sin(rot - sy) / math.cos(sy)
+    d = math.cos(rot) - c * math.tan(sx)
+    m = [d, -b, 0.0, -c, a, 0.0]
+    m[2] += cx - m[0] * (cx + tx) - m[1] * (cy + ty)
+    m[5] += cy - m[3] * (cx + tx) - m[4] * (cy + ty)
+    return m
+
+
+def ta_wide_matrix(op: str, magnitude: float, size: int) -> List[float]:
+    """The inverse affine matrix of geometric op ``op`` at ``magnitude`` on a ``size x size``
+    image, with the arguments TrivialAugmentWide passes (shears about the top-left corner,
+    translations truncated to whole pixels, rotations about the centre)."""
+    if op in ('ShearX', 'ShearY'):
+        deg = math.degrees(math.atan(magnitude))
+        shear = [deg, 0.0] if op == 'ShearX' else [0.0, deg]
+        return inverse_affine_matrix([-size * 0.5, -size * 0.5], 0.0, [0.0, 0.0], shear)
+    if op in ('TranslateX', 'TranslateY'):
+        t = [float(int(magnitude)), 0.0] if op == 'TranslateX' else [0.0, float(int(magnitude))]
+        return inverse_affine_matrix([0.0, 0.0], 0.0, t, [0.0, 0.0])
+    if op == 'Rotate':
+        return inverse_affine_matrix([0.0, 0.0], -(magnitude % 360), [0.0, 0.0], [0.0, 0.0])
+    raise ValueError('%s is not a geometric op' % op)
+
+
 class GpuAugment(object):
     """uint8 ``[B, S, S, 3]`` -> normalised ``[B, 3, out, out]`` (channels-last memory format).
 
     training: ``RandomResizedCrop(out, scale, ratio)`` + horizontal flip, all samples in ONE
     ``grid_sample`` (the crop box of sample i is the affine map ``theta_i``; flip negates its x
     scale); evaluation: centre crop of ``out / eval_ratio`` resized to ``out`` (the reference's
-    ``Resize(256) + CenterCrop(224)`` when the shards were stored at 256)."""
+    ``Resize(256) + CenterCrop(224)`` when the shards were stored at 256).
+
+    ``auto_augment='ta_wide'`` adds TrivialAugmentWide and ``random_erase=p`` adds
+    ``RandomErasing(p, value=0)`` after the normalisation, in torchvision's recipe order.  With
+    either on, a training batch on the GPU is ONE launch of the sm_90a augment kernel
+    (``csrc/augment_kernels.cu``): the crop rounded to uint8 as torchvision's uint8 pipeline
+    rounds it, the op, the normalisation and the erase box.  Their draws come from a second
+    generator, so the crop boxes and flips of a seed do not depend on these options.  CPU batches
+    take the reference composition (``ops.oracle.reference_augment``); evaluation never augments."""
 
     def __init__(self, out_size: int = 224, scale=(0.08, 1.0), ratio=(3.0 / 4.0, 4.0 / 3.0),
                  mean=IMAGENET_MEAN, std=IMAGENET_STD, dtype=torch.float32, eval_ratio: float = 0.875,
-                 seed: int = 0, channels_last: bool = True):
+                 seed: int = 0, channels_last: bool = True, auto_augment: Optional[str] = None,
+                 random_erase: float = 0.0):
         self.out = int(out_size)
         self.scale, self.ratio = scale, ratio
         self.mean, self.std = tuple(mean), tuple(std)
@@ -256,6 +354,29 @@ class GpuAugment(object):
         self.channels_last = channels_last
         self._gen = torch.Generator().manual_seed(int(seed))
         self._consts = {}
+        if auto_augment not in (None, 'ta_wide'):
+            raise ValueError("auto_augment must be None or 'ta_wide', got %r" % (auto_augment,))
+        if not 0.0 <= float(random_erase) <= 1.0:
+            raise ValueError('random_erase must be in [0, 1], got %r' % (random_erase,))
+        self.auto_augment = auto_augment
+        self.random_erase = float(random_erase)
+        if self.augments and augment_smem_bytes(self.out) > SM90_SMEM_PER_CTA:
+            raise ValueError('out_size %d needs %d bytes of shared memory per image with auto_augment / '
+                             'random_erase; an sm_90 CTA has %d' % (self.out, augment_smem_bytes(self.out),
+                                                                   SM90_SMEM_PER_CTA))
+        self._aug_gen = torch.Generator().manual_seed(int(seed) * 1000003 + 0x7A5)
+        tables = ta_wide_magnitudes()
+        self._table = torch.stack([torch.zeros(TA_WIDE_BINS, dtype=torch.float64) if tables[k] is None
+                                   else tables[k].double() for k in TA_WIDE_OPS])
+        self._signed = torch.tensor([k in TA_WIDE_SIGNED for k in TA_WIDE_OPS])
+        self._ring = None
+        self._events = [None] * RING_SLOTS
+        self._slot = 0
+
+    @property
+    def augments(self) -> bool:
+        """True when training batches take the augment kernel (TrivialAugment or erasing on)."""
+        return self.auto_augment is not None or self.random_erase > 0
 
     def _norm(self, device):
         key = str(device)
@@ -282,8 +403,138 @@ class GpuAugment(object):
         flip = torch.where(torch.rand(n, generator=g) < 0.5, -torch.ones(n), torch.ones(n))
         return cx, cy, w, h, flip
 
+    @staticmethod
+    def crop_theta(cx, cy, w, h, flip) -> torch.Tensor:
+        """fp32 ``[n, 2, 3]`` affine maps of the crop boxes (``F.affine_grid`` convention)."""
+        theta = torch.zeros(len(cx), 2, 3)
+        theta[:, 0, 0] = w * flip          # output x in [-1, 1] -> input x: centre + half-width * x
+        theta[:, 0, 2] = 2 * cx - 1
+        theta[:, 1, 1] = h
+        theta[:, 1, 2] = 2 * cy - 1
+        return theta
+
+    def sample_params(self, n: int) -> AugmentParams:
+        """The next training batch's :class:`AugmentParams`: crop boxes and flips from
+        :meth:`sample_boxes`, then, from the second generator, per sample, TrivialAugmentWide's op
+        (uniform over :data:`TA_WIDE_OPS`), bin (uniform over 31) and sign (negative with
+        probability 1/2, signed ops only), and RandomErasing's box: with probability ``p``, up to
+        10 attempts of area fraction U(0.02, 0.33) and log aspect ratio U(log 0.3, log 3.3),
+        ``h = round(sqrt(area r))``, ``w = round(sqrt(area / r))``; the first box strictly inside
+        the image is placed at a uniform integer position, none if no attempt fits."""
+        cx, cy, w, h, flip = self.sample_boxes(n)
+        g = self._aug_gen
+        op = torch.zeros(n, dtype=torch.int64)
+        magnitude = torch.zeros(n, dtype=torch.float64)
+        if self.auto_augment == 'ta_wide':
+            op = torch.randint(len(TA_WIDE_OPS), (n,), generator=g)
+            bins = torch.randint(TA_WIDE_BINS, (n,), generator=g)
+            negate = torch.rand(n, generator=g) <= 0.5
+            sign = torch.where(negate & self._signed[op], -1.0, 1.0).double()
+            magnitude = self._table[op, bins] * sign
+        erase = torch.zeros(n, 4, dtype=torch.int64)
+        if self.random_erase > 0:
+            size = self.out
+            hit = torch.rand(n, generator=g) < self.random_erase
+            area = size * size * torch.empty(n, ERASE_ATTEMPTS, dtype=torch.float64).uniform_(
+                ERASE_SCALE[0], ERASE_SCALE[1], generator=g)
+            logr = torch.empty(n, ERASE_ATTEMPTS, dtype=torch.float64).uniform_(
+                math.log(ERASE_RATIO[0]), math.log(ERASE_RATIO[1]), generator=g)
+            pos = torch.rand(n, 2, dtype=torch.float64, generator=g).numpy()
+            # (numpy for the elementwise math: torch's intra-op pool costs more than these few
+            # thousand elements)
+            r = np.exp(logr.numpy())
+            area = area.numpy()
+            eh = np.round(np.sqrt(area * r)).astype(np.int64)
+            ew = np.round(np.sqrt(area / r)).astype(np.int64)
+            fits = (eh < size) & (ew < size)
+            first = fits.argmax(1)[:, None]                               # first attempt that fits
+            bh, bw = np.take_along_axis(eh, first, 1)[:, 0], np.take_along_axis(ew, first, 1)[:, 0]
+            on = hit.numpy() & fits.any(1)
+            top = np.minimum((pos[:, 0] * (size - bh + 1)).astype(np.int64), size - bh)
+            left = np.minimum((pos[:, 1] * (size - bw + 1)).astype(np.int64), size - bw)
+            erase = torch.from_numpy(np.where(on[:, None], np.stack([top, left, bh, bw], 1), 0))
+        return AugmentParams(cx, cy, w, h, flip, op, magnitude, erase)
+
+    def kernel_rows(self, params: AugmentParams, S: int) -> np.ndarray:
+        """fp32 ``[n, AUGMENT_ROW]``: the augment kernel's per-image rows for ``params`` (layout in
+        ``csrc/augment_kernels.cu``).  Every op scalar is rounded to fp32 the way torch rounds a
+        Python scalar against an fp32 tensor."""
+        n = len(params.op)
+        out = self.out
+        rows = np.zeros((n, AUGMENT_ROW), dtype=np.float32)
+        rows[:, 0:6] = self.crop_theta(params.cx, params.cy, params.w, params.h, params.flip).reshape(n, 6).numpy()
+        op = params.op.numpy()
+        mag = params.magnitude.numpy()
+        rows[:, 6] = op
+        is_op = lambda *names: np.isin(op, [TA_WIDE_OPS.index(k) for k in names])  # noqa: E731
+        sel = is_op('Brightness', 'Color', 'Contrast')
+        rows[sel, 7] = 1.0 + mag[sel]
+        sel = is_op('Color', 'Contrast', 'Sharpness')
+        rows[sel, 8] = 1.0 - (1.0 + mag[sel])
+        sel = is_op('Posterize')
+        bits = mag[sel].astype(np.int64)
+        rows[sel, 7] = np.where(bits >= 8, 255, ((1 << bits) - 1) << np.maximum(8 - bits, 0))
+        sel = is_op('Solarize')
+        rows[sel, 7] = 255.0 * mag[sel]
+        half = np.float32(0.5 * out)
+        for i in np.nonzero(is_op(*GEOMETRIC_OPS))[0]:
+            m = np.asarray(ta_wide_matrix(TA_WIDE_OPS[op[i]], float(mag[i]), out), dtype=np.float32)
+            rows[i, 9:15] = m / half           # torchvision's _affine_grid: theta^T / [w / 2, h / 2] in fp32
+        e = params.erase.numpy()
+        rows[:, 15], rows[:, 16], rows[:, 17], rows[:, 18] = e[:, 0], e[:, 0] + e[:, 2], e[:, 1], e[:, 1] + e[:, 3]
+        return rows
+
+    def _stage_rows(self, rows: np.ndarray, device) -> torch.Tensor:
+        """``rows`` -> a fresh device tensor through ONE non-blocking H2D copy from a slot of a
+        pinned ring; a slot is rewritten only after the copy that last read it has executed."""
+        n = rows.shape[0]
+        if self._ring is None or self._ring.shape[1] < n:
+            for ev in self._events:
+                if ev is not None:
+                    ev.synchronize()
+            self._ring = torch.empty(RING_SLOTS, n, AUGMENT_ROW, dtype=torch.float32, pin_memory=True)
+            self._events = [None] * RING_SLOTS
+        slot = self._slot
+        self._slot = (slot + 1) % RING_SLOTS
+        if self._events[slot] is not None:
+            self._events[slot].synchronize()
+        host = self._ring[slot, :n]
+        host.numpy()[:] = rows
+        dev_rows = torch.empty(n, AUGMENT_ROW, dtype=torch.float32, device=device)
+        dev_rows.copy_(host, non_blocking=True)
+        ev = self._events[slot] = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(device))
+        return dev_rows
+
+    def apply(self, batch_u8: torch.Tensor, params: AugmentParams) -> torch.Tensor:
+        """The training output of ``batch_u8`` for explicit per-sample ``params``: crop, round to
+        uint8, TrivialAugmentWide op, normalise, erase.  CUDA: one launch of the sm_90a augment
+        kernel (a missing extension is an error) and no host synchronisation; CPU: the reference
+        composition ``ops.oracle.reference_augment``."""
+        assert batch_u8.dtype == torch.uint8 and batch_u8.dim() == 4 and batch_u8.shape[-1] == 3
+        n, S = batch_u8.shape[0], batch_u8.shape[1]
+        if augment_smem_bytes(self.out) > SM90_SMEM_PER_CTA:
+            raise ValueError('out_size %d is too large for the augment kernel' % self.out)
+        mean, inv = self._norm('cpu')
+        if not batch_u8.is_cuda:
+            from ..ops.oracle import reference_augment
+            theta = self.crop_theta(params.cx, params.cy, params.w, params.h, params.flip)
+            y = reference_augment(batch_u8, theta, params.op, params.magnitude, params.erase, self.out, mean, inv)
+        else:
+            from ..ops import native
+            C = native.load()
+            y = torch.empty(n, 3, self.out, self.out, dtype=self.dtype, device=batch_u8.device,
+                            memory_format=torch.channels_last)
+            rows = self._stage_rows(self.kernel_rows(params, S), batch_u8.device)
+            C.gpu_augment(batch_u8.contiguous(), rows, y, mean.view(-1).tolist(), inv.view(-1).tolist())
+        if not self.channels_last:
+            y = y.contiguous()
+        return y.to(self.dtype)
+
     def __call__(self, batch_u8: torch.Tensor, train: bool = True) -> torch.Tensor:
         assert batch_u8.dtype == torch.uint8 and batch_u8.dim() == 4 and batch_u8.shape[-1] == 3
+        if train and self.augments:
+            return self.apply(batch_u8, self.sample_params(batch_u8.shape[0]))
         dev = batch_u8.device
         n = batch_u8.shape[0]
         x = batch_u8.permute(0, 3, 1, 2).float()            # NCHW view of the NHWC bytes (= channels-last)
@@ -293,11 +544,7 @@ class GpuAugment(object):
             cx = cy = torch.full((n,), 0.5)
             w = h = torch.full((n,), self.eval_ratio)
             flip = torch.ones(n)
-        theta = torch.zeros(n, 2, 3)
-        theta[:, 0, 0] = w * flip          # output x in [-1, 1] -> input x: centre + half-width * x
-        theta[:, 0, 2] = 2 * cx - 1
-        theta[:, 1, 1] = h
-        theta[:, 1, 2] = 2 * cy - 1
+        theta = self.crop_theta(cx, cy, w, h, flip)
         theta = theta.to(dev, non_blocking=True)
         grid = F.affine_grid(theta, (n, 3, self.out, self.out), align_corners=False)
         y = F.grid_sample(x, grid, mode='bilinear', padding_mode='border', align_corners=False)

@@ -53,6 +53,69 @@ def mix_columns(xs: Sequence[torch.Tensor], ws: Sequence[float], graphs, mixings
     return new_x, new_w
 
 
+def ta_wide_op(img: torch.Tensor, op: str, magnitude: float) -> torch.Tensor:
+    """TrivialAugmentWide's op ``op`` at the signed ``magnitude`` on a uint8 ``[3, H, W]`` image,
+    through ``torchvision.transforms.v2.functional`` with the arguments TrivialAugmentWide passes
+    (nearest interpolation, fill 0)."""
+    import math
+    import torchvision.transforms.v2.functional as TF
+    from torchvision.transforms import InterpolationMode
+    nearest = InterpolationMode.NEAREST
+    if op == 'Identity':
+        return img
+    if op in ('ShearX', 'ShearY'):
+        deg = math.degrees(math.atan(magnitude))
+        return TF.affine(img, angle=0.0, translate=[0, 0], scale=1.0,
+                         shear=[deg, 0.0] if op == 'ShearX' else [0.0, deg], interpolation=nearest,
+                         fill=None, center=[0, 0])
+    if op in ('TranslateX', 'TranslateY'):
+        t = [int(magnitude), 0] if op == 'TranslateX' else [0, int(magnitude)]
+        return TF.affine(img, angle=0.0, translate=t, scale=1.0, shear=[0.0, 0.0], interpolation=nearest,
+                         fill=None)
+    if op == 'Rotate':
+        return TF.rotate(img, angle=magnitude, interpolation=nearest, fill=None)
+    if op == 'Brightness':
+        return TF.adjust_brightness(img, 1.0 + magnitude)
+    if op == 'Color':
+        return TF.adjust_saturation(img, 1.0 + magnitude)
+    if op == 'Contrast':
+        return TF.adjust_contrast(img, 1.0 + magnitude)
+    if op == 'Sharpness':
+        return TF.adjust_sharpness(img, 1.0 + magnitude)
+    if op == 'Posterize':
+        return TF.posterize(img, int(magnitude))
+    if op == 'Solarize':
+        return TF.solarize(img, 255 * magnitude)
+    if op == 'AutoContrast':
+        return TF.autocontrast(img)
+    if op == 'Equalize':
+        return TF.equalize(img)
+    raise ValueError('unknown TrivialAugmentWide op %r' % (op,))
+
+
+def reference_augment(batch_u8: torch.Tensor, theta: torch.Tensor, ops, magnitudes, erase, out_size: int,
+                      mean: torch.Tensor, inv: torch.Tensor) -> torch.Tensor:
+    """What the augment kernel computes, in plain PyTorch + torchvision: ``grid_sample`` of the
+    uint8 NHWC batch with the crop maps ``theta`` (bilinear, border, align_corners=False), rounded
+    to uint8; the TrivialAugmentWide op ``data.shards.TA_WIDE_OPS[ops[i]]`` at ``magnitudes[i]``
+    per sample; ``(v - mean) * inv`` in fp32; 0 inside each ``erase[i] = (top, left, h, w)`` box.
+    Returns fp32 ``[n, 3, out, out]`` in channels-last memory format."""
+    import torch.nn.functional as F
+    from ..data.shards import TA_WIDE_OPS
+    n = batch_u8.shape[0]
+    x = batch_u8.permute(0, 3, 1, 2).float()
+    grid = F.affine_grid(theta.to(x.device), (n, 3, out_size, out_size), align_corners=False)
+    crop = F.grid_sample(x, grid, mode='bilinear', padding_mode='border', align_corners=False)
+    crop = crop.round().clamp(0, 255).to(torch.uint8)
+    y = torch.empty(n, 3, out_size, out_size)
+    for i in range(n):
+        img = ta_wide_op(crop[i], TA_WIDE_OPS[int(ops[i])], float(magnitudes[i]))
+        y[i] = (img.float() - mean[0]) * inv[0]
+        top, left, h, w = (int(v) for v in erase[i])
+        y[i, :, top:top + h, left:left + w] = 0.0
+    return y.contiguous(memory_format=torch.channels_last)
+
+
 def rotate_all(graphs):
     for g in graphs:
         if g.is_dynamic_graph():

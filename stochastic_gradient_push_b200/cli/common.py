@@ -387,6 +387,22 @@ def check_grad_clip_flags(args, adpsgd=False):
                              'D-PSGD' % (flag, unsupported))
 
 
+def check_eval_graph_flags(args):
+    """ValueError for --eval_graph True outside the captured fused gossip step (GossipTrainer), whose
+    ``evaluate()`` it calls."""
+    if not getattr(args, 'eval_graph', False):
+        return
+    unsupported = ('--all_reduce' if args.all_reduce else
+                   '--fused False' if not args.fused else
+                   '--cuda_graph False' if not args.cuda_graph else
+                   '--transport c10d' if args.transport == 'c10d' else
+                   '--device cpu' if args.device == 'cpu' else None)
+    if unsupported:
+        raise ValueError('--eval_graph is not supported with %s: the captured evaluation is '
+                         'GossipTrainer.evaluate, which needs the captured fused gossip step (--cuda_graph True '
+                         '--fused True on the CUDA kernel transport) for SGP, OSGP and D-PSGD' % unsupported)
+
+
 def check_accumulation_flags(args):
     """ValueError for --accumulation_steps < 1, for K > 1 outside the captured fused gossip step
     (GossipTrainer), and for a --batch_size that K does not divide."""

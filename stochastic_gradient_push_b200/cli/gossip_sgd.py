@@ -48,8 +48,15 @@ def parse_args(argv=None):
                              '(GossipTrainer(accumulation_steps=K)); --batch_size stays the per-rank step batch '
                              'and must be divisible by K.  BatchNorm statistics are per micro-batch.  SGP / OSGP '
                              '/ D-PSGD with --cuda_graph True --fused True and --nprocs_per_node 1')
+    parser.add_argument('--eval_graph', default=False, type=common.str2bool, nargs='?', const=True,
+                        help='validate (and --model_ema_decay / --validate_average validation) through '
+                             'GossipTrainer.evaluate: one captured eval graph per batch shape, BatchNorm in the '
+                             '1x1-conv GEMM epilogue, loss and top-1 / top-5 counted on the device and read back '
+                             'once per pass.  Needs the captured trainer (--cuda_graph True --fused True on '
+                             'the CUDA kernel transport, not --all_reduce)')
     args = parser.parse_args(argv)
     common.check_accumulation_flags(args)
+    common.check_eval_graph_flags(args)
     return finalize_args(args, adpsgd=False)
 
 
@@ -155,6 +162,10 @@ def main(argv=None):
                                       amp_dtype=torch.bfloat16 if args.amp else None,
                                       batch_mix=args._batch_mix, ema=args._ema,
                                       accumulation_steps=args.accumulation_steps)
+    if args.eval_graph and args._trainer is None:
+        raise ValueError('--eval_graph is not supported with transport %s: the captured evaluation is '
+                         'GossipTrainer.evaluate, which runs on the CUDA kernel transport only'
+                         % getattr(model, 'transport', 'c10d'))
     if args.accumulation_steps > 1 and args._trainer is None:
         raise ValueError('--accumulation_steps > 1 needs the captured GossipTrainer step, which runs on the '
                          'CUDA kernel transport only (got device %s, transport %s)' % (args.device, model.transport))
@@ -432,7 +443,14 @@ def validate(args, val_loader, model, criterion, log):
 
 
 def evaluate(args, val_loader, model, criterion, log, label=''):
-    """(prec@1, prec@5) over the validation set, logged as `` * <label>Prec@1 .. Prec@5 ..``"""
+    """(prec@1, prec@5) over the validation set, logged as `` * <label>Prec@1 .. Prec@5 ..``;
+    with --eval_graph through the trainer's captured evaluation"""
+    trainer = getattr(args, '_trainer', None)
+    if getattr(args, 'eval_graph', False) and trainer is not None:
+        r = trainer.evaluate((common.device_batch(args, features, train=False), target)
+                             for features, target in val_loader)
+        log.info(' * {label}Prec@1 {p1:.3f} Prec@5 {p5:.3f}'.format(label=label, p1=r.prec1, p5=r.prec5))
+        return r.prec1, r.prec5
     losses, top1, top5 = Meter(ptag='Loss'), Meter(ptag='Prec@1'), Meter(ptag='Prec@5')
     model.eval()
     dev = args.device

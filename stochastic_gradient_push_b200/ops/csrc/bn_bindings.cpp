@@ -402,6 +402,9 @@ cudaError_t c1_launch_gemm(const void* x, const void* w, void* y, long long M, i
 cudaError_t c1_launch_stats_finalize(const float* partial, int R, int C, const float* gamma, const float* beta,
                                      float* rmean, float* rvar, long long* nbt, float momentum, float eps,
                                      float* mean, float* invstd, float* scale, float* shift, cudaStream_t st);
+cudaError_t c1_launch_gemm_bn_eval(const void* x, const void* w, void* y, long long M, int N, int K,
+                                   const void* residual, const float* gamma, const float* beta, const float* mean,
+                                   const float* var, float eps, int relu, int num_sms, int f32, cudaStream_t st);
 }
 
 // x: NHWC bf16 / fp32 activation (4-D channels_last) or [M, K] matrix; w: [N, K, 1, 1] or [N, K], rows
@@ -563,12 +566,44 @@ static std::vector<torch::Tensor> conv1x1_bn_forward(torch::Tensor x, torch::Ten
     return {yraw, out, coef};
 }
 
+// eval-mode  out = act(bn(conv1x1(x, w)) [+ residual]) with the running statistics, in ONE launch: the
+// BatchNorm affine map (from gamma, beta, mean, var as they are at launch time), the residual add and the
+// ReLU run in the GEMM epilogue (MODES 4 / 5).  Nothing is updated.
+static torch::Tensor conv1x1_bn_eval(torch::Tensor x, torch::Tensor w, torch::Tensor gamma, torch::Tensor beta,
+                                     torch::Tensor mean, torch::Tensor var, double eps, bool relu,
+                                     c10::optional<torch::Tensor> residual, int num_sms)
+{
+    TORCH_CHECK(conv1x1_can_fuse(x, w), "conv1x1_bn_eval: unsupported tensors");
+    const int K = (int)x.size(1), N = (int)w.size(0);
+    const long long M = x.numel() / K;
+    for (const torch::Tensor* t : {&gamma, &beta, &mean, &var})
+        TORCH_CHECK(t->is_cuda() && t->get_device() == x.get_device() && t->scalar_type() == torch::kFloat32 &&
+                        t->is_contiguous() && t->numel() == N,
+                    "conv1x1_bn_eval: gamma, beta, mean and var must be contiguous fp32 [N] tensors on x's device");
+    c10::cuda::CUDAGuard guard(x.get_device());
+    auto y = conv1x1_alloc_out(x, N);
+    const bool has_res = residual.has_value() && residual->defined();
+    if (has_res)
+        TORCH_CHECK(residual->is_cuda() && residual->scalar_type() == x.scalar_type() &&
+                        residual->sizes() == y.sizes() && residual->strides() == y.strides() &&
+                        (reinterpret_cast<uintptr_t>(residual->data_ptr()) & 15) == 0,
+                    "conv1x1_bn_eval: residual must match the output's shape and layout");
+    BN_CHECK(c1_launch_gemm_bn_eval(x.data_ptr(), w.data_ptr(), y.data_ptr(), M, N, K,
+                                    has_res ? residual->data_ptr() : nullptr, gamma.data_ptr<float>(),
+                                    beta.data_ptr<float>(), mean.data_ptr<float>(), var.data_ptr<float>(), (float)eps,
+                                    relu ? 1 : 0, plan_sms(num_sms), x.scalar_type() == torch::kFloat32 ? 1 : 0,
+                                    at::cuda::getCurrentCUDAStream()));
+    return y;
+}
+
 // ---------------------------------------------------------------------------
 // fused softmax cross-entropy + top-1 / top-5 accuracy (csrc/loss_kernels.cu)
 // ---------------------------------------------------------------------------
 extern "C" {
 cudaError_t xent_launch_fwd(int dtype, const void* logits, const long long* target, float* lse, float* out3, int B,
                             int C, float eps, const float* mix, cudaStream_t st);
+cudaError_t xent_launch_eval(int dtype, const void* logits, const long long* target, unsigned long long* acc, int B,
+                             int C, cudaStream_t st);
 cudaError_t xent_launch_bwd(int dtype, const void* logits, const long long* target, const float* lse,
                             const float* grad_out, void* dlogits, int B, int C, float eps, const float* mix,
                             cudaStream_t st);
@@ -640,6 +675,21 @@ static torch::Tensor xent_backward(torch::Tensor logits, torch::Tensor target, t
     return dl;
 }
 
+// evaluation: adds the plain cross-entropy sum and the top-1 / top-5 / valid-row counts of this batch to acc,
+// an int64 [4] device tensor: [loss sum as fp64 bits, top-1 hits, top-5 hits, rows with a target in [0, C)]
+static void xent_eval_accumulate(torch::Tensor logits, torch::Tensor target, torch::Tensor acc)
+{
+    TORCH_CHECK(xent_can_fuse(logits, target), "xent_eval_accumulate: unsupported tensors");
+    TORCH_CHECK(acc.is_cuda() && acc.get_device() == logits.get_device() && acc.scalar_type() == torch::kInt64 &&
+                    acc.is_contiguous() && acc.numel() == 4,
+                "xent_eval_accumulate: acc must be a contiguous int64 [4] tensor on the logits' device");
+    c10::cuda::CUDAGuard guard(logits.get_device());
+    BN_CHECK(xent_launch_eval(dtype_code(logits), logits.data_ptr(),
+                              reinterpret_cast<const long long*>(target.data_ptr<int64_t>()),
+                              reinterpret_cast<unsigned long long*>(acc.data_ptr<int64_t>()), (int)logits.size(0),
+                              (int)logits.size(1), at::cuda::getCurrentCUDAStream()));
+}
+
 // ---------------------------------------------------------------------------
 // mixup / CutMix inside the stage -> static input copy (csrc/mix_kernels.cu)
 // ---------------------------------------------------------------------------
@@ -681,6 +731,7 @@ void bind_bn(py::module& mod)
             py::arg("mix") = py::none());
     mod.def("xent_backward", &xent_backward, py::arg("logits"), py::arg("target"), py::arg("lse"),
             py::arg("grad_out"), py::arg("label_smoothing") = 0.0, py::arg("mix") = py::none());
+    mod.def("xent_eval_accumulate", &xent_eval_accumulate, py::arg("logits"), py::arg("target"), py::arg("acc"));
     mod.def("batch_mix", &batch_mix, py::arg("src"), py::arg("out"), py::arg("mix"));
     mod.def("conv1x1_can_fuse", &conv1x1_can_fuse);
     mod.def("conv1x1_plan", &conv1x1_plan, py::arg("M"), py::arg("N"), py::arg("K"), py::arg("num_sms") = 132,
@@ -693,6 +744,9 @@ void bind_bn(py::module& mod)
             py::arg("mask") = py::none(), py::kw_only(), py::arg("num_sms") = 0);
     mod.def("conv1x1_dgrad_bn_reduce", &conv1x1_dgrad_bn_reduce, py::arg("x"), py::arg("w"), py::arg("residual"),
             py::arg("bn_x"), py::arg("coef"), py::arg("mask"), py::kw_only(), py::arg("num_sms") = 0);
+    mod.def("conv1x1_bn_eval", &conv1x1_bn_eval, py::arg("x"), py::arg("w"), py::arg("gamma"), py::arg("beta"),
+            py::arg("mean"), py::arg("var"), py::arg("eps"), py::arg("relu"), py::arg("residual") = py::none(),
+            py::kw_only(), py::arg("num_sms") = 0);
     mod.def("stem_can_fuse", &stem_can_fuse);
     mod.def("stem_forward", &stem_forward);
     mod.def("stem_wgrad", &stem_wgrad);

@@ -333,18 +333,31 @@ struct C1Plan {            // host-computed shared-memory plan (bytes are multip
     int x_hint_first;      // 1: X tiles are read by one CTA only -> L2 evict_first
 };
 
+// MODES 4 / 5 (c1_gemm_eval_kernel): eval-mode BatchNorm of the live parameters and running statistics,
+// Y = act(acc * s[c] + t[c] (+ R)) with s = gamma * rsqrt(running_var + eps), t = beta - running_mean * s
+struct C1Eval {
+    const float* gamma;
+    const float* beta;
+    const float* mean;
+    const float* var;
+    float eps;
+    int relu;
+};
+
 // MODE 0: Y = X.W^T          MODE 1: + BatchNorm statistics of Y          MODE 2: Y = X.W^T + R
 // MODE 3: dz = mask ? X.W^T + R : 0, + BatchNorm backward reduction against bn_x (tm_b), coef, mask
+// MODE 4: Y = act(X.W^T * s + t)                                           MODE 5: Y = act(X.W^T * s + t + R)
+// (one body for both kernels; ev is read by MODES 4 / 5 only)
 template <int BN, int MODE, bool F32>
-__global__ void __launch_bounds__(kThreads, 1)
-c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w,
-               const __grid_constant__ CUtensorMap tm_y, const __grid_constant__ CUtensorMap tm_r,
-               const __grid_constant__ CUtensorMap tm_b, int M, int N, int K, float* __restrict__ partial,
-               const float* __restrict__ coef, const uint8_t* __restrict__ mask, const C1Plan plan)
+__device__ __forceinline__ void
+c1_gemm_body(const CUtensorMap& tm_x, const CUtensorMap& tm_w, const CUtensorMap& tm_y, const CUtensorMap& tm_r,
+             const CUtensorMap& tm_b, int M, int N, int K, float* __restrict__ partial,
+             const float* __restrict__ coef, const uint8_t* __restrict__ mask, const C1Plan& plan, const C1Eval& ev)
 {
     constexpr bool STATS = MODE == 1;
-    constexpr bool RES = MODE >= 2;
+    constexpr bool RES = MODE == 2 || MODE == 3 || MODE == 5;
     constexpr bool BNR = MODE == 3;
+    constexpr bool EVAL = MODE >= 4;
     constexpr int BK = Elt<F32>::BK;
     constexpr int MMA_K = Elt<F32>::MMA_K;
     constexpr int COLS = Elt<F32>::COLS;
@@ -367,13 +380,13 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
     const int nbuf = plan.nbuf;
 
     // [ resident W : k_blocks x B_BYTES ][ ring : stages x (X tile [+ W tile]) ][ store slabs ]
-    // [ MODE 3: bn_x slabs, 8 warps x 2 ][ barriers ]
+    // [ MODE 3: bn_x slabs, 8 warps x 2 | MODES 4 / 5: (s, t) of the BN columns ][ barriers ]
     uint8_t* sW = smem;
     uint8_t* ring = sW + (resident ? k_blocks * B_BYTES : 0);
     const int stage_bytes = A_BYTES + (resident ? 0 : B_BYTES);
     uint8_t* sO = ring + stages * stage_bytes;
     uint8_t* sB = sO + 8 * nbuf * SLAB_BYTES;
-    uint64_t* full = reinterpret_cast<uint64_t*>(sB + (BNR ? 16 * SLAB_BYTES : 0));
+    uint64_t* full = reinterpret_cast<uint64_t*>(sB + (BNR ? 16 * SLAB_BYTES : 0) + (EVAL ? BN * 8 : 0));
     uint64_t* empty = full + MAX_STAGES;
     uint64_t* wfull = empty + MAX_STAGES;    // resident W landed
     uint64_t* rbar0 = wfull + 1;             // MODE 2: residual slab landed, [8 warps][2 slots]
@@ -387,6 +400,15 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         if (RES) { tma_prefetch_desc(&tm_r); for (int i = 0; i < 16; ++i) mbar_init(&rbar0[i], 1); }
         if (BNR) tma_prefetch_desc(&tm_b);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    if (EVAL) {
+        // the CTA's channel block never changes: (s, t) once per launch, from the live tensors
+        float2* st = reinterpret_cast<float2*>(sB);
+        for (int c = (int)threadIdx.x; c < BN; c += kThreads) {
+            const int ch = nb * BN + c;
+            const float sc = __ldg(ev.gamma + ch) * rsqrtf(__ldg(ev.var + ch) + ev.eps);
+            st[c] = make_float2(sc, fmaf(-__ldg(ev.mean + ch), sc, __ldg(ev.beta + ch)));
+        }
     }
     __syncthreads();
 
@@ -540,14 +562,25 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
                         // MODE 3 keep bits of d[0..3] (c is a compile-time index)
                         const uint32_t msh = (uint32_t)(8 * (c & 3) + 2 * (lane & 3));
                         const uint32_t mlo = mk[0][c >> 2] >> msh, mhi = mk[1][c >> 2] >> msh;
+                        float4 st = make_float4(0.f, 0.f, 0.f, 0.f);   // MODES 4 / 5: (s, t) of both columns
+                        if (EVAL)
+                            st = *reinterpret_cast<const float4*>(sB + 8 * (s * COLS + 8 * c + 2 * (lane & 3)));
                         if (F32) {
                             float v0 = d[0], v1 = d[1], v2 = d[2], v3 = d[3];
+                            if (EVAL) {
+                                v0 = fmaf(v0, st.x, st.y); v1 = fmaf(v1, st.z, st.w);
+                                v2 = fmaf(v2, st.x, st.y); v3 = fmaf(v3, st.z, st.w);
+                            }
                             if (RES) {
                                 float a0, a1, a2, a3;
                                 asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(a0), "=f"(a1) : "r"(addr) : "memory");
                                 asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(a2), "=f"(a3) : "r"(addr + 1024u)
                                              : "memory");
                                 v0 += a0; v1 += a1; v2 += a2; v3 += a3;
+                            }
+                            if (EVAL && ev.relu) {                 // (a NaN stays NaN, as in torch.relu)
+                                v0 = v0 < 0.f ? 0.f : v0; v1 = v1 < 0.f ? 0.f : v1;
+                                v2 = v2 < 0.f ? 0.f : v2; v3 = v3 < 0.f ? 0.f : v3;
                             }
                             if (BNR) {
                                 v0 = (mlo & 1u) ? v0 : 0.f; v1 = (mlo & 2u) ? v1 : 0.f;
@@ -558,12 +591,20 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
                                          : "memory");
                         } else {
                             float v0 = d[0], v1 = d[1], v2 = d[2], v3 = d[3];
+                            if (EVAL) {
+                                v0 = fmaf(v0, st.x, st.y); v1 = fmaf(v1, st.z, st.w);
+                                v2 = fmaf(v2, st.x, st.y); v3 = fmaf(v3, st.z, st.w);
+                            }
                             if (RES) {
                                 uint32_t a, b;
                                 asm volatile("ld.shared.b32 %0, [%1];" : "=r"(a) : "r"(addr) : "memory");
                                 asm volatile("ld.shared.b32 %0, [%1];" : "=r"(b) : "r"(addr + 1024u) : "memory");
                                 v0 += __uint_as_float(a << 16); v1 += __uint_as_float(a & 0xFFFF0000u);
                                 v2 += __uint_as_float(b << 16); v3 += __uint_as_float(b & 0xFFFF0000u);
+                            }
+                            if (EVAL && ev.relu) {
+                                v0 = v0 < 0.f ? 0.f : v0; v1 = v1 < 0.f ? 0.f : v1;
+                                v2 = v2 < 0.f ? 0.f : v2; v3 = v3 < 0.f ? 0.f : v3;
                             }
                             if (BNR) {
                                 v0 = (mlo & 1u) ? v0 : 0.f; v1 = (mlo & 2u) ? v1 : 0.f;
@@ -741,6 +782,28 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
         }
         if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
     }
+}
+
+template <int BN, int MODE, bool F32>
+__global__ void __launch_bounds__(kThreads, 1)
+c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w,
+               const __grid_constant__ CUtensorMap tm_y, const __grid_constant__ CUtensorMap tm_r,
+               const __grid_constant__ CUtensorMap tm_b, int M, int N, int K, float* __restrict__ partial,
+               const float* __restrict__ coef, const uint8_t* __restrict__ mask, const C1Plan plan)
+{
+    static_assert(MODE >= 0 && MODE <= 3, "MODES 4 / 5 are c1_gemm_eval_kernel");
+    c1_gemm_body<BN, MODE, F32>(tm_x, tm_w, tm_y, tm_r, tm_b, M, N, K, partial, coef, mask, plan, C1Eval{});
+}
+
+// MODE 4 (no residual) / MODE 5 (+ R through tm_r, as MODE 2): the eval-mode conv + BatchNorm (+ R) (+ ReLU)
+template <int BN, int MODE, bool F32>
+__global__ void __launch_bounds__(kThreads, 1)
+c1_gemm_eval_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w,
+                    const __grid_constant__ CUtensorMap tm_y, const __grid_constant__ CUtensorMap tm_r, int M, int N,
+                    int K, const C1Plan plan, const C1Eval ev)
+{
+    static_assert(MODE == 4 || MODE == 5, "eval modes only");
+    c1_gemm_body<BN, MODE, F32>(tm_x, tm_w, tm_y, tm_r, tm_r, M, N, K, nullptr, nullptr, nullptr, plan, ev);
 }
 
 // ---------------------------------------------------------------------------
@@ -942,13 +1005,15 @@ void grid_shape(long long M, int N, int K, int num_sms, bool f32, bool bn_reduce
 
 // Shared-memory plan.  W stays resident when the CTA's [BN, K] block plus a >= 3-deep X ring
 // fits (then every row tile costs one 16 KB X load instead of X + W); the store slabs shrink
-// from 2 to 1 per warp if that is what makes it fit.  MODE 3 adds 8 x 2 bn_x slabs.
-C1Plan make_plan(int bn, int K, int n_blocks, bool residual, bool bn_reduce, bool f32, int& smem_bytes)
+// from 2 to 1 per warp if that is what makes it fit.  MODE 3 adds 8 x 2 bn_x slabs, MODES 4 / 5 (eval_bn)
+// the BN x 8 bytes of (s, t).
+C1Plan make_plan(int bn, int K, int n_blocks, bool residual, bool bn_reduce, bool f32, int& smem_bytes,
+                 bool eval_bn = false)
 {
     const int bk = f32 ? Elt<true>::BK : Elt<false>::BK;
     const int k_blocks = (K + bk - 1) / bk;
     const int b_bytes = bn * ROW_BYTES;
-    const int extra = bn_reduce ? 16 * SLAB_BYTES : 0;
+    const int extra = bn_reduce ? 16 * SLAB_BYTES : eval_bn ? bn * 8 : 0;
     residual = residual || bn_reduce;
     C1Plan p;
     p.x_hint_first = n_blocks == 1;
@@ -989,6 +1054,26 @@ cudaError_t launch(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorM
     const C1Plan plan = make_plan(BN, K, N / BN, mode == 2, mode == 3, F32, smem);
     if (plan.stages < 2) return cudaErrorInvalidValue;
     kern<<<grid, kThreads, smem, st>>>(tx, tw, ty, tr, tb, M, N, K, partial, coef, mask, plan);
+    return cudaGetLastError();
+}
+
+template <int BN, bool F32>
+cudaError_t launch_eval(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap& ty, const CUtensorMap& tr,
+                        int M, int N, int K, bool residual, const C1Eval& ev, int grid, cudaStream_t st)
+{
+    auto kern = residual ? c1_gemm_eval_kernel<BN, 5, F32> : c1_gemm_eval_kernel<BN, 4, F32>;
+    static bool configured[2][64] = {};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev < 0 || dev >= 64 || !configured[residual][dev]) {
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
+        if (e != cudaSuccess) return e;
+        if (dev >= 0 && dev < 64) configured[residual][dev] = true;
+    }
+    int smem = 0;
+    const C1Plan plan = make_plan(BN, K, N / BN, residual, false, F32, smem, true);
+    if (plan.stages < 2) return cudaErrorInvalidValue;
+    kern<<<grid, kThreads, smem, st>>>(tx, tw, ty, tr, M, N, K, plan, ev);
     return cudaGetLastError();
 }
 
@@ -1054,6 +1139,37 @@ cudaError_t c1_launch_gemm(const void* x, const void* w, void* y, long long M, i
     case 256: return launch<256, false>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st);
     case 128: return launch<128, false>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st);
     default: return launch<64, false>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st);
+    }
+}
+
+// eval-mode conv + BatchNorm: y = act(x . w^T * s + t [+ residual]), s = gamma * rsqrt(var + eps),
+// t = beta - mean * s per output channel, computed by each CTA from the live fp32 [N] tensors at every
+// launch (a captured graph follows in-place parameter swaps).  Same plan and grid as MODE 0 / MODE 2.
+cudaError_t c1_launch_gemm_bn_eval(const void* x, const void* w, void* y, long long M, int N, int K,
+                                   const void* residual, const float* gamma, const float* beta, const float* mean,
+                                   const float* var, float eps, int relu, int num_sms, int f32, cudaStream_t st)
+{
+    if (!c1_supported(M, N, K, f32)) return cudaErrorInvalidValue;
+    const bool f = f32 != 0;
+    int bn, per, grid;
+    grid_shape(M, N, K, num_sms, f, false, bn, per, grid);
+    CUtensorMap tx, tw, ty, tr;
+    if (!make_map(&tx, x, M, K, BM, true, f) || !make_map(&tw, w, N, K, bn, true, f) ||
+        !make_map(&ty, y, M, N, 16, false, f) || !make_map(&tr, residual ? residual : y, M, N, 16, false, f))
+        return cudaErrorInvalidValue;
+    const C1Eval ev{gamma, beta, mean, var, eps, relu ? 1 : 0};
+    const bool r = residual != nullptr;
+    if (f) {
+        switch (bn) {
+        case 256: return launch_eval<256, true>(tx, tw, ty, tr, (int)M, N, K, r, ev, grid, st);
+        case 128: return launch_eval<128, true>(tx, tw, ty, tr, (int)M, N, K, r, ev, grid, st);
+        default: return launch_eval<64, true>(tx, tw, ty, tr, (int)M, N, K, r, ev, grid, st);
+        }
+    }
+    switch (bn) {
+    case 256: return launch_eval<256, false>(tx, tw, ty, tr, (int)M, N, K, r, ev, grid, st);
+    case 128: return launch_eval<128, false>(tx, tw, ty, tr, (int)M, N, K, r, ev, grid, st);
+    default: return launch_eval<64, false>(tx, tw, ty, tr, (int)M, N, K, r, ev, grid, st);
     }
 }
 

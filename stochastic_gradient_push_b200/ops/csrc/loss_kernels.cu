@@ -58,6 +58,29 @@ __device__ __forceinline__ float warp_sum(float v)
     return v;
 }
 
+// One warp over row z (lane-strided): lse = log sum_j exp(z_j) by the online softmax, above = #{ j : z_j > zt }
+// (the row's rank: top-k hit <=> above < k) and, with SMOOTH, sum_j z_j -- each logit read once.  Shared by
+// the training forward and the evaluation accumulate kernel, so both count hits the same way.
+template <typename T, bool SMOOTH>
+__device__ __forceinline__ void xent_row_scan(const T* z, int C, float zt, int lane, float& lse, float& above,
+                                              float& sum_z)
+{
+    float m = -INFINITY, s = 0.f, ab = 0.f, sz = 0.f;
+    for (int j = lane; j < C; j += 32) {
+        const float v = to_f<T>(z[j]);
+        const float mn = fmaxf(m, v);
+        s = s * __expf(m - mn) + __expf(v - mn);
+        m = mn;
+        ab += (v > zt) ? 1.f : 0.f;
+        if (SMOOTH) sz += v;
+    }
+    const float mw = warp_max(m);
+    s = warp_sum(s * __expf(m - mw));
+    above = warp_sum(ab);
+    sum_z = SMOOTH ? warp_sum(sz) : sz;
+    lse = mw + __logf(s);
+}
+
 template <typename T, bool SMOOTH, bool MIX>
 __global__ void __launch_bounds__(XE_THREADS)
 xent_fwd_kernel(const T* __restrict__ logits, const long long* __restrict__ target, float* __restrict__ lse_out,
@@ -83,20 +106,8 @@ xent_fwd_kernel(const T* __restrict__ logits, const long long* __restrict__ targ
             zb = to_f<T>(z[tb]);
         }
         // online softmax: one pass for max + sum, rank counted in the same pass
-        float m = -INFINITY, s = 0.f, above = 0.f, sum_z = 0.f;
-        for (int j = lane; j < C; j += 32) {
-            const float v = to_f<T>(z[j]);
-            const float mn = fmaxf(m, v);
-            s = s * __expf(m - mn) + __expf(v - mn);
-            m = mn;
-            above += (v > zt) ? 1.f : 0.f;
-            if (SMOOTH) sum_z += v;
-        }
-        const float mw = warp_max(m);
-        s = warp_sum(s * __expf(m - mw));
-        above = warp_sum(above);
-        if (SMOOTH) sum_z = warp_sum(sum_z);
-        const float lse = mw + __logf(s);
+        float lse, above, sum_z;
+        xent_row_scan<T, SMOOTH>(z, C, zt, lane, lse, above, sum_z);
         if (lane == 0) {
             lse_out[row] = lse;
             if (valid) {
@@ -117,6 +128,41 @@ xent_fwd_kernel(const T* __restrict__ logits, const long long* __restrict__ targ
     }
     __syncthreads();
     if (threadIdx.x < 3) atomicAdd(out3 + threadIdx.x, s_acc[threadIdx.x]);
+}
+
+// Evaluation: plain cross-entropy, forward only, summed over batches into a persistent device accumulator
+// acc = [loss sum (fp64 bits), top-1 hits, top-5 hits, valid rows].  A row whose target is outside [0, C)
+// adds to none of the four.  No lse is stored.
+template <typename T>
+__global__ void __launch_bounds__(XE_THREADS)
+xent_eval_kernel(const T* __restrict__ logits, const long long* __restrict__ target,
+                 unsigned long long* __restrict__ acc, int B, int C)
+{
+    __shared__ double s_loss;
+    __shared__ unsigned int s_cnt[3];
+    if (threadIdx.x == 0) s_loss = 0.0;
+    if (threadIdx.x < 3) s_cnt[threadIdx.x] = 0u;
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    const int row = blockIdx.x * (XE_THREADS / 32) + (threadIdx.x >> 5);
+    if (row < B) {
+        const long long t = target[row];
+        if (t >= 0 && t < C) {                              // (warp-uniform)
+            const T* z = logits + (size_t)row * C;
+            const float zt = to_f<T>(z[t]);
+            float lse, above, sum_z;
+            xent_row_scan<T, false>(z, C, zt, lane, lse, above, sum_z);
+            if (lane == 0) {
+                atomicAdd(&s_loss, (double)(lse - zt));
+                if (above < 0.5f) atomicAdd(&s_cnt[0], 1u);
+                if (above < 4.5f) atomicAdd(&s_cnt[1], 1u);
+                atomicAdd(&s_cnt[2], 1u);
+            }
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0 && s_cnt[2] != 0u) atomicAdd(reinterpret_cast<double*>(acc), s_loss);
+    if (threadIdx.x < 3 && s_cnt[threadIdx.x] != 0u) atomicAdd(acc + 1 + threadIdx.x, (unsigned long long)s_cnt[threadIdx.x]);
 }
 
 template <typename T, bool SMOOTH, bool MIX>
@@ -180,6 +226,18 @@ cudaError_t xent_launch_fwd(int dtype, const void* logits, const long long* targ
                      : (smooth ? xent_fwd_kernel<float, true, false> : xent_fwd_kernel<float, false, false>);
         k<<<grid, XE_THREADS, 0, st>>>((const float*)logits, target, lse, out3, B, C, eps, mix);
     }
+    return cudaGetLastError();
+}
+
+// acc: [4] 8-byte device words, see xent_eval_kernel; B >= 1
+cudaError_t xent_launch_eval(int dtype, const void* logits, const long long* target, unsigned long long* acc, int B,
+                             int C, cudaStream_t st)
+{
+    const int grid = (B + XE_THREADS / 32 - 1) / (XE_THREADS / 32);
+    if (dtype == 0)
+        xent_eval_kernel<__nv_bfloat16><<<grid, XE_THREADS, 0, st>>>((const __nv_bfloat16*)logits, target, acc, B, C);
+    else
+        xent_eval_kernel<float><<<grid, XE_THREADS, 0, st>>>((const float*)logits, target, acc, B, C);
     return cudaGetLastError();
 }
 

@@ -68,6 +68,25 @@ def bn_f32_map(split: bool):
         C.bn_f32_map(prev)
 
 
+# set by eval_bn_gemm(): eval-mode conv_bn_act calls the GEMM with BatchNorm in its epilogue
+_EVAL_GEMM = [False]
+
+
+@contextlib.contextmanager
+def eval_bn_gemm():
+    """Inside the block, ``conv_bn_act`` with an eval-mode BatchNorm and gradients disabled runs every
+    1x1 / stride-1 convolution the GEMM covers as ONE launch: the GEMM with the BatchNorm affine map of
+    the running statistics, the residual add and the ReLU in its epilogue (``C.conv1x1_bn_eval``)
+    instead of the library convolution and a separate BatchNorm pass.  Outside it an eval forward runs
+    as before, bit for bit.  ``GossipTrainer.evaluate`` uses it."""
+    prev = _EVAL_GEMM[0]
+    _EVAL_GEMM[0] = True
+    try:
+        yield
+    finally:
+        _EVAL_GEMM[0] = prev
+
+
 def _can_fuse(x: torch.Tensor) -> bool:
     if FORCE_REFERENCE or not x.is_cuda or not native.available():
         return False
@@ -274,7 +293,8 @@ class _Conv1x1BNActSplit(torch.autograd.Function):
 def _conv1x1_operands(conv, bn, x, residual, relu):
     """(x, fusable): x possibly cast the way autocast would; fusable says whether the wgmma
     conv + BN path covers this call."""
-    if not (USE_TCGEN05_CONV1X1 and not FORCE_REFERENCE and bn.training and bn.track_running_stats
+    train_or_eval = bn.training or (_EVAL_GEMM[0] and not torch.is_grad_enabled())
+    if not (USE_TCGEN05_CONV1X1 and not FORCE_REFERENCE and train_or_eval and bn.track_running_stats
             and x.is_cuda and native.available() and x.dim() == 4
             and conv.kernel_size == (1, 1) and conv.stride == (1, 1) and conv.padding == (0, 0)
             and conv.groups == 1 and conv.bias is None and bn.weight is not None
@@ -299,8 +319,13 @@ def _conv1x1_operands(conv, bn, x, residual, relu):
 
 def conv_bn_act(conv: nn.Conv2d, bn: 'FusedBatchNormAct2d', x, residual=None, relu=False):
     """``bn(conv(x), residual=residual, relu=relu)``; 1x1 / stride-1 convolutions of NHWC bf16
-    activations in training mode take the fused wgmma path."""
+    activations in training mode take the fused wgmma path, and so do eval-mode ones inside
+    :func:`eval_bn_gemm`."""
     xk, ok = _conv1x1_operands(conv, bn, x, residual, relu)
+    if ok and not bn.training:
+        w = conv.weight if conv.weight.dtype == xk.dtype else conv.weight.detach().to(xk.dtype)
+        return native.load().conv1x1_bn_eval(xk, w, bn.weight, bn.bias, bn.running_mean, bn.running_var,
+                                             bn.eps, relu, residual)
     if ok:
         momentum = 0.1 if bn.momentum is None else bn.momentum
         return _Conv1x1BNAct.apply(xk, conv.weight, residual, bn.weight, bn.bias, bn.running_mean,

@@ -99,6 +99,25 @@ def fused_cross_entropy(logits: torch.Tensor, target: torch.Tensor, label_smooth
     return loss, torch.stack([loss.detach().float(), p1, p5])
 
 
+def eval_accumulator(device) -> torch.Tensor:
+    """a zeroed evaluation accumulator for :func:`eval_accumulate`: int64 ``[4]`` on ``device`` =
+    ``[loss sum (fp64 bits: acc[:1].view(torch.float64)), top-1 hits, top-5 hits, counted rows]``"""
+    return torch.zeros(4, dtype=torch.int64, device=device)
+
+
+def eval_accumulate(logits: torch.Tensor, target: torch.Tensor, acc: torch.Tensor) -> None:
+    """Adds this batch's plain cross-entropy sum (fp64) and top-1 / top-5 / row counts to ``acc``
+    (:func:`eval_accumulator`) in one launch of the forward kernel's row scan: no per-row loss is
+    stored and nothing is read back.  Rows whose target is outside ``[0, C)`` are not counted.  A logit
+    tied with the target's counts as ranked below it.  CUDA fp32 / bf16 logits only."""
+    lg = logits if logits.is_contiguous() else logits.contiguous()
+    C = native.load()
+    if not C.xent_can_fuse(lg, target):
+        raise ValueError('eval_accumulate needs 2-d fp32 / bf16 CUDA logits and int64 CUDA targets, got %s %s '
+                         'and %s %s' % (tuple(logits.shape), logits.dtype, tuple(target.shape), target.dtype))
+    C.xent_eval_accumulate(lg, target, acc)
+
+
 class FusedCrossEntropyWithAccuracy(nn.Module):
     """Drop-in for ``nn.CrossEntropyLoss(label_smoothing=label_smoothing)`` (mean reduction) that
     also measures accuracy."""

@@ -639,6 +639,10 @@ def make_bilat_trainer(model: BilatGossipDataParallel, lr, criterion=None, amp_d
             torch.cuda.synchronize(self.device)
             self.model._check()
 
+        def evaluate(self, batches):
+            raise ValueError('evaluate() is not supported with AD-PSGD: its gossip daemon rewrites the '
+                             'parameters asynchronously, so a captured evaluation would not see one model')
+
         def check(self):
             self.model._check()
 

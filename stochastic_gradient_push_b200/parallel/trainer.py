@@ -42,18 +42,27 @@ BatchNorm running statistics are updated k times per step (momentum applied each
 ``num_batches_tracked`` grows by k; the metrics row is the mean of the k micro-batches' ``[loss,
 prec@1, prec@5]``; ``static_out`` holds the LAST micro-batch's logits.  With ``batch_mix`` one draw
 serves the step and each micro-batch is mixed with its own flipped micro-batch.
+
+Evaluation (``evaluate(batches)``): the same network and precision as the step (the bf16 twin, else the
+module under the trainer's autocast) in eval mode, one captured graph per batch shape: the forward, with
+every 1x1 / stride-1 convolution and its BatchNorm (+ residual) (+ ReLU) as one GEMM launch
+(``ops.fused_bn.eval_bn_gemm``), and one ``xent_eval_accumulate`` launch that adds the batch's loss sum
+and top-1 / top-5 / row counts to a device accumulator, read back once at the end.  Nothing the
+training step owns is touched.
 """
 
 from __future__ import annotations
 
 import contextlib
+import math
 import numbers
 import os
-from typing import Callable, Optional
+from typing import Callable, NamedTuple, Optional
 
 import torch
 
-from ..ops.fused_loss import FusedCrossEntropyWithAccuracy
+from ..ops.fused_bn import eval_bn_gemm
+from ..ops.fused_loss import FusedCrossEntropyWithAccuracy, eval_accumulate, eval_accumulator
 from ..optim import FusedGossipSGD
 from .distributed import GossipDataParallel
 
@@ -63,6 +72,28 @@ def check_accumulation_steps(k) -> int:
     if isinstance(k, bool) or not isinstance(k, numbers.Integral) or k < 1:
         raise ValueError('accumulation_steps must be an integer >= 1, got %r' % (k,))
     return int(k)
+
+
+class EvalResult(NamedTuple):
+    """What :meth:`GossipTrainer.evaluate` measured over the rows whose target is in ``[0, classes)``:
+    the mean plain cross-entropy, prec@1 and prec@5 in percent, and the number of such rows."""
+    loss: float
+    prec1: float
+    prec5: float
+    count: int
+
+    @classmethod
+    def from_sums(cls, loss_sum: float, top1: int, top5: int, count: int) -> 'EvalResult':
+        """from the accumulated sums; NaN means (and a count of 0) when no row was counted"""
+        count = int(count)
+        if count <= 0:
+            return cls(math.nan, math.nan, math.nan, 0)
+        return cls(float(loss_sum) / count, 100.0 * int(top1) / count, 100.0 * int(top5) / count, count)
+
+
+class _EvalSlot(object):
+    """per evaluation batch shape: staging and static buffers, and the captured graph"""
+    __slots__ = ('stage', 'stage_tgt', 'static_in', 'static_tgt', 'ready', 'free', 'graph', 'out')
 
 
 class GossipTrainer(object):
@@ -152,6 +183,10 @@ class GossipTrainer(object):
         self.own_launches_per_step = None
         self._graphs = {}               # overlap + DMA gather: one captured graph per (row, parity)
         self._pool = None
+        self._eval_slots = {}           # evaluate(): one _EvalSlot (and graph) per batch shape
+        self._eval_acc = None
+        self.eval_out = None            # logits of the last batch of the last evaluate()
+        self.eval_launches_per_batch = None
 
     # ------------------------------------------------------------------ #
     def _autocast(self):
@@ -515,3 +550,122 @@ class GossipTrainer(object):
     def check(self):
         """Raise if a gossip kernel reported a heartbeat / ack timeout (reads one word)."""
         self.engine.check()
+
+    # ------------------------------------------------------------------ #
+    def evaluate(self, batches) -> EvalResult:
+        """Validation of the current model over ``batches`` (an iterable of ``(input, target)``, (pinned)
+        host or device tensors; a loader).  Drains the trainer first (:meth:`finish`), then runs the step's
+        network in eval mode -- BatchNorm with its running statistics -- and restores the previous mode.
+        Loss is the plain cross-entropy (no smoothing, no mixing); rows whose target is outside
+        ``[0, classes)`` are not counted.  The H2D copy of batch i+1 overlaps batch i; each batch shape
+        is captured once (in the trainer's graph pool) and replayed on later calls, so this works inside
+        ``ModelEma.applied()`` and ``GossipDataParallel.averaged()``, which swap values in place.
+        Parameters, momentum, BatchNorm statistics, the engine's step counter, the metrics ring, the
+        training buffers and graphs, the EMA and the batch-mix iteration are left as they were.
+        ``eval_out``: the last batch's logits; ``eval_launches_per_batch``: our kernels per batch."""
+        self.finish()
+        twin = getattr(self.model, '_twin', None)
+        net = twin[0] if twin else self.model.module
+        modules = [self.model.module] + ([net] if twin else [])
+        modes = [m.training for m in modules]
+        main = torch.cuda.current_stream(self.device)
+        if self._eval_acc is None:
+            self._eval_acc = eval_accumulator(self.device)
+        self.stream.wait_stream(main)            # (in-place swaps by ema.applied() / averaged() on main)
+        with torch.cuda.stream(self.stream):
+            self._eval_acc.zero_()
+        out = None
+        try:
+            for m in modules:
+                m.eval()
+            with torch.no_grad():
+                it = iter(batches)
+                nxt = next(it, None)
+                slot = self._eval_prefetch(*nxt) if nxt is not None else None
+                while slot is not None:
+                    self._eval_load(slot)
+                    nxt = next(it, None)
+                    cur, slot = slot, (self._eval_prefetch(*nxt) if nxt is not None else None)
+                    out = self._eval_run(cur, net)
+        finally:
+            for m, mode in zip(modules, modes):
+                m.train(mode)
+        with torch.cuda.stream(self.stream):
+            if out is not None:
+                self.eval_out = out.clone()
+            acc = self._eval_acc.cpu()           # the one read-back (synchronises the stream)
+        main.wait_stream(self.stream)
+        return EvalResult.from_sums(float(acc[:1].view(torch.float64)), int(acc[1]), int(acc[2]), int(acc[3]))
+
+    def _eval_prefetch(self, batch, target) -> _EvalSlot:
+        """start the H2D copy of an evaluation batch into its shape's staging buffers (copy stream)"""
+        key = (tuple(batch.shape), batch.dtype, tuple(target.shape), target.dtype)
+        slot = self._eval_slots.get(key)
+        if slot is None:
+            slot = self._eval_slots[key] = _EvalSlot()
+            fmt = torch.channels_last if (self.channels_last and batch.dim() == 4) else torch.contiguous_format
+            in_dtype = torch.bfloat16 if getattr(self.model, '_twin', None) else batch.dtype
+            slot.static_in = torch.empty(batch.shape, dtype=in_dtype, device=self.device
+                                         ).contiguous(memory_format=fmt)
+            slot.static_tgt = torch.empty(target.shape, dtype=target.dtype, device=self.device)
+            slot.stage = torch.empty(batch.shape, dtype=batch.dtype, device=self.device)
+            slot.stage_tgt = torch.empty_like(slot.static_tgt)
+            slot.ready, slot.free = torch.cuda.Event(), torch.cuda.Event()
+            slot.graph = slot.out = None
+            slot.free.record(self.stream)
+        cs = self._copy_stream
+        cs.wait_event(slot.free)
+        on_device = [t for t in (batch, target) if t.is_cuda]
+        if on_device:
+            cs.wait_stream(torch.cuda.current_stream(self.device))
+            for t in on_device:
+                t.record_stream(cs)
+        with torch.cuda.stream(cs):
+            slot.stage.copy_(batch, non_blocking=True)
+            slot.stage_tgt.copy_(target, non_blocking=True)
+            slot.ready.record(cs)
+        return slot
+
+    def _eval_load(self, slot: _EvalSlot):
+        self.stream.wait_event(slot.ready)
+        with torch.cuda.stream(self.stream):
+            slot.static_in.copy_(slot.stage, non_blocking=True)
+            slot.static_tgt.copy_(slot.stage_tgt, non_blocking=True)
+            slot.free.record(self.stream)
+
+    def _eval_autocast(self):
+        """the step's precision: the bf16 twin runs without autocast, the module under the trainer's"""
+        return contextlib.nullcontext() if getattr(self.model, '_twin', None) else self._autocast()
+
+    def _eval_forward(self, slot: _EvalSlot, net):
+        """forward + accumulate of one batch on the trainer's stream (captured or eager)"""
+        with eval_bn_gemm(), self._eval_autocast():
+            out = net(slot.static_in)
+        eval_accumulate(out, slot.static_tgt, self._eval_acc)
+        return out
+
+    def _eval_run(self, slot: _EvalSlot, net):
+        C = self.engine.C
+        with torch.cuda.stream(self.stream):
+            if not self.use_graph:
+                c0 = C.launch_count()
+                out = self._eval_forward(slot, net)
+                self.eval_launches_per_batch = C.launch_count() - c0
+                return out
+            if slot.graph is None:
+                # warm-up forward outside the capture (library algorithm choice, lazy initialisation);
+                # eval mode writes no state, and the accumulator is not touched
+                with eval_bn_gemm(), self._eval_autocast():
+                    net(slot.static_in)
+                torch.cuda.synchronize(self.device)
+                if self._pool is None:
+                    self._pool = torch.cuda.graph_pool_handle()
+                graph = torch.cuda.CUDAGraph()
+                c0 = C.launch_count()
+                with torch.cuda.graph(graph, stream=self.stream, capture_error_mode='thread_local',
+                                      pool=self._pool):
+                    slot.out = self._eval_forward(slot, net)
+                self.eval_launches_per_batch = C.launch_count() - c0
+                slot.graph = graph
+            slot.graph.replay()
+            return slot.out

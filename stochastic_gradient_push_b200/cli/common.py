@@ -403,6 +403,25 @@ def check_eval_graph_flags(args):
                          '--fused True on the CUDA kernel transport) for SGP, OSGP and D-PSGD' % unsupported)
 
 
+def check_precise_bn_flags(args):
+    """ValueError for --precise_bn_batches < 0, and for N > 0 outside the captured fused gossip step
+    (GossipTrainer), whose ``update_bn()`` it calls."""
+    n = getattr(args, 'precise_bn_batches', 0)
+    if n < 0:
+        raise ValueError('--precise_bn_batches must be >= 0, got %r' % (n,))
+    if n == 0:
+        return
+    unsupported = ('--all_reduce' if args.all_reduce else
+                   '--fused False' if not args.fused else
+                   '--cuda_graph False' if not args.cuda_graph else
+                   '--transport c10d' if args.transport == 'c10d' else
+                   '--device cpu' if args.device == 'cpu' else None)
+    if unsupported:
+        raise ValueError('--precise_bn_batches is not supported with %s: the statistics are recomputed by '
+                         'GossipTrainer.update_bn, which needs the captured fused gossip step (--cuda_graph True '
+                         '--fused True on the CUDA kernel transport) for SGP, OSGP and D-PSGD' % unsupported)
+
+
 def check_accumulation_flags(args):
     """ValueError for --accumulation_steps < 1, for K > 1 outside the captured fused gossip step
     (GossipTrainer), and for a --batch_size that K does not divide."""

@@ -21,6 +21,7 @@ syncs per iteration, optional whole-step CUDA graph (``--cuda_graph True``).
 
 from __future__ import annotations
 
+import itertools
 import os
 import socket
 import time
@@ -54,9 +55,17 @@ def parse_args(argv=None):
                              '1x1-conv GEMM epilogue, loss and top-1 / top-5 counted on the device and read back '
                              'once per pass.  Needs the captured trainer (--cuda_graph True --fused True on '
                              'the CUDA kernel transport, not --all_reduce)')
+    parser.add_argument('--precise_bn_batches', default=0, type=int,
+                        help='precise BatchNorm statistics: before each validation (the rank model, the '
+                             '--model_ema_decay EMA and the --validate_average average model) set every running '
+                             'mean / variance to the average of the batch statistics of the next N training '
+                             'batches (augmented, never mixed), through GossipTrainer.update_bn.  0 = off.  '
+                             'Needs the captured trainer (--cuda_graph True --fused True on the CUDA kernel '
+                             'transport, not --all_reduce)')
     args = parser.parse_args(argv)
     common.check_accumulation_flags(args)
     common.check_eval_graph_flags(args)
+    common.check_precise_bn_flags(args)
     return finalize_args(args, adpsgd=False)
 
 
@@ -166,6 +175,10 @@ def main(argv=None):
         raise ValueError('--eval_graph is not supported with transport %s: the captured evaluation is '
                          'GossipTrainer.evaluate, which runs on the CUDA kernel transport only'
                          % getattr(model, 'transport', 'c10d'))
+    if args.precise_bn_batches > 0 and args._trainer is None:
+        raise ValueError('--precise_bn_batches is not supported with transport %s: the statistics are recomputed '
+                         'by GossipTrainer.update_bn, which runs on the CUDA kernel transport only'
+                         % getattr(model, 'transport', 'c10d'))
     if args.accumulation_steps > 1 and args._trainer is None:
         raise ValueError('--accumulation_steps > 1 needs the captured GossipTrainer step, which runs on the '
                          'CUDA kernel transport only (got device %s, transport %s)' % (args.device, model.transport))
@@ -219,6 +232,7 @@ def main(argv=None):
               epoch, start_itr, csv, log)
         start_itr = 0
         if not args.train_fast:
+            precise_bn(args, loader, log)          # (before the state is taken: checkpointed that way)
             elapsed_time = time.time() - begin_time
             update_state(state, {
                 'epoch': epoch + 1, 'itr': 0, 'is_best': False,
@@ -230,22 +244,23 @@ def main(argv=None):
             prec1 = validate(args, val_loader, model, criterion, log)
             csv.val_row(epoch, batch_meter, nn_meter, data_meter, prec1)
             if args._ema is not None:
-                validate_ema(args, val_loader, model, criterion, log, epoch)
+                validate_ema(args, val_loader, model, criterion, log, epoch, loader)
             if prec1 > best_val_prec1:
                 update_state(state, {'is_best': True, 'best_prec1': prec1})
                 best_val_prec1 = prec1
         if args._consensus_log is not None:
-            epoch_end_consensus(args, model, criterion, val_loader, epoch, log)
+            epoch_end_consensus(args, model, criterion, val_loader, epoch, log, loader)
         if not args.train_fast:
             epoch_id = None if args.overwrite_checkpoints else epoch
             cmanager.save_checkpoint(epoch_id, requeue_on_signal=(epoch != args.num_epochs - 1))
 
     if args.train_fast:
         val_loader = make_dataloader(args, train=False)
+        precise_bn(args, loader, log)
         prec1 = validate(args, val_loader, model, criterion, log)
         log.info('Test accuracy: {}'.format(prec1))
         if args._ema is not None:
-            validate_ema(args, val_loader, model, criterion, log, args.num_epochs - 1)
+            validate_ema(args, val_loader, model, criterion, log, args.num_epochs - 1, loader)
     log.info('elapsed_time {0}'.format(time.time() - begin_time))
     if tracing.get_tracer().enabled:            # shorter run than --trace_iters
         log.info('trace written to %s' % tracing.disable().dump())
@@ -401,10 +416,30 @@ def log_consensus(args, stats, epoch, itr, log, avg_prec1=None):
     args._consensus_log.row(epoch, itr, stats, avg_prec1)
 
 
-def epoch_end_consensus(args, model, criterion, val_loader, epoch, log):
+def precise_bn(args, loader, log, label=''):
+    """--precise_bn_batches N > 0: recompute the BatchNorm running statistics of the model the trainer
+    runs now from the next N training batches (``GossipTrainer.update_bn``).  The batches come from a
+    fresh iterator over ``loader``, closed afterwards (a shard loader's gather thread ends), and carry
+    the training augmentation but are never mixed; they consume draws of the augmentation generator."""
+    n = getattr(args, 'precise_bn_batches', 0)
+    if n <= 0 or loader is None:
+        return
+    it = iter(loader)
+    try:
+        k = args._trainer.update_bn((common.device_batch(args, features, train=True), target)
+                                    for features, target in itertools.islice(it, n))
+    finally:
+        close = getattr(it, 'close', None)
+        if close is not None:
+            close()
+    log.info('precise BN: {}statistics from {} training batches'.format(label, k))
+
+
+def epoch_end_consensus(args, model, criterion, val_loader, epoch, log, loader=None):
     """Consensus distance at the end of an epoch; with ``--validate_average`` also the validation
     accuracy of the push-sum average model.  BatchNorm running statistics are not gossiped: for
-    that validation they are averaged over the ranks, and restored afterwards."""
+    that validation they are averaged over the ranks, and restored afterwards.  With
+    --precise_bn_batches each rank first recomputes them for the average model from ``loader``."""
     trainer = getattr(args, '_trainer', None)
     if trainer is not None:
         trainer.finish()
@@ -413,13 +448,22 @@ def epoch_end_consensus(args, model, criterion, val_loader, epoch, log):
         return
     bufs = [b for b in model.module.buffers() if b.is_floating_point()]
     saved = [b.detach().clone() for b in bufs]
-    if args.world_size > 1 and bufs:
-        with torch.no_grad():
-            communicate(bufs, dist.all_reduce)
-            for b in bufs:
-                b.div_(args.world_size)
+
+    def average_buffers():
+        if args.world_size > 1 and bufs:
+            with torch.no_grad():
+                communicate(bufs, dist.all_reduce)
+                for b in bufs:
+                    b.div_(args.world_size)
+
+    precise = getattr(args, 'precise_bn_batches', 0) > 0 and loader is not None
+    if not precise:
+        average_buffers()
     try:
         with model.averaged() as stats:
+            if precise:
+                precise_bn(args, loader, log, label='average-model ')
+                average_buffers()
             prec1 = validate(args, val_loader, model, criterion, log)
     finally:
         with torch.no_grad():
@@ -428,11 +472,13 @@ def epoch_end_consensus(args, model, criterion, val_loader, epoch, log):
     log_consensus(args, stats, epoch, -1, log, avg_prec1=prec1)
 
 
-def validate_ema(args, val_loader, model, criterion, log, epoch):
+def validate_ema(args, val_loader, model, criterion, log, epoch, loader=None):
     """Validate the EMA weights and BatchNorm statistics (``ModelEma.applied``, restored afterwards)
-    and log their prec@1 / prec@5 to stdout and the EMA CSV."""
+    and log their prec@1 / prec@5 to stdout and the EMA CSV.  With --precise_bn_batches the
+    statistics are first recomputed for the EMA weights from ``loader``."""
     ema = args._ema
     with ema.applied():
+        precise_bn(args, loader, log, label='EMA ')
         prec1, prec5 = evaluate(args, val_loader, model, criterion, log, label='EMA ')
     args._ema_log.row(epoch, ema.num_updates, prec1, prec5)
     return prec1

@@ -233,7 +233,7 @@ class ShardLoader(object):
                     q.get_nowait()
                 except queue.Empty:
                     break
-
+            t.join()                    # it puts at most one more batch into the drained queue, then sees stop
 
 # --------------------------------------------------------------------------- #
 # GPU-side augmentation

@@ -19,9 +19,11 @@ int bn_partial_rows_bwd(long long M, int C);
 int bn_f32_map(int value);
 cudaError_t bn_launch_stats(int dtype, const void* x, float* partial, long long M, int C, int G, cudaStream_t st);
 cudaError_t bn_launch_stats_finalize(const float* partial, int G, long long M, int C, const float* gamma,
-                                     const float* beta, float* rmean, float* rvar, long long* nbt,
+                                     const float* beta, float* rmean, float* rvar, long long* nbt, double* acc,
                                      float momentum, float eps, float* mean, float* invstd,
                                      float* scale, float* shift, cudaStream_t st);
+int bn_commit_max_segs();
+cudaError_t bn_launch_stats_commit(const long long* rows, int nseg, double k, cudaStream_t st);
 cudaError_t bn_launch_eval_coeff(int C, const float* gamma, const float* beta, const float* rmean,
                                  const float* rvar, float eps, float* scale, float* shift, cudaStream_t st);
 cudaError_t bn_launch_apply(int dtype, int relu, int add, const void* x, const void* res,
@@ -80,13 +82,26 @@ static bool bn_can_fuse(const torch::Tensor& x)
     return bn_supported(x.numel() / C, C) != 0;
 }
 
+// acc (training only): a contiguous fp64 [2C] tensor on x's device, or None.  Given, the finalize adds the
+// batch mean and unbiased variance to acc[0:C] and acc[C:2C] and leaves the running buffers and nbt alone
+// (precise BatchNorm statistics, ops/fused_bn.py precise_bn_stats)
+static double* bn_acc_ptr(const c10::optional<torch::Tensor>& acc, const torch::Tensor& x, int C)
+{
+    if (!acc.has_value() || !acc->defined()) return nullptr;
+    TORCH_CHECK(acc->is_cuda() && acc->get_device() == x.get_device() && acc->scalar_type() == torch::kFloat64 &&
+                    acc->is_contiguous() && acc->numel() == 2 * (int64_t)C,
+                "acc must be a contiguous fp64 [2C] tensor on x's device");
+    return acc->data_ptr<double>();
+}
+
 // returns (y, mean, invstd, scale, shift)
 static std::vector<torch::Tensor> bn_forward(torch::Tensor x, c10::optional<torch::Tensor> residual,
                                              torch::Tensor gamma, torch::Tensor beta,
                                              c10::optional<torch::Tensor> running_mean,
                                              c10::optional<torch::Tensor> running_var,
                                              c10::optional<torch::Tensor> num_batches_tracked,
-                                             bool training, double momentum, double eps, bool relu)
+                                             bool training, double momentum, double eps, bool relu,
+                                             c10::optional<torch::Tensor> acc)
 {
     long long M; int C;
     nhwc_dims(x, M, C);
@@ -103,6 +118,8 @@ static std::vector<torch::Tensor> bn_forward(torch::Tensor x, c10::optional<torc
     const bool has_res = residual.has_value() && residual->defined();
     if (has_res) TORCH_CHECK(residual->sizes() == x.sizes() && residual->scalar_type() == x.scalar_type()
                              && residual->strides() == x.strides());
+    double* accp = bn_acc_ptr(acc, x, C);
+    TORCH_CHECK(training || accp == nullptr, "bn_forward: acc needs training mode");
     if (training) {
         const int G = bn_partial_rows(M, C);
         auto partial = torch::empty({G + 1, 2, C}, fopt);   // last row carries the shift K
@@ -115,7 +132,7 @@ static std::vector<torch::Tensor> bn_forward(torch::Tensor x, c10::optional<torc
         if (num_batches_tracked.has_value() && num_batches_tracked->defined())
             nbt = reinterpret_cast<long long*>(num_batches_tracked->data_ptr<int64_t>());
         BN_CHECK(bn_launch_stats_finalize(partial.data_ptr<float>(), G, M, C, gamma.data_ptr<float>(),
-                                          beta.data_ptr<float>(), rm, rv, nbt, (float)momentum,
+                                          beta.data_ptr<float>(), rm, rv, nbt, accp, (float)momentum,
                                           (float)eps, mean, invstd, scale, shift, st));
     } else {
         TORCH_CHECK(running_mean.has_value() && running_var.has_value());
@@ -190,6 +207,46 @@ static std::vector<torch::Tensor> bn_backward_from_partials(torch::Tensor dz, to
     BN_CHECK(bn_launch_bwd_dx(dt, 0, dz.data_ptr(), x.data_ptr(), scale, shift, gg + 2 * C, gg + 3 * C,
                               dx.data_ptr(), M, C, 0, st));
     return {dx, grads.select(0, 0), grads.select(0, 1)};
+}
+
+// running_mean[l] = fp32(acc[l][0:C] / k), running_var[l] = fp32(acc[l][C:2C] / k) for every layer l: one
+// launch per BN_COMMIT_MAX_SEGS layers on the current stream (precise BatchNorm statistics).  acc[l]: contiguous
+// fp64 [2C]; running_mean[l], running_var[l]: contiguous fp32 [C], all on one device; k >= 1.
+static void bn_stats_commit(const std::vector<torch::Tensor>& acc, const std::vector<torch::Tensor>& running_mean,
+                            const std::vector<torch::Tensor>& running_var, int64_t k)
+{
+    auto fail = [](size_t i, const char* what) {
+        throw std::runtime_error("bn_stats_commit: layer " + std::to_string(i) + ": " + what);
+    };
+    if (acc.size() != running_mean.size() || acc.size() != running_var.size())
+        throw std::runtime_error("bn_stats_commit: acc, running_mean and running_var must have the same length");
+    if (k < 1) throw std::runtime_error("bn_stats_commit: k must be >= 1");
+    if (acc.empty()) return;
+    const auto device = acc[0].device();
+    std::vector<long long> rows;
+    rows.reserve(4 * acc.size());
+    for (size_t i = 0; i < acc.size(); ++i) {
+        const torch::Tensor& a = acc[i];
+        const torch::Tensor& m = running_mean[i];
+        const torch::Tensor& v = running_var[i];
+        const int64_t C = m.numel();
+        if (!(a.is_cuda() && m.is_cuda() && v.is_cuda() && a.device() == device && m.device() == device &&
+              v.device() == device))
+            fail(i, "every tensor must be a CUDA tensor on the first acc's device");
+        if (!(a.scalar_type() == torch::kFloat64 && a.is_contiguous() && a.numel() == 2 * C && C >= 1))
+            fail(i, "acc must be a contiguous fp64 [2C] tensor");
+        if (!(m.scalar_type() == torch::kFloat32 && v.scalar_type() == torch::kFloat32 && m.is_contiguous() &&
+              v.is_contiguous() && v.numel() == C))
+            fail(i, "running_mean and running_var must be contiguous fp32 [C] tensors");
+        rows.insert(rows.end(), {(long long)reinterpret_cast<uintptr_t>(a.data_ptr()),
+                                 (long long)reinterpret_cast<uintptr_t>(m.data_ptr()),
+                                 (long long)reinterpret_cast<uintptr_t>(v.data_ptr()), (long long)C});
+    }
+    c10::cuda::CUDAGuard guard(device);
+    const auto st = at::cuda::getCurrentCUDAStream();
+    const long long nseg = (long long)rows.size() / 4, per = bn_commit_max_segs();
+    for (long long b = 0; b < nseg; b += per)
+        BN_CHECK(bn_launch_stats_commit(rows.data() + 4 * b, (int)std::min(per, nseg - b), (double)k, st));
 }
 
 // ---------------------------------------------------------------------------
@@ -400,8 +457,9 @@ cudaError_t c1_launch_gemm(const void* x, const void* w, void* y, long long M, i
                            const void* residual, const void* bn_x, const float* coef, const uint8_t* mask,
                            int num_sms, int f32, cudaStream_t st);
 cudaError_t c1_launch_stats_finalize(const float* partial, int R, int C, const float* gamma, const float* beta,
-                                     float* rmean, float* rvar, long long* nbt, float momentum, float eps,
-                                     float* mean, float* invstd, float* scale, float* shift, cudaStream_t st);
+                                     float* rmean, float* rvar, long long* nbt, double* acc, float momentum,
+                                     float eps, float* mean, float* invstd, float* scale, float* shift,
+                                     cudaStream_t st);
 cudaError_t c1_launch_gemm_bn_eval(const void* x, const void* w, void* y, long long M, int N, int K,
                                    const void* residual, const float* gamma, const float* beta, const float* mean,
                                    const float* var, float eps, int relu, int num_sms, int f32, cudaStream_t st);
@@ -515,6 +573,7 @@ static std::vector<torch::Tensor> conv1x1_dgrad_bn_reduce(torch::Tensor x, torch
 
 // training-mode  out = act(bn(conv1x1(x, w)) [+ residual]);  returns (conv output, out, coef).
 // mask (optional, residual + relu only): filled with out's 1-bit ReLU mask, [M, N/8] uint8
+// acc (optional): accumulate mode of the statistics finalize, as in bn_forward
 static std::vector<torch::Tensor> conv1x1_bn_forward(torch::Tensor x, torch::Tensor w,
                                                      c10::optional<torch::Tensor> residual,
                                                      torch::Tensor gamma, torch::Tensor beta,
@@ -522,7 +581,8 @@ static std::vector<torch::Tensor> conv1x1_bn_forward(torch::Tensor x, torch::Ten
                                                      c10::optional<torch::Tensor> running_var,
                                                      c10::optional<torch::Tensor> num_batches_tracked,
                                                      double momentum, double eps, bool relu,
-                                                     c10::optional<torch::Tensor> mask, int num_sms)
+                                                     c10::optional<torch::Tensor> mask, int num_sms,
+                                                     c10::optional<torch::Tensor> acc)
 {
     TORCH_CHECK(conv1x1_can_fuse(x, w), "conv1x1_bn_forward: unsupported tensors");
     const int K = (int)x.size(1), N = (int)w.size(0);
@@ -543,6 +603,7 @@ static std::vector<torch::Tensor> conv1x1_bn_forward(torch::Tensor x, torch::Ten
         TORCH_CHECK(has_res && relu && mask->is_cuda() && mask->scalar_type() == torch::kUInt8 &&
                     mask->is_contiguous() && mask->numel() == M * (N / 8),
                     "conv1x1_bn_forward: mask must be [M, N/8] uint8 (residual + relu only)");
+    double* accp = bn_acc_ptr(acc, x, N);
     const int R = c1_partial_rows(M, N, K, sms, 0, f32);
     auto partial = torch::empty({R, 3, N}, fopt);
     BN_CHECK(c1_launch_gemm(x.data_ptr(), w.data_ptr(), yraw.data_ptr(), M, N, K, partial.data_ptr<float>(),
@@ -557,7 +618,7 @@ static std::vector<torch::Tensor> conv1x1_bn_forward(torch::Tensor x, torch::Ten
     if (num_batches_tracked.has_value() && num_batches_tracked->defined())
         nbt = reinterpret_cast<long long*>(num_batches_tracked->data_ptr<int64_t>());
     BN_CHECK(c1_launch_stats_finalize(partial.data_ptr<float>(), R, N, gamma.data_ptr<float>(),
-                                      beta.data_ptr<float>(), rm, rv, nbt, (float)momentum, (float)eps,
+                                      beta.data_ptr<float>(), rm, rv, nbt, accp, (float)momentum, (float)eps,
                                       mean, mean + N, mean + 2 * N, mean + 3 * N, st));
     auto out = torch::empty_like(yraw);
     BN_CHECK(bn_launch_apply(f32, relu ? 1 : 0, has_res ? 1 : 0, yraw.data_ptr(),
@@ -741,7 +802,7 @@ void bind_bn(py::module& mod)
     mod.def("conv1x1_bn_forward", &conv1x1_bn_forward, py::arg("x"), py::arg("w"), py::arg("residual"),
             py::arg("gamma"), py::arg("beta"), py::arg("running_mean"), py::arg("running_var"),
             py::arg("num_batches_tracked"), py::arg("momentum"), py::arg("eps"), py::arg("relu"),
-            py::arg("mask") = py::none(), py::kw_only(), py::arg("num_sms") = 0);
+            py::arg("mask") = py::none(), py::kw_only(), py::arg("num_sms") = 0, py::arg("acc") = py::none());
     mod.def("conv1x1_dgrad_bn_reduce", &conv1x1_dgrad_bn_reduce, py::arg("x"), py::arg("w"), py::arg("residual"),
             py::arg("bn_x"), py::arg("coef"), py::arg("mask"), py::kw_only(), py::arg("num_sms") = 0);
     mod.def("conv1x1_bn_eval", &conv1x1_bn_eval, py::arg("x"), py::arg("w"), py::arg("gamma"), py::arg("beta"),
@@ -754,7 +815,12 @@ void bind_bn(py::module& mod)
     mod.def("maxpool_forward", &maxpool_forward);
     mod.def("maxpool_backward", &maxpool_backward);
     mod.def("bn_can_fuse", &bn_can_fuse);
-    mod.def("bn_forward", &bn_forward);
+    mod.def("bn_forward", &bn_forward, py::arg("x"), py::arg("residual"), py::arg("gamma"), py::arg("beta"),
+            py::arg("running_mean"), py::arg("running_var"), py::arg("num_batches_tracked"), py::arg("training"),
+            py::arg("momentum"), py::arg("eps"), py::arg("relu"), py::arg("acc") = py::none());
+    mod.def("bn_stats_commit", &bn_stats_commit, py::arg("acc"), py::arg("running_mean"), py::arg("running_var"),
+            py::arg("k"), "running = fp32(acc / k) for every BatchNorm layer: one launch per BN_COMMIT_MAX_SEGS layers");
+    mod.attr("BN_COMMIT_MAX_SEGS") = bn_commit_max_segs();
     mod.def("bn_backward", &bn_backward);
     mod.def("bn_backward_from_partials", &bn_backward_from_partials);
     mod.def("bn_f32_map", &bn_f32_map, py::arg("value") = -1,

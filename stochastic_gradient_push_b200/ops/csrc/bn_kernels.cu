@@ -9,6 +9,9 @@
 //              the ReLU mask is recomputed from x*scale+shift (no mask tensor, no
 //              extra read); with a residual the mask comes from the saved output
 //              and dz is written once because it IS the residual branch's grad.
+//   precise statistics: the finalize adds the batch statistics to an fp64 accumulator
+//              instead of the running update; one commit launch per pass writes
+//              running = fp32(sum / K) for every layer (GossipTrainer.update_bn)
 //
 // Layout: x is [M, C] row-major (M = N*H*W, NHWC), C % 8 == 0, C <= 2048.
 // One thread owns 8 channels and strides over rows, so per-channel constants
@@ -194,17 +197,19 @@ __device__ __forceinline__ void sum_partials(const float* __restrict__ partial, 
     q_out = q;
 }
 
+// acc (accumulate mode, precise BatchNorm statistics): acc[c] += mu, acc[C + c] += unbiased variance, the
+// fp32 values the running update would blend in; the running buffers and nbt are then left alone
 __global__ void __launch_bounds__(BN_FIN_THREADS)
 bn_stats_finalize_kernel(const float* __restrict__ partial, int G, long long M, int C,
                          const float* __restrict__ gamma, const float* __restrict__ beta,
-                         float* running_mean, float* running_var, long long* nbt,
+                         float* running_mean, float* running_var, long long* nbt, double* acc,
                          float momentum, float eps,
                          float* __restrict__ mean, float* __restrict__ invstd,
                          float* __restrict__ scale, float* __restrict__ shift)
 {
     float s, q; bool owner; int c;
     sum_partials(partial, G, C, s, q, owner, c);
-    if (blockIdx.x == 0 && threadIdx.x == 0 && nbt != nullptr) *nbt += 1;
+    if (blockIdx.x == 0 && threadIdx.x == 0 && nbt != nullptr && acc == nullptr) *nbt += 1;
     if (!owner) return;
     const float k = partial[(size_t)G * 2 * C + c];          // the shift K = x[row 0]
     const float inv_m = 1.f / (float)M;
@@ -217,11 +222,55 @@ bn_stats_finalize_kernel(const float* __restrict__ partial, int G, long long M, 
     const float sc = gamma[c] * is;
     scale[c] = sc;
     shift[c] = fmaf(-mu, sc, beta[c]);
-    if (running_mean != nullptr) {
-        const float unbiased = (M > 1) ? var * ((float)M / (float)(M - 1)) : var;
+    const float unbiased = (M > 1) ? var * ((float)M / (float)(M - 1)) : var;
+    if (acc != nullptr) {
+        acc[c] += (double)mu;
+        acc[C + c] += (double)unbiased;
+    } else if (running_mean != nullptr) {
         running_mean[c] = fmaf(momentum, mu - running_mean[c], running_mean[c]);
         running_var[c] = fmaf(momentum, unbiased - running_var[c], running_var[c]);
     }
+}
+
+// ---------------------------------------------------------------------------
+// precise BatchNorm statistics: running = fp32(acc / K) for every layer, ONE launch per pass.  The table
+// is the kernel's __grid_constant__ parameter (as in accum_kernels.cu), one thread per channel; a row holds
+// the prefix of its first channel, so a thread finds its layer by a binary search over the table.
+// ---------------------------------------------------------------------------
+#define BN_COMMIT_THREADS 256
+#define BN_COMMIT_MAX_SEGS 1000           // 1000 x 32 B + the header fits the 32,764-byte parameter space
+
+struct BnCommitSeg {                      // 32 bytes
+    const double* acc;                    // [2C]: sum of the batch means, then of the unbiased variances
+    float* rmean;
+    float* rvar;
+    int C;
+    int c0;                               // flat index of the layer's first channel
+};
+
+struct BnCommitTable {
+    int nseg;
+    int total;
+    BnCommitSeg seg[BN_COMMIT_MAX_SEGS];
+};
+
+static_assert(sizeof(BnCommitSeg) == 32, "BnCommitSeg layout");
+static_assert(sizeof(BnCommitTable) <= 32764, "the commit table must fit the kernel parameter space");
+
+__global__ void __launch_bounds__(BN_COMMIT_THREADS)
+bn_stats_commit_kernel(const __grid_constant__ BnCommitTable tab, double k)
+{
+    const int i = blockIdx.x * BN_COMMIT_THREADS + threadIdx.x;
+    if (i >= tab.total) return;
+    int lo = 0, hi = tab.nseg - 1;        // the last layer whose first channel is <= i
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (tab.seg[mid].c0 <= i) lo = mid; else hi = mid - 1;
+    }
+    const BnCommitSeg& sg = tab.seg[lo];
+    const int c = i - sg.c0;
+    sg.rmean[c] = __double2float_rn(__ddiv_rn(sg.acc[c], k));
+    sg.rvar[c] = __double2float_rn(__ddiv_rn(sg.acc[sg.C + c], k));
 }
 
 // eval mode: scale/shift from the running statistics
@@ -494,12 +543,39 @@ cudaError_t bn_launch_stats(int dtype, const void* x, float* partial, long long 
 }
 
 cudaError_t bn_launch_stats_finalize(const float* partial, int G, long long M, int C, const float* gamma,
-                                     const float* beta, float* rmean, float* rvar, long long* nbt,
+                                     const float* beta, float* rmean, float* rvar, long long* nbt, double* acc,
                                      float momentum, float eps, float* mean, float* invstd,
                                      float* scale, float* shift, cudaStream_t st)
 {
     bn_stats_finalize_kernel<<<(C + 31) / 32, BN_FIN_THREADS, 0, st>>>(partial, G, M, C, gamma, beta, rmean, rvar,
-                                                              nbt, momentum, eps, mean, invstd, scale, shift);
+                                                              nbt, acc, momentum, eps, mean, invstd, scale, shift);
+    return cudaGetLastError();
+}
+
+int bn_commit_max_segs() { return BN_COMMIT_MAX_SEGS; }
+
+// rows: host int64 [nseg, 4] = (acc address, running_mean address, running_var address, C >= 1),
+// 1 <= nseg <= BN_COMMIT_MAX_SEGS, fewer than 2^31 channels in all; k >= 1.  One launch.
+cudaError_t bn_launch_stats_commit(const long long* rows, int nseg, double k, cudaStream_t st)
+{
+    if (nseg < 1 || nseg > BN_COMMIT_MAX_SEGS || !(k >= 1.0)) return cudaErrorInvalidValue;
+    BnCommitTable tab;
+    long long total = 0;
+    for (int i = 0; i < nseg; ++i) {
+        const long long* r = rows + 4 * i;
+        if (r[3] < 1) return cudaErrorInvalidValue;
+        tab.seg[i].acc = reinterpret_cast<const double*>(r[0]);
+        tab.seg[i].rmean = reinterpret_cast<float*>(r[1]);
+        tab.seg[i].rvar = reinterpret_cast<float*>(r[2]);
+        tab.seg[i].C = (int)r[3];
+        tab.seg[i].c0 = (int)total;
+        total += r[3];
+        if (total > 0x7fffffffLL) return cudaErrorInvalidValue;
+    }
+    tab.nseg = nseg;
+    tab.total = (int)total;
+    bn_stats_commit_kernel<<<(unsigned)((total + BN_COMMIT_THREADS - 1) / BN_COMMIT_THREADS), BN_COMMIT_THREADS, 0,
+                             st>>>(tab, k);
     return cudaGetLastError();
 }
 

@@ -808,13 +808,15 @@ c1_gemm_eval_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_const
 
 // ---------------------------------------------------------------------------
 // statistics finalize: merge the R per-CTA rows (n, mean, M2) per channel (Chan et al.),
-// then the same outputs as bn_stats_finalize_kernel.  1024 threads = 32 row lanes x 32 channels.
+// then the same outputs as bn_stats_finalize_kernel (accumulate mode included: acc != nullptr adds
+// mu / the unbiased variance to acc in fp64 and leaves the running buffers and nbt alone).
+// 1024 threads = 32 row lanes x 32 channels.
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(1024, 1)
 c1_stats_finalize_kernel(const float* __restrict__ partial, int R, int C, const float* __restrict__ gamma,
                          const float* __restrict__ beta, float* running_mean, float* running_var, long long* nbt,
-                         float momentum, float eps, float* __restrict__ mean, float* __restrict__ invstd,
-                         float* __restrict__ scale, float* __restrict__ shift)
+                         double* acc, float momentum, float eps, float* __restrict__ mean,
+                         float* __restrict__ invstd, float* __restrict__ scale, float* __restrict__ shift)
 {
     __shared__ float sm_a[32][33];
     __shared__ float sm_b[32][33];
@@ -823,7 +825,7 @@ c1_stats_finalize_kernel(const float* __restrict__ partial, int R, int C, const 
     const int lane = threadIdx.x >> 5;
     const int ch = blockIdx.x * 32 + cl;
     const bool live = ch < C;
-    if (blockIdx.x == 0 && threadIdx.x == 0 && nbt != nullptr) *nbt += 1;
+    if (blockIdx.x == 0 && threadIdx.x == 0 && nbt != nullptr && acc == nullptr) *nbt += 1;
 
     // every row of this lane is loaded up front (R <= 160 -> at most 5 rows per lane per batch), so
     // the kernel pays one L2 round trip instead of one per row
@@ -888,8 +890,11 @@ c1_stats_finalize_kernel(const float* __restrict__ partial, int R, int C, const 
     const float sc = gamma[ch] * is;
     scale[ch] = sc;
     shift[ch] = fmaf(-mu, sc, beta[ch]);
-    if (running_mean != nullptr) {
-        const float unbiased = (n_tot > 1.f) ? var * (n_tot / (n_tot - 1.f)) : var;
+    const float unbiased = (n_tot > 1.f) ? var * (n_tot / (n_tot - 1.f)) : var;
+    if (acc != nullptr) {
+        acc[ch] += (double)mu;
+        acc[C + ch] += (double)unbiased;
+    } else if (running_mean != nullptr) {
         running_mean[ch] = fmaf(momentum, mu - running_mean[ch], running_mean[ch]);
         running_var[ch] = fmaf(momentum, unbiased - running_var[ch], running_var[ch]);
     }
@@ -1174,11 +1179,12 @@ cudaError_t c1_launch_gemm_bn_eval(const void* x, const void* w, void* y, long l
 }
 
 cudaError_t c1_launch_stats_finalize(const float* partial, int R, int C, const float* gamma, const float* beta,
-                                     float* rmean, float* rvar, long long* nbt, float momentum, float eps,
-                                     float* mean, float* invstd, float* scale, float* shift, cudaStream_t st)
+                                     float* rmean, float* rvar, long long* nbt, double* acc, float momentum,
+                                     float eps, float* mean, float* invstd, float* scale, float* shift,
+                                     cudaStream_t st)
 {
-    c1_stats_finalize_kernel<<<(C + 31) / 32, 1024, 0, st>>>(partial, R, C, gamma, beta, rmean, rvar, nbt, momentum,
-                                                            eps, mean, invstd, scale, shift);
+    c1_stats_finalize_kernel<<<(C + 31) / 32, 1024, 0, st>>>(partial, R, C, gamma, beta, rmean, rvar, nbt, acc,
+                                                            momentum, eps, mean, invstd, scale, shift);
     return cudaGetLastError();
 }
 

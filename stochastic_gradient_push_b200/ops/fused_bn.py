@@ -87,6 +87,84 @@ def eval_bn_gemm():
         _EVAL_GEMM[0] = prev
 
 
+# set by precise_bn_stats(): the BNStatsAccumulator train-mode BatchNorm layers add their batch statistics to
+_PRECISE_BN = [None]
+
+
+class BNStatsAccumulator(object):
+    """fp64 sums of the per-batch statistics of every BatchNorm layer of ``module``, for precise BatchNorm
+    statistics (``GossipTrainer.update_bn``).  One flat fp64 buffer (:attr:`flat`), allocated once, so its
+    addresses are stable under graph capture; layer l's view (:attr:`views`) is ``[2 C_l]``: the sum of its
+    batch means, then the sum of its unbiased batch variances -- the fp32 values the training forward would
+    blend into the running buffers.  Every BatchNorm layer that tracks running statistics must be a
+    :class:`FusedBatchNormAct2d` (ValueError otherwise)."""
+
+    def __init__(self, module: nn.Module):
+        from torch.nn.modules.batchnorm import _BatchNorm
+        layers = [m for m in module.modules() if isinstance(m, _BatchNorm) and m.track_running_stats]
+        other = sorted(set(type(m).__name__ for m in layers if not isinstance(m, FusedBatchNormAct2d)))
+        if other:
+            raise ValueError('precise BatchNorm statistics need every BatchNorm layer to be a FusedBatchNormAct2d; '
+                             'found %s' % ', '.join(other))
+        sizes = [2 * m.num_features for m in layers]
+        device = layers[0].running_mean.device if layers else torch.device('cpu')
+        self.layers = layers
+        self.flat = torch.zeros(sum(sizes), dtype=torch.float64, device=device)
+        self.views = list(self.flat.split(sizes))
+        self._view_of = {m: v for m, v in zip(layers, self.views)}
+
+    def view_of(self, bn) -> torch.Tensor:
+        v = self._view_of.get(bn)
+        if v is None:
+            raise ValueError('precise_bn_stats: a train-mode BatchNorm layer (%s) is not one of the '
+                             "accumulator's layers" % bn)
+        return v
+
+    def zero_(self):
+        self.flat.zero_()
+
+    @torch.no_grad()
+    def commit(self, k: int):
+        """``running_mean = fp32(sum of means / k)``, ``running_var = fp32(sum of variances / k)`` for every
+        layer, k >= 1: one ``bn_stats_commit`` launch on CUDA, torch ops on the reference path."""
+        if k < 1:
+            raise ValueError('commit needs k >= 1, got %r' % (k,))
+        if not self.layers:
+            return
+        if FORCE_REFERENCE or not self.flat.is_cuda:
+            for m, v in zip(self.layers, self.views):
+                c = m.num_features
+                m.running_mean.copy_((v[:c] / k).float())
+                m.running_var.copy_((v[c:] / k).float())
+            return
+        native.load().bn_stats_commit(self.views, [m.running_mean for m in self.layers],
+                                      [m.running_var for m in self.layers], int(k))
+
+
+@contextlib.contextmanager
+def precise_bn_stats(acc: BNStatsAccumulator):
+    """Inside the block every train-mode ``FusedBatchNormAct2d``, ``conv_bn_act`` and ``conv_bn_act_split``
+    of ``acc``'s layers normalises with its batch statistics as in training, but adds those statistics
+    (the batch mean and unbiased variance, as fp32 values) to its view of ``acc`` in fp64 instead of
+    updating its running buffers; ``num_batches_tracked`` is not advanced.  The forward's outputs are those
+    of a training forward, bit for bit.  Outside it a forward runs as before.
+    ``GossipTrainer.update_bn`` uses it, then ``acc.commit(K)``."""
+    prev = _PRECISE_BN[0]
+    _PRECISE_BN[0] = acc
+    try:
+        yield acc
+    finally:
+        _PRECISE_BN[0] = prev
+
+
+def _acc_of(bn, training: bool):
+    """the accumulator view of a train-mode BatchNorm inside :func:`precise_bn_stats`, else None"""
+    acc = _PRECISE_BN[0]
+    if acc is None or not training or not bn.track_running_stats:
+        return None
+    return acc.view_of(bn)
+
+
 def _can_fuse(x: torch.Tensor) -> bool:
     if FORCE_REFERENCE or not x.is_cuda or not native.available():
         return False
@@ -97,10 +175,10 @@ class _FusedBNAct(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, residual, weight, bias, running_mean, running_var, nbt,
-                training, momentum, eps, relu):
+                training, momentum, eps, relu, acc):
         C = native.load()
         y, coef = C.bn_forward(x, residual, weight, bias, running_mean, running_var, nbt,
-                               training, momentum, eps, relu)
+                               training, momentum, eps, relu, acc)
         ctx.relu = relu
         ctx.add = residual is not None
         ctx.training = training
@@ -126,29 +204,37 @@ class _FusedBNAct(torch.autograd.Function):
                 out = y if ctx.add else torch.relu(F.batch_norm(x, None, None, training=False))
                 dz = dy * (out > 0)
             return dz * scale, (dz if ctx.add else None), None, None, None, None, None, \
-                None, None, None, None
+                None, None, None, None, None
         dx, dz, ggamma, gbeta = C.bn_backward(dy, x, y, coef, ctx.relu, ctx.add)
-        return dx, (dz if ctx.add else None), ggamma, gbeta, None, None, None, None, None, None, None
+        return dx, (dz if ctx.add else None), ggamma, gbeta, None, None, None, None, None, None, None, None
 
 
 def fused_bn_act(x, weight, bias, running_mean, running_var, num_batches_tracked=None,
-                 residual=None, relu=False, training=True, momentum=0.1, eps=1e-5):
-    """Functional form; falls back to plain PyTorch when the kernels cannot run."""
+                 residual=None, relu=False, training=True, momentum=0.1, eps=1e-5, acc=None):
+    """Functional form; falls back to plain PyTorch when the kernels cannot run.  ``acc`` (training
+    only): an fp64 ``[2C]`` accumulator that receives the batch statistics instead of the running
+    buffers (see :func:`precise_bn_stats`)."""
     fusable = _can_fuse(x) and weight is not None and weight.dtype == torch.float32 \
         and (residual is None or (relu and residual.dtype == x.dtype
                                   and residual.stride() == x.stride()))
     if fusable and (training or not torch.is_grad_enabled() or not x.requires_grad):
         return _FusedBNAct.apply(x, residual, weight, bias, running_mean, running_var,
-                                 num_batches_tracked, training, momentum, eps, relu)
+                                 num_batches_tracked, training, momentum, eps, relu, acc)
     return reference_bn_act(x, weight, bias, running_mean, running_var, num_batches_tracked,
-                            residual, relu, training, momentum, eps)
+                            residual, relu, training, momentum, eps, acc)
 
 
 def reference_bn_act(x, weight, bias, running_mean, running_var, num_batches_tracked=None,
-                     residual=None, relu=False, training=True, momentum=0.1, eps=1e-5):
-    if training and num_batches_tracked is not None:
-        num_batches_tracked.add_(1)
-    y = F.batch_norm(x, running_mean, running_var, weight, bias, training, momentum, eps)
+                     residual=None, relu=False, training=True, momentum=0.1, eps=1e-5, acc=None):
+    if acc is not None:
+        # the batch statistics exactly as a momentum-1 update of zeroed running buffers writes them
+        stats = torch.zeros(2, x.shape[1], dtype=running_mean.dtype, device=x.device)
+        y = F.batch_norm(x, stats[0], stats[1], weight, bias, True, 1.0, eps)
+        acc.add_(stats.view(-1))
+    else:
+        if training and num_batches_tracked is not None:
+            num_batches_tracked.add_(1)
+        y = F.batch_norm(x, running_mean, running_var, weight, bias, training, momentum, eps)
     if residual is not None:
         y = y + residual
     return F.relu(y) if relu else y
@@ -165,7 +251,8 @@ class FusedBatchNormAct2d(nn.BatchNorm2d):
             self.running_mean if self.track_running_stats else None,
             self.running_var if self.track_running_stats else None,
             self.num_batches_tracked if (self.track_running_stats and training) else None,
-            residual=residual, relu=relu, training=training, momentum=momentum, eps=self.eps)
+            residual=residual, relu=relu, training=training, momentum=momentum, eps=self.eps,
+            acc=_acc_of(self, training))
 
 
 # --------------------------------------------------------------------------- #
@@ -191,7 +278,7 @@ class _Conv1x1BNAct(torch.autograd.Function):
     fused BN backward, then the library's dgrad / wgrad for the convolution."""
 
     @staticmethod
-    def forward(ctx, x, w, residual, gamma, beta, running_mean, running_var, nbt, momentum, eps, relu):
+    def forward(ctx, x, w, residual, gamma, beta, running_mean, running_var, nbt, momentum, eps, relu, acc):
         C = native.load()
         w16 = w if w.dtype == x.dtype else w.detach().to(x.dtype)      # compute-dtype weights
         mask = None
@@ -199,7 +286,7 @@ class _Conv1x1BNAct(torch.autograd.Function):
             M, N = x.numel() // x.shape[1], w.shape[0]
             mask = torch.empty((M, N // 8), dtype=torch.uint8, device=x.device)
         yraw, out, coef = C.conv1x1_bn_forward(x, w16, residual, gamma, beta, running_mean, running_var,
-                                               nbt, momentum, eps, relu, mask)
+                                               nbt, momentum, eps, relu, mask, acc=acc)
         ctx.relu = relu
         ctx.add = residual is not None
         ctx.w_dtype = w.dtype
@@ -232,7 +319,7 @@ class _Conv1x1BNAct(torch.autograd.Function):
             [ctx.needs_input_grad[0], ctx.needs_input_grad[1], False])
         if dw is not None and dw.dtype != ctx.w_dtype:
             dw = dw.to(ctx.w_dtype)
-        return dx, dw, (dz if ctx.add else None), ggamma, gbeta, None, None, None, None, None, None
+        return dx, dw, (dz if ctx.add else None), ggamma, gbeta, None, None, None, None, None, None, None
 
 
 class _Conv1x1BNActSplit(torch.autograd.Function):
@@ -242,11 +329,11 @@ class _Conv1x1BNActSplit(torch.autograd.Function):
     separate read-read-write accumulation pass over the widest activation of the block."""
 
     @staticmethod
-    def forward(ctx, x, w, gamma, beta, running_mean, running_var, nbt, momentum, eps, relu, handoff):
+    def forward(ctx, x, w, gamma, beta, running_mean, running_var, nbt, momentum, eps, relu, handoff, acc):
         C = native.load()
         w16 = w if w.dtype == x.dtype else w.detach().to(x.dtype)
         yraw, out, coef = C.conv1x1_bn_forward(x, w16, None, gamma, beta, running_mean, running_var,
-                                               nbt, momentum, eps, relu)
+                                               nbt, momentum, eps, relu, acc=acc)
         ctx.relu = relu
         ctx.w_dtype = w.dtype
         ctx.handoff = handoff
@@ -287,7 +374,7 @@ class _Conv1x1BNActSplit(torch.autograd.Function):
                 dyraw, x, w16, None, [1, 1], [0, 0], [1, 1], False, [0, 0], 1, [False, True, False])[1]
             if dw.dtype != ctx.w_dtype:
                 dw = dw.to(ctx.w_dtype)
-        return dx, dw, ggamma, gbeta, None, None, None, None, None, None, None
+        return dx, dw, ggamma, gbeta, None, None, None, None, None, None, None, None
 
 
 def _conv1x1_operands(conv, bn, x, residual, relu):
@@ -329,7 +416,8 @@ def conv_bn_act(conv: nn.Conv2d, bn: 'FusedBatchNormAct2d', x, residual=None, re
     if ok:
         momentum = 0.1 if bn.momentum is None else bn.momentum
         return _Conv1x1BNAct.apply(xk, conv.weight, residual, bn.weight, bn.bias, bn.running_mean,
-                                   bn.running_var, bn.num_batches_tracked, momentum, bn.eps, relu)
+                                   bn.running_var, bn.num_batches_tracked, momentum, bn.eps, relu,
+                                   _acc_of(bn, True))
     return bn(conv(x), residual=residual, relu=relu)
 
 
@@ -351,7 +439,7 @@ def conv_bn_act_split(conv: nn.Conv2d, bn: 'FusedBatchNormAct2d', x, relu=False)
                 handoff = None
             return _Conv1x1BNActSplit.apply(x, conv.weight, bn.weight, bn.bias, bn.running_mean,
                                             bn.running_var, bn.num_batches_tracked, momentum, bn.eps, relu,
-                                            handoff)
+                                            handoff, _acc_of(bn, True))
     return conv_bn_act(conv, bn, x, relu=relu), x
 
 

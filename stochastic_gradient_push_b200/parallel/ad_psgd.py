@@ -643,6 +643,10 @@ def make_bilat_trainer(model: BilatGossipDataParallel, lr, criterion=None, amp_d
             raise ValueError('evaluate() is not supported with AD-PSGD: its gossip daemon rewrites the '
                              'parameters asynchronously, so a captured evaluation would not see one model')
 
+        def update_bn(self, batches):
+            raise ValueError('update_bn() is not supported with AD-PSGD: its gossip daemon rewrites the '
+                             'parameters asynchronously, so the statistics would not be those of one model')
+
         def check(self):
             self.model._check()
 

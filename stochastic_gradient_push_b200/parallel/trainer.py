@@ -49,6 +49,14 @@ every 1x1 / stride-1 convolution and its BatchNorm (+ residual) (+ ReLU) as one 
 (``ops.fused_bn.eval_bn_gemm``), and one ``xent_eval_accumulate`` launch that adds the batch's loss sum
 and top-1 / top-5 / row counts to a device accumulator, read back once at the end.  Nothing the
 training step owns is touched.
+
+Precise BatchNorm statistics (``update_bn(batches)``): the same network and precision in train mode
+under ``torch.no_grad()``, over K batches, staged and captured per batch shape as in ``evaluate``.
+Inside ``ops.fused_bn.precise_bn_stats`` every BatchNorm finalize launch adds its batch's mean and
+unbiased variance to an fp64 accumulator instead of its running buffers; one ``bn_stats_commit``
+launch then sets every running buffer to ``fp32(sum / K)``.  The first batch of a shape runs eagerly
+(and is counted) before its graph is captured; a capture does not execute, so every batch is counted
+once.
 """
 
 from __future__ import annotations
@@ -61,7 +69,7 @@ from typing import Callable, NamedTuple, Optional
 
 import torch
 
-from ..ops.fused_bn import eval_bn_gemm
+from ..ops.fused_bn import BNStatsAccumulator, eval_bn_gemm, precise_bn_stats
 from ..ops.fused_loss import FusedCrossEntropyWithAccuracy, eval_accumulate, eval_accumulator
 from ..optim import FusedGossipSGD
 from .distributed import GossipDataParallel
@@ -92,8 +100,9 @@ class EvalResult(NamedTuple):
 
 
 class _EvalSlot(object):
-    """per evaluation batch shape: staging and static buffers, and the captured graph"""
-    __slots__ = ('stage', 'stage_tgt', 'static_in', 'static_tgt', 'ready', 'free', 'graph', 'out')
+    """per evaluation batch shape: staging and static buffers, and the captured graphs of
+    ``evaluate`` (``graph``) and ``update_bn`` (``bn_graph``)"""
+    __slots__ = ('stage', 'stage_tgt', 'static_in', 'static_tgt', 'ready', 'free', 'graph', 'out', 'bn_graph')
 
 
 class GossipTrainer(object):
@@ -187,6 +196,8 @@ class GossipTrainer(object):
         self._eval_acc = None
         self.eval_out = None            # logits of the last batch of the last evaluate()
         self.eval_launches_per_batch = None
+        self._bn_acc = None             # update_bn(): the fp64 BatchNorm statistics accumulator
+        self.update_bn_launches_per_batch = None
 
     # ------------------------------------------------------------------ #
     def _autocast(self):
@@ -574,19 +585,11 @@ class GossipTrainer(object):
         self.stream.wait_stream(main)            # (in-place swaps by ema.applied() / averaged() on main)
         with torch.cuda.stream(self.stream):
             self._eval_acc.zero_()
-        out = None
         try:
             for m in modules:
                 m.eval()
             with torch.no_grad():
-                it = iter(batches)
-                nxt = next(it, None)
-                slot = self._eval_prefetch(*nxt) if nxt is not None else None
-                while slot is not None:
-                    self._eval_load(slot)
-                    nxt = next(it, None)
-                    cur, slot = slot, (self._eval_prefetch(*nxt) if nxt is not None else None)
-                    out = self._eval_run(cur, net)
+                _, out = self._staged_pass(batches, lambda slot: self._eval_run(slot, net))
         finally:
             for m, mode in zip(modules, modes):
                 m.train(mode)
@@ -596,6 +599,22 @@ class GossipTrainer(object):
             acc = self._eval_acc.cpu()           # the one read-back (synchronises the stream)
         main.wait_stream(self.stream)
         return EvalResult.from_sums(float(acc[:1].view(torch.float64)), int(acc[1]), int(acc[2]), int(acc[3]))
+
+    def _staged_pass(self, batches, run):
+        """``run(slot)`` for every ``(input, target)`` of ``batches`` in order, each staged through its
+        shape's :class:`_EvalSlot`; the H2D copy of batch i+1 overlaps batch i.  Returns (number of
+        batches, what the last ``run`` returned)."""
+        n, out = 0, None
+        it = iter(batches)
+        nxt = next(it, None)
+        slot = self._eval_prefetch(*nxt) if nxt is not None else None
+        while slot is not None:
+            self._eval_load(slot)
+            nxt = next(it, None)
+            cur, slot = slot, (self._eval_prefetch(*nxt) if nxt is not None else None)
+            out = run(cur)
+            n += 1
+        return n, out
 
     def _eval_prefetch(self, batch, target) -> _EvalSlot:
         """start the H2D copy of an evaluation batch into its shape's staging buffers (copy stream)"""
@@ -611,7 +630,7 @@ class GossipTrainer(object):
             slot.stage = torch.empty(batch.shape, dtype=batch.dtype, device=self.device)
             slot.stage_tgt = torch.empty_like(slot.static_tgt)
             slot.ready, slot.free = torch.cuda.Event(), torch.cuda.Event()
-            slot.graph = slot.out = None
+            slot.graph = slot.out = slot.bn_graph = None
             slot.free.record(self.stream)
         cs = self._copy_stream
         cs.wait_event(slot.free)
@@ -669,3 +688,68 @@ class GossipTrainer(object):
                 slot.graph = graph
             slot.graph.replay()
             return slot.out
+
+    # ------------------------------------------------------------------ #
+    def update_bn(self, batches) -> int:
+        """Precise BatchNorm statistics: set every BatchNorm layer's running mean and variance to the
+        average over ``batches`` (an iterable of ``(input, target)`` as for :meth:`evaluate`; targets are
+        ignored) of the batch mean and unbiased variance that the training forward computes for each batch,
+        ``running = fp32(sum_k stat_k / K)`` with the sum in fp64 in batch order.  Every batch weighs the
+        same, a partial one included (as ``torch.optim.swa_utils.update_bn``).  Drains the trainer first
+        (:meth:`finish`), then runs the step's network and precision in train mode under ``no_grad``, each
+        batch normalised by its own statistics; restores the previous mode.  Each batch shape is captured
+        once (in the trainer's graph pool) and replayed on later calls, so this works inside
+        ``ModelEma.applied()`` and ``GossipDataParallel.averaged()``.  Only the running statistics change:
+        ``num_batches_tracked``, parameters, momentum, the engine's step counter, the metrics ring, the
+        training buffers and graphs, the EMA and the batch-mix iteration are left as they were.  Returns K;
+        with K = 0 nothing changes.  ``update_bn_launches_per_batch``: our kernels per batch."""
+        self.finish()
+        twin = getattr(self.model, '_twin', None)
+        net = twin[0] if twin else self.model.module
+        modules = [self.model.module] + ([net] if twin else [])
+        modes = [m.training for m in modules]
+        if self._bn_acc is None:
+            self._bn_acc = BNStatsAccumulator(net)
+        main = torch.cuda.current_stream(self.device)
+        self.stream.wait_stream(main)            # (in-place swaps by ema.applied() / averaged() on main)
+        with torch.cuda.stream(self.stream):
+            self._bn_acc.zero_()
+        try:
+            for m in modules:
+                m.train()
+            with torch.no_grad(), precise_bn_stats(self._bn_acc):
+                k, _ = self._staged_pass(batches, lambda slot: self._bn_run(slot, net))
+        finally:
+            for m, mode in zip(modules, modes):
+                m.train(mode)
+        if k > 0:
+            with torch.cuda.stream(self.stream):
+                self._bn_acc.commit(k)
+        main.wait_stream(self.stream)
+        return k
+
+    def _bn_forward(self, slot: _EvalSlot, net):
+        with self._eval_autocast():
+            net(slot.static_in)
+
+    def _bn_run(self, slot: _EvalSlot, net):
+        """one batch of :meth:`update_bn` on the trainer's stream: its statistics go to the accumulator"""
+        C = self.engine.C
+        with torch.cuda.stream(self.stream):
+            if slot.bn_graph is not None:
+                slot.bn_graph.replay()
+                return
+            # eager: every batch; graphs: the first batch of a shape (library algorithm choice, lazy
+            # initialisation) -- it is counted here, so the capture below is not replayed for it
+            c0 = C.launch_count()
+            self._bn_forward(slot, net)
+            self.update_bn_launches_per_batch = C.launch_count() - c0
+            if not self.use_graph:
+                return
+            torch.cuda.synchronize(self.device)
+            if self._pool is None:
+                self._pool = torch.cuda.graph_pool_handle()
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph, stream=self.stream, capture_error_mode='thread_local', pool=self._pool):
+                self._bn_forward(slot, net)
+            slot.bn_graph = graph

@@ -115,6 +115,11 @@ def build_parser(adpsgd: bool = False) -> argparse.ArgumentParser:
                         '<checkpoint_dir><tag>ema_r<rank>_n<world>.csv; 0 = off.  Not with AD-PSGD')
     p.add_argument('--model_ema_warmup', default=False, **B,
                    help='EMA decay warm-up: min(decay, (1 + t) / (10 + t)) after t updates')
+    p.add_argument('--drop_path_rate', default=0.0, type=float,
+                   help='stochastic depth (Huang et al. 2016; timm drop_path_rate) in [0, 1) on the ResNet residual '
+                        'blocks, linear in the block index (block 0 never drops, the last drops with this rate); '
+                        'applied inside the fused BatchNorm kernels, drawn from (--seed, rank); 0 = off.  Not with '
+                        '--model tiny')
     p.add_argument('--seed', default=47, type=int)
     p.add_argument('--resume', default=False, **B)
     p.add_argument('--backend', default='nccl', choices=['nccl', 'gloo', 'mpi'])
@@ -303,6 +308,7 @@ def finalize_args(args, adpsgd=False):
     check_mix_flags(args)
     check_augment_flags(args)
     check_ema_flags(args, adpsgd)
+    check_drop_path_flags(args)
     args.ema_fname = '{}{}ema_r{}_n{}.csv'.format(args.checkpoint_dir, args.tag, args.rank, args.world_size)
     args.consensus_fname = '{}{}consensus_r{}_n{}.csv'.format(args.checkpoint_dir, args.tag, args.rank,
                                                               args.world_size)
@@ -443,6 +449,40 @@ def check_accumulation_flags(args):
     if args.batch_size % k:
         raise ValueError('--batch_size %d is not divisible by --accumulation_steps %d'
                          % (args.batch_size, k))
+
+
+def check_drop_path_flags(args):
+    """ValueError for --drop_path_rate outside [0, 1), and for a rate > 0 with --model tiny (no residual blocks)."""
+    p = getattr(args, 'drop_path_rate', 0.0)
+    if not 0.0 <= p < 1.0:
+        raise ValueError('--drop_path_rate must be in [0, 1), got %r' % (p,))
+    if p > 0 and args.model == 'tiny':
+        raise ValueError('--drop_path_rate is not supported with --model tiny: stochastic depth drops residual '
+                         'blocks, and TinyConvNet has none')
+
+
+def stochastic_depth_of(model):
+    """the ``ops.stochastic_depth.StochasticDepth`` of ``model`` (through a data-parallel wrapper), or None"""
+    return getattr(getattr(model, 'module', model), 'stochastic_depth', None)
+
+
+def save_stochastic_depth(state, model):
+    """checkpoint the draw counter under ``stochastic_depth`` (--drop_path_rate > 0 only)"""
+    sd = stochastic_depth_of(model)
+    if sd is not None:
+        state['stochastic_depth'] = sd.state_dict()
+
+
+def load_stochastic_depth(ckpt, state, model, log):
+    """--resume: continue the draw sequence where the checkpoint left it"""
+    sd = stochastic_depth_of(model)
+    if sd is None:
+        return
+    if 'stochastic_depth' in ckpt:
+        sd.load_state_dict(ckpt['stochastic_depth'])
+        state['stochastic_depth'] = ckpt['stochastic_depth']
+    else:
+        log.warning('checkpoint has no stochastic_depth: the drop masks start again from draw 0')
 
 
 def check_ema_flags(args, adpsgd=False):
@@ -745,9 +785,13 @@ def init_model(args):
     """ResNet (default resnet50) initialised as in "ImageNet in 1 hour"."""
     from .. import models
     kw = {} if args.model == 'tiny' else {'num_classes': args.num_classes}
+    if getattr(args, 'drop_path_rate', 0.0) > 0:
+        kw['drop_path_rate'] = args.drop_path_rate
     net = models.MODEL_ZOO[args.model](**kw)
     if isinstance(net, models.ResNet):
         models.init_imagenet_in_1hr(net)
+        if net.stochastic_depth is not None:
+            net.stochastic_depth.reseed(args.seed, args.rank)
     net = net.to(args.device)
     if args.channels_last and args.device == 'cuda':
         net = net.to(memory_format=torch.channels_last)

@@ -186,6 +186,7 @@ def main(argv=None):
     state = fresh_state(model.state_dict(), optimizer.state_dict())
     if args._ema is not None:
         state['model_ema'] = args._ema.state_dict()
+    common.save_stochastic_depth(state, model)
     cmanager = ClusterManager(rank=args.rank, world_size=args.world_size, model_tag=args.tag,
                               state=state, all_workers=args.checkpoint_all)
     if args.resume and os.path.isfile(cmanager.checkpoint_fpath):
@@ -204,6 +205,7 @@ def main(argv=None):
             else:
                 log.warning('checkpoint has no model_ema: the EMA starts again from the loaded model')
                 args._ema.reset()
+        common.load_stochastic_depth(ckpt, state, model, log)
         log.info("=> loaded checkpoint (epoch {}; itr {})".format(ckpt['epoch'], ckpt['itr']))
     elif args.resume:
         log.info("=> no checkpoint found at '{}'".format(cmanager.checkpoint_fpath))
@@ -241,6 +243,7 @@ def main(argv=None):
                 'data_meter': data_meter.__dict__, 'nn_meter': nn_meter.__dict__})
             if args._ema is not None:
                 state['model_ema'] = args._ema.state_dict()
+            common.save_stochastic_depth(state, model)
             prec1 = validate(args, val_loader, model, criterion, log)
             csv.val_row(epoch, batch_meter, nn_meter, data_meter, prec1)
             if args._ema is not None:

@@ -29,7 +29,8 @@ import torch.distributed as dist
 import torch.nn as nn
 
 from .common import (CSVLog, Meter, accuracy, build_parser, finalize_args, fresh_state,
-                     init_model, learning_rate_at, make_dataloader, update_state)
+                     init_model, learning_rate_at, load_stochastic_depth, make_dataloader,
+                     save_stochastic_depth, update_state)
 from ..experiment import ClusterManager, make_logger
 from ..utils import tracing
 from .common import device_batch, make_batch_mix, mix_train_batch, train_loss
@@ -100,6 +101,7 @@ def main(argv=None):
     args._batch_mix = make_batch_mix(args)
 
     state = fresh_state(model.state_dict(), optimizer.state_dict())
+    save_stochastic_depth(state, model)
     cmanager = ClusterManager(rank=args.rank, world_size=args.world_size, model_tag=args.tag,
                               state=state, all_workers=args.checkpoint_all)
     if args.resume and os.path.isfile(cmanager.checkpoint_fpath):
@@ -108,6 +110,7 @@ def main(argv=None):
         model.load_state_dict(ckpt['state_dict'])
         optimizer.load_state_dict(ckpt['optimizer'])
         model.gossip_flat.copy_(model.arena.flat)
+        load_stochastic_depth(ckpt, state, model, log)
     if args.rank == 0 and not args.resume and os.path.exists(args.shared_fpath):
         os.remove(args.shared_fpath)
     if dist.is_initialized():
@@ -136,6 +139,7 @@ def main(argv=None):
                 'state_dict': model.state_dict(), 'optimizer': optimizer.state_dict(),
                 'elapsed_time': time.time() - begin_time, 'batch_meter': batch_meter.__dict__,
                 'data_meter': data_meter.__dict__, 'nn_meter': nn_meter.__dict__})
+            save_stochastic_depth(state, model)
             prec1 = validate(args, val_loader, model, criterion, log)
             csv.val_row(local_epoch - 1, batch_meter, nn_meter, data_meter, prec1)
             if prec1 > best:

@@ -15,6 +15,11 @@ residual block and N(0, 0.01) weights in the classifier -- see
 :func:`init_imagenet_in_1hr`.  ``resnet50()`` here has the same 25,557,032
 parameters in the same order (161 tensors), so arenas, checkpoints and gossip
 message sizes match the reference's.
+
+Stochastic depth (``drop_path_rate=p > 0``, see :mod:`..ops.stochastic_depth`): a training forward draws
+the ``[L, N]`` branch scales of its ``L`` blocks in one launch and hands block ``l`` its row, which the
+block's last BN applies inside the fused kernels, ``relu(s_n * bn(conv(x)) + identity)``.  Eval-mode
+forwards and forwards inside ``precise_bn_stats`` draw nothing and scale nothing.
 """
 
 from __future__ import annotations
@@ -25,7 +30,8 @@ import torch
 import torch.nn as nn
 
 from ..ops.fused_bn import (FusedBatchNormAct2d as _BN, MaxPool2dNHWC, conv_bn_act, conv_bn_act_split,
-                             stem_conv)
+                             precise_bn_active, stem_conv)
+from ..ops.stochastic_depth import StochasticDepth
 
 
 def _conv3x3(cin, cout, stride=1):
@@ -52,10 +58,13 @@ class BasicBlock(nn.Module):
     def last_bn(self):
         return self.bn2
 
-    def forward(self, x):
+    def forward(self, x, branch_scale=None):
+        """``branch_scale``: the per-sample stochastic-depth scale of the residual branch, fp32 ``[N]``"""
         identity = x if self.downsample is None else conv_bn_act(self.downsample[0], self.downsample[1], x)
         out = self.bn1(self.conv1(x), relu=True)
-        return self.bn2(self.conv2(out), residual=identity, relu=True)
+        if branch_scale is None:
+            return self.bn2(self.conv2(out), residual=identity, relu=True)
+        return self.bn2(self.conv2(out), residual=identity, relu=True, branch_scale=branch_scale)
 
 
 class Bottleneck(nn.Module):
@@ -76,18 +85,21 @@ class Bottleneck(nn.Module):
     def last_bn(self):
         return self.bn3
 
-    def forward(self, x):
+    def forward(self, x, branch_scale=None):
+        """``branch_scale``: the per-sample stochastic-depth scale of the residual branch, fp32 ``[N]``"""
         # x feeds conv1 and the skip branch: the split op folds the skip gradient into conv1's dgrad
         out, skip = conv_bn_act_split(self.conv1, self.bn1, x, relu=True)
         identity = skip if self.downsample is None else conv_bn_act(self.downsample[0], self.downsample[1], skip)
         out = self.bn2(self.conv2(out), relu=True)
-        return conv_bn_act(self.conv3, self.bn3, out, residual=identity, relu=True)
+        return conv_bn_act(self.conv3, self.bn3, out, residual=identity, relu=True, branch_scale=branch_scale)
 
 
 class ResNet(nn.Module):
 
     def __init__(self, block: Type[nn.Module], layers: List[int], num_classes=1000,
-                 in_channels=3, base_width=64):
+                 in_channels=3, base_width=64, drop_path_rate=0.0):
+        """``drop_path_rate``: stochastic depth with timm's linear rule over the residual blocks (0 = off;
+        :attr:`stochastic_depth` is then None).  Seed it with ``model.stochastic_depth.reseed(seed, rank)``."""
         super().__init__()
         self.inplanes = base_width
         self.conv1 = nn.Conv2d(in_channels, base_width, 7, 2, 3, bias=False)
@@ -106,6 +118,10 @@ class ResNet(nn.Module):
             elif isinstance(m, nn.BatchNorm2d):
                 nn.init.ones_(m.weight)
                 nn.init.zeros_(m.bias)
+        if not 0.0 <= drop_path_rate < 1.0:
+            raise ValueError('drop_path_rate must be in [0, 1), got %r' % (drop_path_rate,))
+        # a plain attribute: no parameters or buffers, so state_dict keys and the arena are unchanged
+        self.stochastic_depth = StochasticDepth(sum(layers), drop_path_rate) if drop_path_rate > 0 else None
 
     def _make_layer(self, block, width, blocks, stride=1):
         downsample = None
@@ -119,7 +135,14 @@ class ResNet(nn.Module):
 
     def forward(self, x):
         x = self.maxpool(self.bn1(stem_conv(self.conv1, x), relu=True))
-        x = self.layer4(self.layer3(self.layer2(self.layer1(x))))
+        sd = self.stochastic_depth
+        if sd is None or not self.training or precise_bn_active():
+            x = self.layer4(self.layer3(self.layer2(self.layer1(x))))
+        else:
+            scales = sd.draw(x.shape[0], x.device)            # [L, N]: one launch
+            blocks = [b for layer in (self.layer1, self.layer2, self.layer3, self.layer4) for b in layer]
+            for l, (blk, rate) in enumerate(zip(blocks, sd.rates)):
+                x = blk(x, scales[l] if rate > 0 else None)
         x = torch.flatten(self.avgpool(x), 1)
         return self.fc(x)
 

@@ -39,6 +39,19 @@ cudaError_t bn_launch_bwd_finalize(const float* partial, int G, long long M, int
 cudaError_t bn_launch_bwd_dx(int dtype, int mode, const void* dz, const void* x, const float* scale,
                              const float* shift, const float* c2, const float* c3, void* dx,
                              long long M, int C, int G, cudaStream_t st);
+cudaError_t bn_launch_apply_drop(int dtype, const void* x, const void* res, const float* scale, const float* shift,
+                                 void* y, uint8_t* mask, const float* sdrop, int hw, long long M, int C, int G,
+                                 cudaStream_t st);
+cudaError_t bn_launch_bwd_reduce_drop(int dtype, const void* dy, const void* x, const void* y, const float* mean,
+                                      const float* invstd, float* partial, void* dz, const float* sdrop, int hw,
+                                      long long M, int C, int G, cudaStream_t st);
+cudaError_t bn_launch_bwd_dx_drop(int dtype, const void* dz, const void* x, const float* scale, const float* c2,
+                                  const float* c3, void* dx, const float* sdrop, int hw, long long M, int C, int G,
+                                  cudaStream_t st);
+int drop_path_max_blocks();
+cudaError_t drop_path_launch_draw(const unsigned int* thresh, const float* keep_scale, int L, int n,
+                                  unsigned long long seed, unsigned long long rank, long long* counter, float* out,
+                                  cudaStream_t st);
 }
 
 extern std::atomic<long long> g_sgp_kernel_launches;       // bindings.cpp
@@ -94,6 +107,21 @@ static double* bn_acc_ptr(const c10::optional<torch::Tensor>& acc, const torch::
     return acc->data_ptr<double>();
 }
 
+// branch_scale (stochastic depth): a contiguous fp32 [n] tensor on x's device, one value per sample of x, whose
+// M rows are n samples of hw = M / n rows each (4-D x: n = x.size(0)); or None.  Returns its pointer and sets hw.
+static const float* branch_scale_ptr(const c10::optional<torch::Tensor>& s, const torch::Tensor& x, long long M,
+                                     int& hw)
+{
+    hw = 1;
+    if (!s.has_value() || !s->defined()) return nullptr;
+    TORCH_CHECK(s->is_cuda() && s->get_device() == x.get_device() && s->scalar_type() == torch::kFloat32 &&
+                    s->is_contiguous() && s->dim() == 1 && s->numel() >= 1 && M % s->numel() == 0 &&
+                    (x.dim() != 4 || s->numel() == x.size(0)) && M < (1LL << 31),
+                "branch_scale must be a contiguous fp32 [N] tensor on x's device, one value per sample");
+    hw = (int)(M / s->numel());
+    return s->data_ptr<float>();
+}
+
 // returns (y, mean, invstd, scale, shift)
 static std::vector<torch::Tensor> bn_forward(torch::Tensor x, c10::optional<torch::Tensor> residual,
                                              torch::Tensor gamma, torch::Tensor beta,
@@ -101,7 +129,8 @@ static std::vector<torch::Tensor> bn_forward(torch::Tensor x, c10::optional<torc
                                              c10::optional<torch::Tensor> running_var,
                                              c10::optional<torch::Tensor> num_batches_tracked,
                                              bool training, double momentum, double eps, bool relu,
-                                             c10::optional<torch::Tensor> acc)
+                                             c10::optional<torch::Tensor> acc,
+                                             c10::optional<torch::Tensor> branch_scale)
 {
     long long M; int C;
     nhwc_dims(x, M, C);
@@ -140,16 +169,25 @@ static std::vector<torch::Tensor> bn_forward(torch::Tensor x, c10::optional<torc
                                       running_mean->data_ptr<float>(), running_var->data_ptr<float>(),
                                       (float)eps, scale, shift, st));
     }
+    int hw;
+    const float* sdrop = branch_scale_ptr(branch_scale, x, M, hw);
+    if (sdrop != nullptr) {
+        TORCH_CHECK(has_res && relu && training, "bn_forward: branch_scale needs a residual, relu and training mode");
+        BN_CHECK(bn_launch_apply_drop(dt, x.data_ptr(), residual->data_ptr(), scale, shift, y.data_ptr(), nullptr,
+                                      sdrop, hw, M, C, 0, st));
+        return {y, coef};
+    }
     BN_CHECK(bn_launch_apply(dt, relu ? 1 : 0, has_res ? 1 : 0, x.data_ptr(),
                              has_res ? residual->data_ptr() : nullptr, scale, shift, y.data_ptr(), nullptr,
                              M, C, 0, st));
     return {y, coef};
 }
 
-// returns (dx, dres or undefined, grad_gamma, grad_beta)
+// returns (dx, dres or undefined, grad_gamma, grad_beta).  branch_scale (residual + relu only): the forward's
+// per-sample scale s of the BN output; dres = dy * (y > 0) unscaled, the BN's gradient is s * dres
 static std::vector<torch::Tensor> bn_backward(torch::Tensor dy, torch::Tensor x,
                                               c10::optional<torch::Tensor> y, torch::Tensor coef,
-                                              bool relu, bool add)
+                                              bool relu, bool add, c10::optional<torch::Tensor> branch_scale)
 {
     long long M; int C;
     nhwc_dims(x, M, C);
@@ -171,6 +209,19 @@ static std::vector<torch::Tensor> bn_backward(torch::Tensor dy, torch::Tensor x,
     float* gg = grads.data_ptr<float>();
     torch::Tensor dz;
     if (mode == 2) dz = torch::empty_like(x);
+    int hw;
+    const float* sdrop = branch_scale_ptr(branch_scale, x, M, hw);
+    if (sdrop != nullptr) {
+        TORCH_CHECK(mode == 2, "bn_backward: branch_scale needs a residual and relu");
+        BN_CHECK(bn_launch_bwd_reduce_drop(dt, dy.data_ptr(), x.data_ptr(), y->data_ptr(), mean, invstd,
+                                           partial.data_ptr<float>(), dz.data_ptr(), sdrop, hw, M, C, G, st));
+        BN_CHECK(bn_launch_bwd_finalize(partial.data_ptr<float>(), G, M, C, scale, mean, invstd,
+                                        gg, gg + C, gg + 2 * C, gg + 3 * C, st));
+        auto dx = torch::empty_like(x);
+        BN_CHECK(bn_launch_bwd_dx_drop(dt, dz.data_ptr(), x.data_ptr(), scale, gg + 2 * C, gg + 3 * C, dx.data_ptr(),
+                                       sdrop, hw, M, C, 0, st));
+        return {dx, dz, grads.select(0, 0), grads.select(0, 1)};
+    }
     BN_CHECK(bn_launch_bwd_reduce(dt, mode, dy.data_ptr(), x.data_ptr(),
                                   mode == 2 ? y->data_ptr() : nullptr, scale, shift, mean, invstd,
                                   partial.data_ptr<float>(), mode == 2 ? dz.data_ptr() : nullptr,
@@ -185,9 +236,11 @@ static std::vector<torch::Tensor> bn_backward(torch::Tensor dy, torch::Tensor x,
 }
 
 // bn_backward's finalize + dx passes for a dz whose reduction partial[G][2][C] (sum dz, sum dz * xhat)
-// was produced elsewhere (the MODE 3 dgrad epilogue); returns (dx, grad_gamma, grad_beta)
+// was produced elsewhere (the MODE 3 dgrad epilogue); returns (dx, grad_gamma, grad_beta).  branch_scale: as in
+// bn_backward (the partials are then those of s * dz)
 static std::vector<torch::Tensor> bn_backward_from_partials(torch::Tensor dz, torch::Tensor x, torch::Tensor coef,
-                                                            torch::Tensor partial)
+                                                            torch::Tensor partial,
+                                                            c10::optional<torch::Tensor> branch_scale)
 {
     long long M; int C;
     nhwc_dims(x, M, C);
@@ -204,8 +257,14 @@ static std::vector<torch::Tensor> bn_backward_from_partials(torch::Tensor dz, to
     BN_CHECK(bn_launch_bwd_finalize(partial.data_ptr<float>(), (int)partial.size(0), M, C, scale, mean, invstd,
                                     gg, gg + C, gg + 2 * C, gg + 3 * C, st));
     auto dx = torch::empty_like(x);
-    BN_CHECK(bn_launch_bwd_dx(dt, 0, dz.data_ptr(), x.data_ptr(), scale, shift, gg + 2 * C, gg + 3 * C,
-                              dx.data_ptr(), M, C, 0, st));
+    int hw;
+    const float* sdrop = branch_scale_ptr(branch_scale, x, M, hw);
+    if (sdrop != nullptr)
+        BN_CHECK(bn_launch_bwd_dx_drop(dt, dz.data_ptr(), x.data_ptr(), scale, gg + 2 * C, gg + 3 * C, dx.data_ptr(),
+                                       sdrop, hw, M, C, 0, st));
+    else
+        BN_CHECK(bn_launch_bwd_dx(dt, 0, dz.data_ptr(), x.data_ptr(), scale, shift, gg + 2 * C, gg + 3 * C,
+                                  dx.data_ptr(), M, C, 0, st));
     return {dx, grads.select(0, 0), grads.select(0, 1)};
 }
 
@@ -463,6 +522,10 @@ cudaError_t c1_launch_stats_finalize(const float* partial, int R, int C, const f
 cudaError_t c1_launch_gemm_bn_eval(const void* x, const void* w, void* y, long long M, int N, int K,
                                    const void* residual, const float* gamma, const float* beta, const float* mean,
                                    const float* var, float eps, int relu, int num_sms, int f32, cudaStream_t st);
+cudaError_t c1_launch_gemm_bn_reduce_drop(const void* x, const void* w, void* y, long long M, int N, int K,
+                                          float* partial, const void* residual, const void* bn_x, const float* coef,
+                                          const uint8_t* mask, const float* sdrop, int hw, int num_sms, int f32,
+                                          cudaStream_t st);
 }
 
 // x: NHWC bf16 / fp32 activation (4-D channels_last) or [M, K] matrix; w: [N, K, 1, 1] or [N, K], rows
@@ -543,9 +606,10 @@ static torch::Tensor conv1x1_forward(torch::Tensor x, torch::Tensor w, bool with
 // MODE 3: dz = mask ? x . w^T + residual : 0 and the backward reduction of the BatchNorm (+ residual
 // + ReLU) whose input was bn_x, output mask `mask` ([M, N/8] uint8) and coefficients `coef` ([4, N]:
 // mean, invstd, scale, shift).  Returns (dz, partial[R][2][N]) for bn_backward_from_partials.
+// branch_scale: that BatchNorm's stochastic-depth scale (bn_forward); the partials are then those of s * dz
 static std::vector<torch::Tensor> conv1x1_dgrad_bn_reduce(torch::Tensor x, torch::Tensor w, torch::Tensor residual,
                                                           torch::Tensor bn_x, torch::Tensor coef, torch::Tensor mask,
-                                                          int num_sms)
+                                                          int num_sms, c10::optional<torch::Tensor> branch_scale)
 {
     TORCH_CHECK(conv1x1_can_fuse(x, w), "conv1x1_dgrad_bn_reduce: unsupported tensors");
     const int K = (int)x.size(1), N = (int)w.size(0);
@@ -565,9 +629,17 @@ static std::vector<torch::Tensor> conv1x1_dgrad_bn_reduce(torch::Tensor x, torch
     const int sms = plan_sms(num_sms);
     auto partial = torch::empty({c1_partial_rows(M, N, K, sms, 1, f32), 2, N},
                                 torch::TensorOptions().dtype(torch::kFloat32).device(x.device()));
-    BN_CHECK(c1_launch_gemm(x.data_ptr(), w.data_ptr(), y.data_ptr(), M, N, K, partial.data_ptr<float>(),
-                            residual.data_ptr(), bn_x.data_ptr(), coef.data_ptr<float>(), mask.data_ptr<uint8_t>(),
-                            sms, f32, at::cuda::getCurrentCUDAStream()));
+    int hw;
+    const float* sdrop = branch_scale_ptr(branch_scale, y, M, hw);
+    if (sdrop != nullptr)
+        BN_CHECK(c1_launch_gemm_bn_reduce_drop(x.data_ptr(), w.data_ptr(), y.data_ptr(), M, N, K,
+                                               partial.data_ptr<float>(), residual.data_ptr(), bn_x.data_ptr(),
+                                               coef.data_ptr<float>(), mask.data_ptr<uint8_t>(), sdrop, hw, sms, f32,
+                                               at::cuda::getCurrentCUDAStream()));
+    else
+        BN_CHECK(c1_launch_gemm(x.data_ptr(), w.data_ptr(), y.data_ptr(), M, N, K, partial.data_ptr<float>(),
+                                residual.data_ptr(), bn_x.data_ptr(), coef.data_ptr<float>(), mask.data_ptr<uint8_t>(),
+                                sms, f32, at::cuda::getCurrentCUDAStream()));
     return {y, partial};
 }
 
@@ -582,7 +654,8 @@ static std::vector<torch::Tensor> conv1x1_bn_forward(torch::Tensor x, torch::Ten
                                                      c10::optional<torch::Tensor> num_batches_tracked,
                                                      double momentum, double eps, bool relu,
                                                      c10::optional<torch::Tensor> mask, int num_sms,
-                                                     c10::optional<torch::Tensor> acc)
+                                                     c10::optional<torch::Tensor> acc,
+                                                     c10::optional<torch::Tensor> branch_scale)
 {
     TORCH_CHECK(conv1x1_can_fuse(x, w), "conv1x1_bn_forward: unsupported tensors");
     const int K = (int)x.size(1), N = (int)w.size(0);
@@ -621,6 +694,15 @@ static std::vector<torch::Tensor> conv1x1_bn_forward(torch::Tensor x, torch::Ten
                                       beta.data_ptr<float>(), rm, rv, nbt, accp, (float)momentum, (float)eps,
                                       mean, mean + N, mean + 2 * N, mean + 3 * N, st));
     auto out = torch::empty_like(yraw);
+    int hw;
+    const float* sdrop = branch_scale_ptr(branch_scale, yraw, M, hw);
+    if (sdrop != nullptr) {
+        TORCH_CHECK(has_res && relu, "conv1x1_bn_forward: branch_scale needs a residual and relu");
+        BN_CHECK(bn_launch_apply_drop(f32, yraw.data_ptr(), residual->data_ptr(), mean + 2 * N, mean + 3 * N,
+                                      out.data_ptr(), has_mask ? mask->data_ptr<uint8_t>() : nullptr, sdrop, hw, M, N,
+                                      0, st));
+        return {yraw, out, coef};
+    }
     BN_CHECK(bn_launch_apply(f32, relu ? 1 : 0, has_res ? 1 : 0, yraw.data_ptr(),
                              has_res ? residual->data_ptr() : nullptr, mean + 2 * N, mean + 3 * N,
                              out.data_ptr(), has_mask ? mask->data_ptr<uint8_t>() : nullptr, M, N, 0, st));
@@ -785,8 +867,42 @@ static void batch_mix(torch::Tensor src, torch::Tensor out, torch::Tensor mix)
                               at::cuda::getCurrentCUDAStream()));
 }
 
+// ---------------------------------------------------------------------------
+// stochastic depth: the per-sample residual-branch scales of one training forward (csrc/drop_path_kernels.cu)
+// ---------------------------------------------------------------------------
+// returns a fresh fp32 [L, n] tensor on counter's device; thresh[l] in [0, 2^24] and keep_scale[l] per block;
+// counter: a contiguous int64 [1] CUDA tensor, read and incremented by the launch
+static torch::Tensor drop_path_draw(torch::Tensor counter, int64_t seed, int64_t rank,
+                                    const std::vector<int64_t>& thresh, const std::vector<double>& keep_scale,
+                                    int64_t n)
+{
+    TORCH_CHECK(counter.is_cuda() && counter.scalar_type() == torch::kInt64 && counter.is_contiguous() &&
+                    counter.numel() == 1,
+                "drop_path_draw: counter must be a contiguous int64 [1] CUDA tensor");
+    const int64_t L = (int64_t)thresh.size();
+    TORCH_CHECK(L >= 1 && L <= drop_path_max_blocks() && (int64_t)keep_scale.size() == L,
+                "drop_path_draw: thresh and keep_scale must have the same length, 1 to ", drop_path_max_blocks());
+    TORCH_CHECK(n >= 1 && L * n < (1LL << 31), "drop_path_draw: bad sample count ", n);
+    std::vector<unsigned int> th((size_t)L);
+    std::vector<float> ks((size_t)L);
+    for (int64_t l = 0; l < L; ++l) {
+        TORCH_CHECK(thresh[l] >= 0 && thresh[l] <= (1LL << 24), "drop_path_draw: thresh must be in [0, 2^24]");
+        th[l] = (unsigned int)thresh[l];
+        ks[l] = (float)keep_scale[l];
+    }
+    c10::cuda::CUDAGuard guard(counter.get_device());
+    auto out = torch::empty({L, n}, counter.options().dtype(torch::kFloat32));
+    BN_CHECK(drop_path_launch_draw(th.data(), ks.data(), (int)L, (int)n, (unsigned long long)seed,
+                                   (unsigned long long)rank, reinterpret_cast<long long*>(counter.data_ptr<int64_t>()),
+                                   out.data_ptr<float>(), at::cuda::getCurrentCUDAStream()));
+    return out;
+}
+
 void bind_bn(py::module& mod)
 {
+    mod.def("drop_path_draw", &drop_path_draw, py::arg("counter"), py::arg("seed"), py::arg("rank"),
+            py::arg("thresh"), py::arg("keep_scale"), py::arg("n"));
+    mod.attr("DROP_PATH_MAX_BLOCKS") = drop_path_max_blocks();
     mod.def("xent_can_fuse", &xent_can_fuse);
     mod.def("xent_forward", &xent_forward, py::arg("logits"), py::arg("target"), py::arg("label_smoothing") = 0.0,
             py::arg("mix") = py::none());
@@ -802,9 +918,11 @@ void bind_bn(py::module& mod)
     mod.def("conv1x1_bn_forward", &conv1x1_bn_forward, py::arg("x"), py::arg("w"), py::arg("residual"),
             py::arg("gamma"), py::arg("beta"), py::arg("running_mean"), py::arg("running_var"),
             py::arg("num_batches_tracked"), py::arg("momentum"), py::arg("eps"), py::arg("relu"),
-            py::arg("mask") = py::none(), py::kw_only(), py::arg("num_sms") = 0, py::arg("acc") = py::none());
+            py::arg("mask") = py::none(), py::kw_only(), py::arg("num_sms") = 0, py::arg("acc") = py::none(),
+            py::arg("branch_scale") = py::none());
     mod.def("conv1x1_dgrad_bn_reduce", &conv1x1_dgrad_bn_reduce, py::arg("x"), py::arg("w"), py::arg("residual"),
-            py::arg("bn_x"), py::arg("coef"), py::arg("mask"), py::kw_only(), py::arg("num_sms") = 0);
+            py::arg("bn_x"), py::arg("coef"), py::arg("mask"), py::kw_only(), py::arg("num_sms") = 0,
+            py::arg("branch_scale") = py::none());
     mod.def("conv1x1_bn_eval", &conv1x1_bn_eval, py::arg("x"), py::arg("w"), py::arg("gamma"), py::arg("beta"),
             py::arg("mean"), py::arg("var"), py::arg("eps"), py::arg("relu"), py::arg("residual") = py::none(),
             py::kw_only(), py::arg("num_sms") = 0);
@@ -817,12 +935,15 @@ void bind_bn(py::module& mod)
     mod.def("bn_can_fuse", &bn_can_fuse);
     mod.def("bn_forward", &bn_forward, py::arg("x"), py::arg("residual"), py::arg("gamma"), py::arg("beta"),
             py::arg("running_mean"), py::arg("running_var"), py::arg("num_batches_tracked"), py::arg("training"),
-            py::arg("momentum"), py::arg("eps"), py::arg("relu"), py::arg("acc") = py::none());
+            py::arg("momentum"), py::arg("eps"), py::arg("relu"), py::arg("acc") = py::none(),
+            py::arg("branch_scale") = py::none());
     mod.def("bn_stats_commit", &bn_stats_commit, py::arg("acc"), py::arg("running_mean"), py::arg("running_var"),
             py::arg("k"), "running = fp32(acc / k) for every BatchNorm layer: one launch per BN_COMMIT_MAX_SEGS layers");
     mod.attr("BN_COMMIT_MAX_SEGS") = bn_commit_max_segs();
-    mod.def("bn_backward", &bn_backward);
-    mod.def("bn_backward_from_partials", &bn_backward_from_partials);
+    mod.def("bn_backward", &bn_backward, py::arg("dy"), py::arg("x"), py::arg("y"), py::arg("coef"), py::arg("relu"),
+            py::arg("add"), py::arg("branch_scale") = py::none());
+    mod.def("bn_backward_from_partials", &bn_backward_from_partials, py::arg("dz"), py::arg("x"), py::arg("coef"),
+            py::arg("partial"), py::arg("branch_scale") = py::none());
     mod.def("bn_f32_map", &bn_f32_map, py::arg("value") = -1,
             "fp32 BatchNorm channel map: returns the one in use (1 = split, 0 = consecutive); "
             "value >= 0 selects one for the launches that follow");

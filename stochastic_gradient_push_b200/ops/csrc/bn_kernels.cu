@@ -9,6 +9,9 @@
 //              the ReLU mask is recomputed from x*scale+shift (no mask tensor, no
 //              extra read); with a residual the mask comes from the saved output
 //              and dz is written once because it IS the residual branch's grad.
+//   stochastic depth (DROP): the BN output of a residual block is scaled per sample before the add,
+//              y = relu((x*scale + shift)*s[row / HW] + res); the backward reduces s*dz and forms
+//              dx from s*dz, the residual-branch gradient dz stays unscaled
 //   precise statistics: the finalize adds the batch statistics to an fp64 accumulator
 //              instead of the running update; one commit launch per pass writes
 //              running = fp32(sum / K) for every layer (GossipTrainer.update_bn)
@@ -293,10 +296,13 @@ __global__ void bn_eval_coeff_kernel(int C, const float* __restrict__ gamma, con
 // With the SPLIT map a byte's 8 channels belong to two neighbouring lanes (C % 16 == 0): the even
 // lane of a pair stores the byte of their first halves, the odd lane the byte of their second halves.
 // ---------------------------------------------------------------------------
-template <typename T, bool RELU, bool ADD, bool MASK = false, bool SPLIT = false>
-__global__ void __launch_bounds__(BN_THREADS, (sizeof(T) == 4 && ADD) ? 3 : 4)     // fp32 + residual: 80 registers
-bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, const float* __restrict__ scale,
-                const float* __restrict__ shift, T* __restrict__ y, uint8_t* __restrict__ mask, long long M, int C)
+// DROP (stochastic depth, with RELU && ADD): y = relu((x*scale + shift)*s[row / hw] + res), s the residual
+// branch's per-sample scale [M / hw]; the mask is still that of y.
+template <typename T, bool RELU, bool ADD, bool MASK, bool SPLIT, bool DROP>
+__device__ __forceinline__ void
+bn_apply_body(const T* __restrict__ x, const T* __restrict__ res, const float* __restrict__ scale,
+              const float* __restrict__ shift, T* __restrict__ y, uint8_t* __restrict__ mask, long long M, int C,
+              const float* __restrict__ sdrop, int hw)
 {
     const Map<SPLIT> mp(C);
     if (!mp.active) return;
@@ -322,12 +328,14 @@ bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, const float*
                 const F8 d = Io<T>::decode(dr[u]);
                 F8 a;
                 if (ADD) a = Io<T>::decode(ar[u]);
+                const float sr = DROP ? __ldg(sdrop + (int)rr / hw) : 1.f;
                 F8 o;
                 uint32_t bits = 0;
 #pragma unroll
                 for (int i = 0; i < 8; ++i) {
                     float v = fmaf(d.v[i], sc.v[i], sh.v[i]);
-                    if (ADD) v += a.v[i];
+                    if (DROP) v = fmaf(v, sr, a.v[i]);
+                    else if (ADD) v += a.v[i];
                     if (RELU) v = fmaxf(v, 0.f);
                     o.v[i] = v;
                     if (MASK) {     // the sign of y as stored (bf16 rounds the tiniest positives to 0)
@@ -348,17 +356,37 @@ bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, const float*
     }
 }
 
+template <typename T, bool RELU, bool ADD, bool MASK = false, bool SPLIT = false>
+__global__ void __launch_bounds__(BN_THREADS, (sizeof(T) == 4 && ADD) ? 3 : 4)     // fp32 + residual: 80 registers
+bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, const float* __restrict__ scale,
+                const float* __restrict__ shift, T* __restrict__ y, uint8_t* __restrict__ mask, long long M, int C)
+{
+    bn_apply_body<T, RELU, ADD, MASK, SPLIT, false>(x, res, scale, shift, y, mask, M, C, nullptr, 1);
+}
+
+// 3 CTAs per SM for both dtypes: with the per-row scale the bf16 kernel spilled under a 64-register cap
+template <typename T, bool MASK, bool SPLIT>
+__global__ void __launch_bounds__(BN_THREADS, 3)
+bn_apply_drop_kernel(const T* __restrict__ x, const T* __restrict__ res, const float* __restrict__ scale,
+                     const float* __restrict__ shift, T* __restrict__ y, uint8_t* __restrict__ mask, long long M,
+                     int C, const float* __restrict__ sdrop, int hw)
+{
+    bn_apply_body<T, true, true, MASK, SPLIT, true>(x, res, scale, shift, y, mask, M, C, sdrop, hw);
+}
+
 // ---------------------------------------------------------------------------
 // backward: reduce   partial[.][0] = sum dz ; partial[.][1] = sum dz * xhat
 // MODE 0: dz = dy            MODE 1: dz = dy * (x*scale+shift > 0)
 // MODE 2: dz = dy * (y > 0), dz is also written (gradient of the residual branch)
+// DROP (MODE 2): dz is written unscaled, the partials are those of s[row / hw] * dz, the BN output's gradient
 // ---------------------------------------------------------------------------
-template <typename T, int MODE, bool SPLIT = false>
-__global__ void __launch_bounds__(BN_THREADS, 3)
-bn_bwd_reduce_kernel(const T* __restrict__ dy, const T* __restrict__ x, const T* __restrict__ y,
-                     const float* __restrict__ scale, const float* __restrict__ shift,
-                     const float* __restrict__ mean, const float* __restrict__ invstd,
-                     float* __restrict__ partial, T* __restrict__ dz_out, long long M, int C)
+template <typename T, int MODE, bool SPLIT, bool DROP>
+__device__ __forceinline__ void
+bn_bwd_reduce_body(const T* __restrict__ dy, const T* __restrict__ x, const T* __restrict__ y,
+                   const float* __restrict__ scale, const float* __restrict__ shift,
+                   const float* __restrict__ mean, const float* __restrict__ invstd,
+                   float* __restrict__ partial, T* __restrict__ dz_out, long long M, int C,
+                   const float* __restrict__ sdrop, int hw)
 {
     const Map<SPLIT> mp(C);
     F8 s, q;
@@ -371,13 +399,16 @@ bn_bwd_reduce_kernel(const T* __restrict__ dy, const T* __restrict__ x, const T*
         F8 sc, sh;
         if (MODE == 1) { sc = load_c8(scale + off, mp.h); sh = load_c8(shift + off, mp.h); }
         const long long stride = (long long)gridDim.x * mp.rpi;
-        constexpr int UN = Unroll<T>::RED;
+        // DROP: one row in flight per tensor (bf16 spilled at two under the 80-register cap)
+        constexpr int UN = DROP ? 1 : Unroll<T>::RED;
         for (long long r = (long long)blockIdx.x * mp.rpi + mp.rl; r < M; r += UN * stride) {
             typename Io<T>::raw_t gr[UN], xr[UN], yr[UN];
+            float srv[UN];
 #pragma unroll
             for (int u = 0; u < UN; ++u) {
                 const long long rr = r + u * stride;
                 if (rr < M) {
+                    if (DROP) srv[u] = __ldg(sdrop + (int)rr / hw);
                     gr[u] = Io<T>::load_raw(dy + rr * C + off, mp.h);
                     xr[u] = Io<T>::load_raw(x + rr * C + off, mp.h);
                     if (MODE == 2) yr[u] = Io<T>::load_raw(y + rr * C + off, mp.h);
@@ -391,6 +422,7 @@ bn_bwd_reduce_kernel(const T* __restrict__ dy, const T* __restrict__ x, const T*
                     const F8 d = Io<T>::decode(xr[u]);
                     F8 o;
                     if (MODE == 2) o = Io<T>::decode(yr[u]);
+                    const float sr = DROP ? srv[u] : 1.f;
                     F8 dz;
 #pragma unroll
                     for (int i = 0; i < 8; ++i) {
@@ -398,6 +430,7 @@ bn_bwd_reduce_kernel(const T* __restrict__ dy, const T* __restrict__ x, const T*
                         if (MODE == 1) gz = (fmaf(d.v[i], sc.v[i], sh.v[i]) > 0.f) ? gz : 0.f;
                         if (MODE == 2) gz = (o.v[i] > 0.f) ? gz : 0.f;
                         dz.v[i] = gz;
+                        if (DROP) gz *= sr;
                         s.v[i] += gz;
                         q.v[i] = fmaf(gz, (d.v[i] - mu.v[i]) * is.v[i], q.v[i]);
                     }
@@ -407,6 +440,26 @@ bn_bwd_reduce_kernel(const T* __restrict__ dy, const T* __restrict__ x, const T*
         }
     }
     reduce_store_partials(mp, s, q, partial, C);
+}
+
+template <typename T, int MODE, bool SPLIT = false>
+__global__ void __launch_bounds__(BN_THREADS, 3)
+bn_bwd_reduce_kernel(const T* __restrict__ dy, const T* __restrict__ x, const T* __restrict__ y,
+                     const float* __restrict__ scale, const float* __restrict__ shift,
+                     const float* __restrict__ mean, const float* __restrict__ invstd,
+                     float* __restrict__ partial, T* __restrict__ dz_out, long long M, int C)
+{
+    bn_bwd_reduce_body<T, MODE, SPLIT, false>(dy, x, y, scale, shift, mean, invstd, partial, dz_out, M, C, nullptr, 1);
+}
+
+template <typename T, bool SPLIT>
+__global__ void __launch_bounds__(BN_THREADS, 3)
+bn_bwd_reduce_drop_kernel(const T* __restrict__ dy, const T* __restrict__ x, const T* __restrict__ y,
+                          const float* __restrict__ mean, const float* __restrict__ invstd,
+                          float* __restrict__ partial, T* __restrict__ dz_out, long long M, int C,
+                          const float* __restrict__ sdrop, int hw)
+{
+    bn_bwd_reduce_body<T, 2, SPLIT, true>(dy, x, y, nullptr, nullptr, mean, invstd, partial, dz_out, M, C, sdrop, hw);
 }
 
 // per-channel: grad_gamma, grad_beta and the dx coefficients
@@ -433,11 +486,13 @@ bn_bwd_finalize_kernel(const float* __restrict__ partial, int G, long long M, in
 
 // MODE 0/2: dz given directly (dy, or the dz written by the reduce kernel)
 // MODE 1  : dz = dy * (x*scale+shift > 0) recomputed
-template <typename T, int MODE, bool SPLIT = false>
-__global__ void __launch_bounds__(BN_THREADS, 3)
-bn_bwd_dx_kernel(const T* __restrict__ dz_in, const T* __restrict__ x, const float* __restrict__ scale,
-                 const float* __restrict__ shift, const float* __restrict__ c2,
-                 const float* __restrict__ c3, T* __restrict__ dx, long long M, int C)
+// DROP (MODE 0): dx = c1*(s[row / hw]*dz) - c2*x + c3 for the unscaled residual-branch gradient dz
+template <typename T, int MODE, bool SPLIT, bool DROP>
+__device__ __forceinline__ void
+bn_bwd_dx_body(const T* __restrict__ dz_in, const T* __restrict__ x, const float* __restrict__ scale,
+               const float* __restrict__ shift, const float* __restrict__ c2,
+               const float* __restrict__ c3, T* __restrict__ dx, long long M, int C,
+               const float* __restrict__ sdrop, int hw)
 {
     // fp32 MODE 1 reads the shift from shared memory at each row: 4 x 8 constants in registers
     // next to 2 x 2 x 8 loads in flight do not fit its 80-register cap (they spilled)
@@ -474,17 +529,37 @@ bn_bwd_dx_kernel(const T* __restrict__ dz_in, const T* __restrict__ x, const flo
                 const F8 g = Io<T>::decode(gr[u]);
                 const F8 d = Io<T>::decode(xr[u]);
                 if (SH_SMEM) sh = load_c8(sh_s + off, mp.h);
+                const float sr = DROP ? __ldg(sdrop + (int)rr / hw) : 1.f;
                 F8 o;
 #pragma unroll
                 for (int i = 0; i < 8; ++i) {
                     float gz = g.v[i];
                     if (MODE == 1) gz = (fmaf(d.v[i], k1.v[i], sh.v[i]) > 0.f) ? gz : 0.f;
+                    if (DROP) gz *= sr;
                     o.v[i] = fmaf(k1.v[i], gz, fmaf(-k2.v[i], d.v[i], k3.v[i]));
                 }
                 Io<T>::store(dx + rr * C + off, o, mp.h);
             }
         }
     }
+}
+
+template <typename T, int MODE, bool SPLIT = false>
+__global__ void __launch_bounds__(BN_THREADS, 3)
+bn_bwd_dx_kernel(const T* __restrict__ dz_in, const T* __restrict__ x, const float* __restrict__ scale,
+                 const float* __restrict__ shift, const float* __restrict__ c2,
+                 const float* __restrict__ c3, T* __restrict__ dx, long long M, int C)
+{
+    bn_bwd_dx_body<T, MODE, SPLIT, false>(dz_in, x, scale, shift, c2, c3, dx, M, C, nullptr, 1);
+}
+
+template <typename T, bool SPLIT>
+__global__ void __launch_bounds__(BN_THREADS, 3)
+bn_bwd_dx_drop_kernel(const T* __restrict__ dz_in, const T* __restrict__ x, const float* __restrict__ scale,
+                      const float* __restrict__ c2, const float* __restrict__ c3, T* __restrict__ dx, long long M,
+                      int C, const float* __restrict__ sdrop, int hw)
+{
+    bn_bwd_dx_body<T, 0, SPLIT, true>(dz_in, x, scale, nullptr, c2, c3, dx, M, C, sdrop, hw);
 }
 
 // ---------------------------------------------------------------------------
@@ -626,6 +701,25 @@ cudaError_t bn_launch_apply(int dtype, int relu, int add, const void* x, const v
     return cudaGetLastError();
 }
 
+#define BN_APPLY_DROP(T, MK, S) bn_apply_drop_kernel<T, MK, S><<<G, BN_THREADS, 0, st>>>( \
+    (const T*)x, (const T*)res, scale, shift, (T*)y, mask, M, C, sdrop, hw)
+
+// stochastic depth: bn_launch_apply with relu and a residual, the BN output scaled by sdrop[row / hw]
+// (sdrop: fp32 [M / hw], M < 2^31); mask nullable as there
+cudaError_t bn_launch_apply_drop(int dtype, const void* x, const void* res, const float* scale, const float* shift,
+                                 void* y, uint8_t* mask, const float* sdrop, int hw, long long M, int C, int G,
+                                 cudaStream_t st)
+{
+    const bool split = dtype == 1 && f32_split();
+    if (hw < 1 || M % hw != 0 || M >= (1LL << 31) || (mask != nullptr && split && C % 16 != 0))
+        return cudaErrorInvalidValue;
+    if (G <= 0) G = bn_grid(M, C, 6);           // 3 CTAs/SM resident -> 2 waves
+    if (dtype == 0) { if (mask) BN_APPLY_DROP(__nv_bfloat16, true, false); else BN_APPLY_DROP(__nv_bfloat16, false, false); }
+    else if (split) { if (mask) BN_APPLY_DROP(float, true, true); else BN_APPLY_DROP(float, false, true); }
+    else            { if (mask) BN_APPLY_DROP(float, true, false); else BN_APPLY_DROP(float, false, false); }
+    return cudaGetLastError();
+}
+
 #define BN_RED(T, MODE, S) bn_bwd_reduce_kernel<T, MODE, S><<<G, BN_THREADS, 0, st>>>( \
     (const T*)dy, (const T*)x, (const T*)y, scale, shift, mean, invstd, partial, (T*)dz, M, C)
 
@@ -642,6 +736,21 @@ cudaError_t bn_launch_bwd_reduce(int dtype, int mode, const void* dy, const void
     } else {
         if (mode == 0) BN_RED(float, 0, false); else if (mode == 1) BN_RED(float, 1, false); else BN_RED(float, 2, false);
     }
+    return cudaGetLastError();
+}
+
+#define BN_RED_DROP(T, S) bn_bwd_reduce_drop_kernel<T, S><<<G, BN_THREADS, 0, st>>>( \
+    (const T*)dy, (const T*)x, (const T*)y, mean, invstd, partial, (T*)dz, M, C, sdrop, hw)
+
+// stochastic depth: bn_launch_bwd_reduce MODE 2 (residual + ReLU) with the partials of sdrop[row / hw] * dz
+cudaError_t bn_launch_bwd_reduce_drop(int dtype, const void* dy, const void* x, const void* y, const float* mean,
+                                      const float* invstd, float* partial, void* dz, const float* sdrop, int hw,
+                                      long long M, int C, int G, cudaStream_t st)
+{
+    if (hw < 1 || M % hw != 0 || M >= (1LL << 31)) return cudaErrorInvalidValue;
+    if (dtype == 0) BN_RED_DROP(__nv_bfloat16, false);
+    else if (f32_split()) BN_RED_DROP(float, true);
+    else BN_RED_DROP(float, false);
     return cudaGetLastError();
 }
 
@@ -666,6 +775,22 @@ cudaError_t bn_launch_bwd_dx(int dtype, int mode, const void* dz, const void* x,
     if (dtype == 0)       { if (mode == 1) BN_DX(__nv_bfloat16, 1, false); else BN_DX(__nv_bfloat16, 0, false); }
     else if (f32_split()) { if (mode == 1) BN_DX(float, 1, true); else BN_DX(float, 0, true); }
     else                  { if (mode == 1) BN_DX(float, 1, false); else BN_DX(float, 0, false); }
+    return cudaGetLastError();
+}
+
+#define BN_DX_DROP(T, S) bn_bwd_dx_drop_kernel<T, S><<<G, BN_THREADS, 0, st>>>( \
+    (const T*)dz, (const T*)x, scale, c2, c3, (T*)dx, M, C, sdrop, hw)
+
+// stochastic depth: bn_launch_bwd_dx MODE 0 with dx = c1*(sdrop[row / hw]*dz) - c2*x + c3
+cudaError_t bn_launch_bwd_dx_drop(int dtype, const void* dz, const void* x, const float* scale, const float* c2,
+                                  const float* c3, void* dx, const float* sdrop, int hw, long long M, int C, int G,
+                                  cudaStream_t st)
+{
+    if (hw < 1 || M % hw != 0 || M >= (1LL << 31)) return cudaErrorInvalidValue;
+    if (G <= 0) G = bn_grid(M, C, 6);
+    if (dtype == 0) BN_DX_DROP(__nv_bfloat16, false);
+    else if (f32_split()) BN_DX_DROP(float, true);
+    else BN_DX_DROP(float, false);
     return cudaGetLastError();
 }
 

@@ -347,12 +347,15 @@ struct C1Eval {
 // MODE 0: Y = X.W^T          MODE 1: + BatchNorm statistics of Y          MODE 2: Y = X.W^T + R
 // MODE 3: dz = mask ? X.W^T + R : 0, + BatchNorm backward reduction against bn_x (tm_b), coef, mask
 // MODE 4: Y = act(X.W^T * s + t)                                           MODE 5: Y = act(X.W^T * s + t + R)
-// (one body for both kernels; ev is read by MODES 4 / 5 only)
-template <int BN, int MODE, bool F32>
+// (one body for all kernels; ev is read by MODES 4 / 5 only)
+// DROP (MODE 3, stochastic depth): the previous block's BN output was scaled by sdrop[row / hw] before the
+// residual add, so the reduction is that of sdrop[row / hw] * dz; dz itself is stored unscaled
+template <int BN, int MODE, bool F32, bool DROP = false>
 __device__ __forceinline__ void
 c1_gemm_body(const CUtensorMap& tm_x, const CUtensorMap& tm_w, const CUtensorMap& tm_y, const CUtensorMap& tm_r,
              const CUtensorMap& tm_b, int M, int N, int K, float* __restrict__ partial,
-             const float* __restrict__ coef, const uint8_t* __restrict__ mask, const C1Plan& plan, const C1Eval& ev)
+             const float* __restrict__ coef, const uint8_t* __restrict__ mask, const C1Plan& plan, const C1Eval& ev,
+             const float* __restrict__ sdrop = nullptr, int hw = 1)
 {
     constexpr bool STATS = MODE == 1;
     constexpr bool RES = MODE == 2 || MODE == 3 || MODE == 5;
@@ -508,6 +511,11 @@ c1_gemm_body(const CUtensorMap& tm_x, const CUtensorMap& tm_w, const CUtensorMap
 
             // ---- epilogue ----
             const int nrows = min(16, M - mt * BM - row0);         // rows of this slab that exist (<= 0: none)
+            float srow = 1.f;                                      // DROP: lane l < 16 holds row l's scale
+            if (DROP && nrows > 0) {
+                const int gr = mt * BM + row0 + (lane & 15);
+                srow = gr < M ? __ldg(sdrop + gr / hw) : 0.f;
+            }
 #pragma unroll
             for (int s = 0; s < NS; ++s) {
                 const uint32_t slab = slab0 + (uint32_t)(slot * SLAB_BYTES);
@@ -653,11 +661,14 @@ c1_gemm_body(const CUtensorMap& tm_x, const CUtensorMap& tm_w, const CUtensorMap
                         uint32_t u, b;
                         asm volatile("ld.shared.b32 %0, [%1];" : "=r"(u) : "r"(rd + o));
                         asm volatile("ld.shared.b32 %0, [%1];" : "=r"(b) : "r"(rb + o));
-                        const float g0 = F32 ? __uint_as_float(u) : __uint_as_float(u << 16);
+                        const float sr = DROP ? __shfl_sync(0xffffffffu, srow, r) : 1.f;
+                        float g0 = F32 ? __uint_as_float(u) : __uint_as_float(u << 16);
+                        if (DROP) g0 *= sr;
                         const float x0 = F32 ? __uint_as_float(b) : __uint_as_float(b << 16);
                         s0[s] += g0; q0[s] = fmaf(g0, (x0 - mu0) * is0, q0[s]);
                         if (!F32) {
-                            const float g1 = __uint_as_float(u & 0xFFFF0000u);
+                            float g1 = __uint_as_float(u & 0xFFFF0000u);
+                            if (DROP) g1 *= sr;
                             const float x1 = __uint_as_float(b & 0xFFFF0000u);
                             s1[s] += g1; q1[s] = fmaf(g1, (x1 - mu1) * is1, q1[s]);
                         }
@@ -793,6 +804,19 @@ c1_gemm_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__
 {
     static_assert(MODE >= 0 && MODE <= 3, "MODES 4 / 5 are c1_gemm_eval_kernel");
     c1_gemm_body<BN, MODE, F32>(tm_x, tm_w, tm_y, tm_r, tm_b, M, N, K, partial, coef, mask, plan, C1Eval{});
+}
+
+// MODE 3 with the stochastic-depth scale sdrop[row / hw] of the BatchNorm being reduced
+template <int BN, bool F32>
+__global__ void __launch_bounds__(kThreads, 1)
+c1_gemm_drop_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w,
+                    const __grid_constant__ CUtensorMap tm_y, const __grid_constant__ CUtensorMap tm_r,
+                    const __grid_constant__ CUtensorMap tm_b, int M, int N, int K, float* __restrict__ partial,
+                    const float* __restrict__ coef, const uint8_t* __restrict__ mask, const C1Plan plan,
+                    const float* __restrict__ sdrop, int hw)
+{
+    c1_gemm_body<BN, 3, F32, true>(tm_x, tm_w, tm_y, tm_r, tm_b, M, N, K, partial, coef, mask, plan, C1Eval{},
+                                   sdrop, hw);
 }
 
 // MODE 4 (no residual) / MODE 5 (+ R through tm_r, as MODE 2): the eval-mode conv + BatchNorm (+ R) (+ ReLU)
@@ -1040,25 +1064,30 @@ C1Plan make_plan(int bn, int K, int n_blocks, bool residual, bool bn_reduce, boo
 template <int BN, bool F32>
 cudaError_t launch(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap& ty, const CUtensorMap& tr,
                    const CUtensorMap& tb, int M, int N, int K, float* partial, const float* coef,
-                   const uint8_t* mask, int mode, int grid, cudaStream_t st)
+                   const uint8_t* mask, int mode, int grid, cudaStream_t st, const float* sdrop, int hw)
 {
     constexpr int M3 = BN <= 128 ? 3 : 0;           // (no 256-wide MODE 3: see pick_bn)
     if (mode == 3 && M3 != 3) return cudaErrorInvalidValue;
+    const bool drop = sdrop != nullptr;             // (MODE 3 only)
     auto kern = mode == 1 ? c1_gemm_kernel<BN, 1, F32>
               : mode == 2 ? c1_gemm_kernel<BN, 2, F32>
               : mode == 3 ? c1_gemm_kernel<BN, M3, F32> : c1_gemm_kernel<BN, 0, F32>;
-    static bool configured[4][64] = {};            // function attributes are per device (and per instantiation)
+    auto dkern = c1_gemm_drop_kernel<BN <= 128 ? BN : 128, F32>;
+    const int slot = drop ? 4 : mode;
+    static bool configured[5][64] = {};            // function attributes are per device (and per instantiation)
     int dev = 0;
     cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64 || !configured[mode][dev]) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
+    if (dev < 0 || dev >= 64 || !configured[slot][dev]) {
+        cudaError_t e = drop ? cudaFuncSetAttribute(dkern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT)
+                             : cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
         if (e != cudaSuccess) return e;
-        if (dev >= 0 && dev < 64) configured[mode][dev] = true;
+        if (dev >= 0 && dev < 64) configured[slot][dev] = true;
     }
     int smem = 0;
     const C1Plan plan = make_plan(BN, K, N / BN, mode == 2, mode == 3, F32, smem);
     if (plan.stages < 2) return cudaErrorInvalidValue;
-    kern<<<grid, kThreads, smem, st>>>(tx, tw, ty, tr, tb, M, N, K, partial, coef, mask, plan);
+    if (drop) dkern<<<grid, kThreads, smem, st>>>(tx, tw, ty, tr, tb, M, N, K, partial, coef, mask, plan, sdrop, hw);
+    else kern<<<grid, kThreads, smem, st>>>(tx, tw, ty, tr, tb, M, N, K, partial, coef, mask, plan);
     return cudaGetLastError();
 }
 
@@ -1118,9 +1147,9 @@ int c1_partial_rows(long long M, int N, int K, int num_sms, int bn_reduce, int f
 // partial and residual are mutually exclusive, except in MODE 3 (mask != nullptr): then residual,
 // bn_x ([M, N], y's dtype), coef (mean [N], invstd [N]) and mask ([M, N/8] bytes) are all given,
 // y = dz and partial = [c1_partial_rows][2][N] (sum dz, sum dz * xhat).
-cudaError_t c1_launch_gemm(const void* x, const void* w, void* y, long long M, int N, int K, float* partial,
-                           const void* residual, const void* bn_x, const float* coef, const uint8_t* mask,
-                           int num_sms, int f32, cudaStream_t st)
+static cudaError_t gemm(const void* x, const void* w, void* y, long long M, int N, int K, float* partial,
+                        const void* residual, const void* bn_x, const float* coef, const uint8_t* mask,
+                        int num_sms, int f32, cudaStream_t st, const float* sdrop, int hw)
 {
     if (!c1_supported(M, N, K, f32)) return cudaErrorInvalidValue;
     if (mask ? !(partial && residual && bn_x && coef) : (partial && residual)) return cudaErrorInvalidValue;
@@ -1135,16 +1164,35 @@ cudaError_t c1_launch_gemm(const void* x, const void* w, void* y, long long M, i
         return cudaErrorInvalidValue;
     if (f) {
         switch (bn) {
-        case 256: return launch<256, true>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st);
-        case 128: return launch<128, true>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st);
-        default: return launch<64, true>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st);
+        case 256: return launch<256, true>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st, sdrop, hw);
+        case 128: return launch<128, true>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st, sdrop, hw);
+        default: return launch<64, true>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st, sdrop, hw);
         }
     }
     switch (bn) {
-    case 256: return launch<256, false>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st);
-    case 128: return launch<128, false>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st);
-    default: return launch<64, false>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st);
+    case 256: return launch<256, false>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st, sdrop, hw);
+    case 128: return launch<128, false>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st, sdrop, hw);
+    default: return launch<64, false>(tx, tw, ty, tr, tb, (int)M, N, K, partial, coef, mask, mode, grid, st, sdrop, hw);
     }
+}
+
+cudaError_t c1_launch_gemm(const void* x, const void* w, void* y, long long M, int N, int K, float* partial,
+                           const void* residual, const void* bn_x, const float* coef, const uint8_t* mask,
+                           int num_sms, int f32, cudaStream_t st)
+{
+    return gemm(x, w, y, M, N, K, partial, residual, bn_x, coef, mask, num_sms, f32, st, nullptr, 1);
+}
+
+// stochastic depth: c1_launch_gemm in MODE 3 (all of partial, residual, bn_x, coef, mask given) for a BatchNorm
+// whose output was scaled by sdrop[row / hw] (fp32 [M / hw]) before the residual add: dz is stored as there,
+// partial holds (sum sdrop * dz, sum sdrop * dz * xhat)
+cudaError_t c1_launch_gemm_bn_reduce_drop(const void* x, const void* w, void* y, long long M, int N, int K,
+                                          float* partial, const void* residual, const void* bn_x, const float* coef,
+                                          const uint8_t* mask, const float* sdrop, int hw, int num_sms, int f32,
+                                          cudaStream_t st)
+{
+    if (!mask || !sdrop || hw < 1 || M % hw != 0) return cudaErrorInvalidValue;
+    return gemm(x, w, y, M, N, K, partial, residual, bn_x, coef, mask, num_sms, f32, st, sdrop, hw);
 }
 
 // eval-mode conv + BatchNorm: y = act(x . w^T * s + t [+ residual]), s = gamma * rsqrt(var + eps),

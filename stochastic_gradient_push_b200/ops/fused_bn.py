@@ -157,6 +157,12 @@ def precise_bn_stats(acc: BNStatsAccumulator):
         _PRECISE_BN[0] = prev
 
 
+def precise_bn_active() -> bool:
+    """True inside :func:`precise_bn_stats` (the forward then describes the network evaluation runs: no
+    stochastic depth)"""
+    return _PRECISE_BN[0] is not None
+
+
 def _acc_of(bn, training: bool):
     """the accumulator view of a train-mode BatchNorm inside :func:`precise_bn_stats`, else None"""
     acc = _PRECISE_BN[0]
@@ -175,10 +181,11 @@ class _FusedBNAct(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, residual, weight, bias, running_mean, running_var, nbt,
-                training, momentum, eps, relu, acc):
+                training, momentum, eps, relu, acc, branch_scale):
         C = native.load()
         y, coef = C.bn_forward(x, residual, weight, bias, running_mean, running_var, nbt,
-                               training, momentum, eps, relu, acc)
+                               training, momentum, eps, relu, acc, **_scale_kw(branch_scale))
+        ctx.branch_scale = branch_scale
         ctx.relu = relu
         ctx.add = residual is not None
         ctx.training = training
@@ -204,28 +211,49 @@ class _FusedBNAct(torch.autograd.Function):
                 out = y if ctx.add else torch.relu(F.batch_norm(x, None, None, training=False))
                 dz = dy * (out > 0)
             return dz * scale, (dz if ctx.add else None), None, None, None, None, None, \
-                None, None, None, None, None
-        dx, dz, ggamma, gbeta = C.bn_backward(dy, x, y, coef, ctx.relu, ctx.add)
-        return dx, (dz if ctx.add else None), ggamma, gbeta, None, None, None, None, None, None, None, None
+                None, None, None, None, None, None
+        dx, dz, ggamma, gbeta = C.bn_backward(dy, x, y, coef, ctx.relu, ctx.add, **_scale_kw(ctx.branch_scale))
+        return dx, (dz if ctx.add else None), ggamma, gbeta, None, None, None, None, None, None, None, None, None
+
+
+def _scale_kw(branch_scale):
+    """the ``branch_scale`` keyword of the native calls: none at all without a scale (today's calls)"""
+    return {} if branch_scale is None else {'branch_scale': branch_scale}
+
+
+def _check_branch_scale(branch_scale, x, residual):
+    if branch_scale is None:
+        return
+    if residual is None:
+        raise ValueError('branch_scale scales a residual branch: it needs a residual')
+    if branch_scale.dim() != 1 or branch_scale.shape[0] != x.shape[0] or branch_scale.dtype != torch.float32:
+        raise ValueError('branch_scale must be an fp32 [N] tensor, one value per sample, got %s %s'
+                         % (tuple(branch_scale.shape), branch_scale.dtype))
 
 
 def fused_bn_act(x, weight, bias, running_mean, running_var, num_batches_tracked=None,
-                 residual=None, relu=False, training=True, momentum=0.1, eps=1e-5, acc=None):
+                 residual=None, relu=False, training=True, momentum=0.1, eps=1e-5, acc=None, branch_scale=None):
     """Functional form; falls back to plain PyTorch when the kernels cannot run.  ``acc`` (training
     only): an fp64 ``[2C]`` accumulator that receives the batch statistics instead of the running
-    buffers (see :func:`precise_bn_stats`)."""
+    buffers (see :func:`precise_bn_stats`).  ``branch_scale`` (with a residual; stochastic depth, see
+    ``ops.stochastic_depth``): an fp32 ``[N]`` per-sample scale of the BN output before the residual add,
+    ``relu?(bn(x) * s[n] + residual)``; the fused kernels apply it in training mode."""
+    _check_branch_scale(branch_scale, x, residual)
     fusable = _can_fuse(x) and weight is not None and weight.dtype == torch.float32 \
         and (residual is None or (relu and residual.dtype == x.dtype
-                                  and residual.stride() == x.stride()))
+                                  and residual.stride() == x.stride())) \
+        and (branch_scale is None or (training and branch_scale.device == x.device))
     if fusable and (training or not torch.is_grad_enabled() or not x.requires_grad):
         return _FusedBNAct.apply(x, residual, weight, bias, running_mean, running_var,
-                                 num_batches_tracked, training, momentum, eps, relu, acc)
+                                 num_batches_tracked, training, momentum, eps, relu, acc,
+                                 None if branch_scale is None else branch_scale.contiguous())
     return reference_bn_act(x, weight, bias, running_mean, running_var, num_batches_tracked,
-                            residual, relu, training, momentum, eps, acc)
+                            residual, relu, training, momentum, eps, acc, branch_scale)
 
 
 def reference_bn_act(x, weight, bias, running_mean, running_var, num_batches_tracked=None,
-                     residual=None, relu=False, training=True, momentum=0.1, eps=1e-5, acc=None):
+                     residual=None, relu=False, training=True, momentum=0.1, eps=1e-5, acc=None,
+                     branch_scale=None):
     if acc is not None:
         # the batch statistics exactly as a momentum-1 update of zeroed running buffers writes them
         stats = torch.zeros(2, x.shape[1], dtype=running_mean.dtype, device=x.device)
@@ -235,7 +263,11 @@ def reference_bn_act(x, weight, bias, running_mean, running_var, num_batches_tra
         if training and num_batches_tracked is not None:
             num_batches_tracked.add_(1)
         y = F.batch_norm(x, running_mean, running_var, weight, bias, training, momentum, eps)
-    if residual is not None:
+    if branch_scale is not None:
+        # in (at least) fp32, rounded once, as the kernels do
+        ct = torch.promote_types(y.dtype, torch.float32)
+        y = (y.to(ct) * branch_scale.view(-1, 1, 1, 1).to(ct) + residual.to(ct)).to(y.dtype)
+    elif residual is not None:
         y = y + residual
     return F.relu(y) if relu else y
 
@@ -243,7 +275,7 @@ def reference_bn_act(x, weight, bias, running_mean, running_var, num_batches_tra
 class FusedBatchNormAct2d(nn.BatchNorm2d):
     """``y = relu?(bn(x) (+ residual)?)`` -- see module docstring."""
 
-    def forward(self, x, residual=None, relu=False):
+    def forward(self, x, residual=None, relu=False, branch_scale=None):
         training = self.training or (self.running_mean is None)
         momentum = 0.1 if self.momentum is None else self.momentum
         return fused_bn_act(
@@ -252,7 +284,7 @@ class FusedBatchNormAct2d(nn.BatchNorm2d):
             self.running_var if self.track_running_stats else None,
             self.num_batches_tracked if (self.track_running_stats and training) else None,
             residual=residual, relu=relu, training=training, momentum=momentum, eps=self.eps,
-            acc=_acc_of(self, training))
+            acc=_acc_of(self, training), branch_scale=branch_scale)
 
 
 # --------------------------------------------------------------------------- #
@@ -261,14 +293,14 @@ class FusedBatchNormAct2d(nn.BatchNorm2d):
 class _BNBackwardHandoff:
     """What a residual block's last BN (``_Conv1x1BNAct`` with a residual) leaves on its output
     so that the next block's conv1 dgrad (``_Conv1x1BNActSplit``) can do that BN's backward
-    reduction in its epilogue: the BN input ``yraw``, its ``coef`` and the output's 1-bit ReLU
-    ``mask``.  The dgrad records which tensor it produced (``dz_key``: data pointer and version)
+    reduction in its epilogue: the BN input ``yraw``, its ``coef``, the output's 1-bit ReLU
+    ``mask`` and its stochastic-depth ``branch_scale`` (or None).  The dgrad records which tensor it produced (``dz_key``: data pointer and version)
     and the reduction ``partial``; the BN backward uses them only if its incoming gradient is
     that very tensor, unmodified."""
-    __slots__ = ('yraw', 'coef', 'mask', 'dz_key', 'partial')
+    __slots__ = ('yraw', 'coef', 'mask', 'branch_scale', 'dz_key', 'partial')
 
-    def __init__(self, yraw, coef, mask):
-        self.yraw, self.coef, self.mask = yraw, coef, mask
+    def __init__(self, yraw, coef, mask, branch_scale=None):
+        self.yraw, self.coef, self.mask, self.branch_scale = yraw, coef, mask, branch_scale
         self.dz_key = self.partial = None
 
 
@@ -278,7 +310,8 @@ class _Conv1x1BNAct(torch.autograd.Function):
     fused BN backward, then the library's dgrad / wgrad for the convolution."""
 
     @staticmethod
-    def forward(ctx, x, w, residual, gamma, beta, running_mean, running_var, nbt, momentum, eps, relu, acc):
+    def forward(ctx, x, w, residual, gamma, beta, running_mean, running_var, nbt, momentum, eps, relu, acc,
+                branch_scale):
         C = native.load()
         w16 = w if w.dtype == x.dtype else w.detach().to(x.dtype)      # compute-dtype weights
         mask = None
@@ -286,13 +319,14 @@ class _Conv1x1BNAct(torch.autograd.Function):
             M, N = x.numel() // x.shape[1], w.shape[0]
             mask = torch.empty((M, N // 8), dtype=torch.uint8, device=x.device)
         yraw, out, coef = C.conv1x1_bn_forward(x, w16, residual, gamma, beta, running_mean, running_var,
-                                               nbt, momentum, eps, relu, mask, acc=acc)
+                                               nbt, momentum, eps, relu, mask, acc=acc, **_scale_kw(branch_scale))
         ctx.relu = relu
         ctx.add = residual is not None
         ctx.w_dtype = w.dtype
+        ctx.branch_scale = branch_scale
         ctx.handoff = None
         if mask is not None:
-            ctx.handoff = out._sgp_bn_handoff = _BNBackwardHandoff(yraw, coef, mask)
+            ctx.handoff = out._sgp_bn_handoff = _BNBackwardHandoff(yraw, coef, mask, branch_scale)
         if ctx.add:
             ctx.save_for_backward(x, w16, yraw, coef, out)
         else:
@@ -308,10 +342,12 @@ class _Conv1x1BNAct(torch.autograd.Function):
         if h is not None and h.dz_key == (dy.data_ptr(), dy._version) and dy.stride() == yraw.stride():
             # dy is the next block's MODE 3 dgrad output: already masked (it is this BN's dz and the
             # residual branch's gradient), its reduction already done
-            dyraw, ggamma, gbeta = C.bn_backward_from_partials(dy, yraw, coef, h.partial)
+            dyraw, ggamma, gbeta = C.bn_backward_from_partials(dy, yraw, coef, h.partial,
+                                                               **_scale_kw(ctx.branch_scale))
             dz = dy
         else:
-            dyraw, dz, ggamma, gbeta = C.bn_backward(dy, yraw, out, coef, ctx.relu, ctx.add)
+            dyraw, dz, ggamma, gbeta = C.bn_backward(dy, yraw, out, coef, ctx.relu, ctx.add,
+                                                     **_scale_kw(ctx.branch_scale))
         if h is not None:
             h.dz_key = h.partial = None
         dx, dw, _ = torch.ops.aten.convolution_backward(
@@ -319,7 +355,7 @@ class _Conv1x1BNAct(torch.autograd.Function):
             [ctx.needs_input_grad[0], ctx.needs_input_grad[1], False])
         if dw is not None and dw.dtype != ctx.w_dtype:
             dw = dw.to(ctx.w_dtype)
-        return dx, dw, (dz if ctx.add else None), ggamma, gbeta, None, None, None, None, None, None, None
+        return dx, dw, (dz if ctx.add else None), ggamma, gbeta, None, None, None, None, None, None, None, None
 
 
 class _Conv1x1BNActSplit(torch.autograd.Function):
@@ -360,7 +396,8 @@ class _Conv1x1BNActSplit(torch.autograd.Function):
             if (h is not None and res is not None and h.yraw.dtype == dyraw.dtype
                     and h.yraw.stride() == res.stride() and C.conv1x1_can_fuse(dyraw, wt)):
                 # + the previous block's last BN backward reduction (MODE 3): dx is that BN's dz
-                dx, h.partial = C.conv1x1_dgrad_bn_reduce(dyraw, wt, res, h.yraw, h.coef, h.mask)
+                dx, h.partial = C.conv1x1_dgrad_bn_reduce(dyraw, wt, res, h.yraw, h.coef, h.mask,
+                                                          **_scale_kw(h.branch_scale))
                 h.dz_key = (dx.data_ptr(), dx._version)
             elif C.conv1x1_can_fuse(dyraw, wt):
                 dx = C.conv1x1_forward(dyraw, wt, False, res)
@@ -404,11 +441,14 @@ def _conv1x1_operands(conv, bn, x, residual, relu):
     return x, bool(native.load().conv1x1_can_fuse(x, wk)) and conv.out_channels % 8 == 0
 
 
-def conv_bn_act(conv: nn.Conv2d, bn: 'FusedBatchNormAct2d', x, residual=None, relu=False):
-    """``bn(conv(x), residual=residual, relu=relu)``; 1x1 / stride-1 convolutions of NHWC bf16
-    activations in training mode take the fused wgmma path, and so do eval-mode ones inside
+def conv_bn_act(conv: nn.Conv2d, bn: 'FusedBatchNormAct2d', x, residual=None, relu=False, branch_scale=None):
+    """``bn(conv(x), residual=residual, relu=relu, branch_scale=branch_scale)``; 1x1 / stride-1 convolutions
+    of NHWC bf16 activations in training mode take the fused wgmma path, and so do eval-mode ones inside
     :func:`eval_bn_gemm`."""
+    _check_branch_scale(branch_scale, x, residual)
     xk, ok = _conv1x1_operands(conv, bn, x, residual, relu)
+    if branch_scale is not None and not (bn.training and branch_scale.device == x.device):
+        ok = False
     if ok and not bn.training:
         w = conv.weight if conv.weight.dtype == xk.dtype else conv.weight.detach().to(xk.dtype)
         return native.load().conv1x1_bn_eval(xk, w, bn.weight, bn.bias, bn.running_mean, bn.running_var,
@@ -417,8 +457,10 @@ def conv_bn_act(conv: nn.Conv2d, bn: 'FusedBatchNormAct2d', x, residual=None, re
         momentum = 0.1 if bn.momentum is None else bn.momentum
         return _Conv1x1BNAct.apply(xk, conv.weight, residual, bn.weight, bn.bias, bn.running_mean,
                                    bn.running_var, bn.num_batches_tracked, momentum, bn.eps, relu,
-                                   _acc_of(bn, True))
-    return bn(conv(x), residual=residual, relu=relu)
+                                   _acc_of(bn, True), None if branch_scale is None else branch_scale.contiguous())
+    if branch_scale is None:
+        return bn(conv(x), residual=residual, relu=relu)
+    return bn(conv(x), residual=residual, relu=relu, branch_scale=branch_scale)
 
 
 def conv_bn_act_split(conv: nn.Conv2d, bn: 'FusedBatchNormAct2d', x, relu=False):

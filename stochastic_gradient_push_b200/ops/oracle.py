@@ -116,6 +116,36 @@ def reference_augment(batch_u8: torch.Tensor, theta: torch.Tensor, ops, magnitud
     return y.contiguous(memory_format=torch.channels_last)
 
 
+_MASK64 = (1 << 64) - 1
+
+
+def _mix64(z):
+    """splitmix64's finaliser on uint64 numpy arrays (wrapping arithmetic)"""
+    import numpy as np
+    z = (z + np.uint64(0x9E3779B97F4A7C15)) & np.uint64(_MASK64)
+    z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+    z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+    return z ^ (z >> np.uint64(31))
+
+
+def drop_path_scales(seed: int, rank: int, draw: int, thresholds, keep_scales, n: int) -> torch.Tensor:
+    """What ``drop_path_draw_kernel`` writes for draw index ``draw``: the fp32 ``[L, n]`` stochastic-depth
+    branch scales, ``out[l][i] = keep_scales[l]`` if the top 24 bits of
+    ``mix(mix(mix(mix(seed) ^ rank) ^ draw) ^ (l << 32 | i))`` are below ``thresholds[l]``, else 0
+    (``mix`` = splitmix64's finaliser, seed / rank / draw as uint64)."""
+    import numpy as np
+    L = len(thresholds)
+    with np.errstate(over='ignore'):
+        base = _mix64(np.array([int(seed) & _MASK64], dtype=np.uint64))
+        base = _mix64(base ^ np.uint64(int(rank) & _MASK64))
+        base = _mix64(base ^ np.uint64(int(draw) & _MASK64))
+        key = (np.arange(L, dtype=np.uint64)[:, None] << np.uint64(32)) | np.arange(n, dtype=np.uint64)[None, :]
+        u = _mix64(base ^ key) >> np.uint64(40)
+    keep = u < np.array(thresholds, dtype=np.uint64)[:, None]
+    out = np.where(keep, np.array(keep_scales, dtype=np.float32)[:, None], np.float32(0.0))
+    return torch.from_numpy(out.astype(np.float32))
+
+
 def rotate_all(graphs):
     for g in graphs:
         if g.is_dynamic_graph():

@@ -57,6 +57,12 @@ unbiased variance to an fp64 accumulator instead of its running buffers; one ``b
 launch then sets every running buffer to ``fp32(sum / K)``.  The first batch of a shape runs eagerly
 (and is counted) before its graph is captured; a capture does not execute, so every batch is counted
 once.
+
+Stochastic depth (a ResNet built with ``drop_path_rate > 0``) lives in the model: each training forward
+draws its masks with one ``drop_path_draw`` launch, so ``own_launches_per_step`` grows by one per forward
+(k with ``accumulation_steps=k``: each micro-batch has its own masks), and every replay draws fresh
+ones.  ``update_bn`` (inside ``precise_bn_stats``) and ``evaluate`` (eval mode) draw nothing and scale
+nothing: precise statistics describe the network that evaluation runs.
 """
 
 from __future__ import annotations

@@ -120,6 +120,19 @@ def build_parser(adpsgd: bool = False) -> argparse.ArgumentParser:
                         'blocks, linear in the block index (block 0 never drops, the last drops with this rate); '
                         'applied inside the fused BatchNorm kernels, drawn from (--seed, rank); 0 = off.  Not with '
                         '--model tiny')
+    p.add_argument('--distill_alpha', default=0.0, type=float,
+                   help='knowledge distillation (Hinton et al. 2015) weight alpha in [0, 1]: the training loss is '
+                        '(1 - alpha) CE + alpha T^2 KL(softmax(teacher / T) || softmax(student / T)), the teacher '
+                        'being --teacher_model loaded from --teacher_checkpoint, frozen in eval mode; 0 = off.  '
+                        'On the fused loss kernel inside the captured step with --cuda_graph True; validation '
+                        'never distils.  Not with AD-PSGD')
+    p.add_argument('--distill_temperature', default=1.0, type=float,
+                   help='softmax temperature T > 0 of --distill_alpha')
+    p.add_argument('--teacher_model', default=None, type=str,
+                   help='architecture of the --distill_alpha teacher, a models.MODEL_ZOO key (with --num_classes)')
+    p.add_argument('--teacher_checkpoint', default=None, type=str,
+                   help='weights of the --distill_alpha teacher: a model state_dict, or a checkpoint this '
+                        'trainer wrote.  Loaded again on --resume (the teacher is not checkpointed)')
     p.add_argument('--seed', default=47, type=int)
     p.add_argument('--resume', default=False, **B)
     p.add_argument('--backend', default='nccl', choices=['nccl', 'gloo', 'mpi'])
@@ -309,6 +322,7 @@ def finalize_args(args, adpsgd=False):
     check_augment_flags(args)
     check_ema_flags(args, adpsgd)
     check_drop_path_flags(args)
+    check_distill_flags(args, adpsgd)
     args.ema_fname = '{}{}ema_r{}_n{}.csv'.format(args.checkpoint_dir, args.tag, args.rank, args.world_size)
     args.consensus_fname = '{}{}consensus_r{}_n{}.csv'.format(args.checkpoint_dir, args.tag, args.rank,
                                                               args.world_size)
@@ -459,6 +473,74 @@ def check_drop_path_flags(args):
     if p > 0 and args.model == 'tiny':
         raise ValueError('--drop_path_rate is not supported with --model tiny: stochastic depth drops residual '
                          'blocks, and TinyConvNet has none')
+
+
+def model_num_classes(name, args) -> int:
+    """the number of classes ``init_model`` gives model ``name`` (``tiny`` keeps TinyConvNet's default)"""
+    if name == 'tiny':
+        import inspect
+        from ..models import TinyConvNet
+        return inspect.signature(TinyConvNet).parameters['num_classes'].default
+    return args.num_classes
+
+
+def check_distill_flags(args, adpsgd=False):
+    """ValueError for --distill_alpha outside [0, 1], --distill_temperature not finite and > 0, and for
+    alpha > 0 with AD-PSGD, without both --teacher_model and --teacher_checkpoint, or with a teacher whose
+    class count differs from the student's."""
+    import math
+    alpha = getattr(args, 'distill_alpha', 0.0)
+    temp = getattr(args, 'distill_temperature', 1.0)
+    if not 0.0 <= alpha <= 1.0:
+        raise ValueError('--distill_alpha must be in [0, 1], got %r' % (alpha,))
+    if not (math.isfinite(temp) and temp > 0.0):
+        raise ValueError('--distill_temperature must be finite and > 0, got %r' % (temp,))
+    if alpha == 0.0:
+        return
+    if adpsgd:
+        raise ValueError('--distill_alpha is not supported with AD-PSGD: only the SGP / OSGP / D-PSGD and '
+                         'all-reduce trainers run a teacher')
+    if not getattr(args, 'teacher_model', None) or not getattr(args, 'teacher_checkpoint', None):
+        raise ValueError('--distill_alpha > 0 needs --teacher_model and --teacher_checkpoint')
+    from ..models import MODEL_ZOO
+    if args.teacher_model not in MODEL_ZOO:
+        raise ValueError('--teacher_model must be one of %s, got %r' % (', '.join(sorted(MODEL_ZOO)), args.teacher_model))
+    nt, ns = model_num_classes(args.teacher_model, args), model_num_classes(args.model, args)
+    if nt != ns:
+        raise ValueError('the teacher --teacher_model %s has %d classes but the student --model %s has %d'
+                         % (args.teacher_model, nt, args.model, ns))
+
+
+def teacher_state_dict(obj):
+    """the model ``state_dict`` inside a loaded --teacher_checkpoint: the object itself, or from a checkpoint this
+    trainer wrote its ``'state_dict'`` (of the data-parallel wrapper: its own ``'state_dict'`` again for the
+    gossip wrappers), with the wrapper's ``module.`` key prefix stripped and the wrapper's own entries dropped"""
+    sd = obj
+    for _ in range(2):                                 # checkpoint -> wrapper state -> module state
+        if isinstance(sd, dict) and isinstance(sd.get('state_dict'), dict):
+            sd = sd['state_dict']
+    if not isinstance(sd, dict):
+        raise ValueError('--teacher_checkpoint holds no state_dict (got %s)' % type(obj).__name__)
+    if any(k.startswith('module.') for k in sd):
+        sd = {k[len('module.'):]: v for k, v in sd.items() if k.startswith('module.')}
+    return sd
+
+
+def load_teacher(args):
+    """The --distill_alpha teacher: --teacher_model with --num_classes, loaded strictly from
+    --teacher_checkpoint (the same file on every rank), on ``args.device`` (channels_last with
+    --channels_last on CUDA), in eval mode without gradients.  None when --distill_alpha is 0."""
+    if not getattr(args, 'distill_alpha', 0.0) > 0:
+        return None
+    from .. import models
+    kw = {} if args.teacher_model == 'tiny' else {'num_classes': args.num_classes}
+    net = models.MODEL_ZOO[args.teacher_model](**kw)
+    ckpt = torch.load(args.teacher_checkpoint, map_location='cpu', weights_only=False)
+    net.load_state_dict(teacher_state_dict(ckpt), strict=True)
+    net = net.to(args.device)
+    if args.channels_last and args.device == 'cuda':
+        net = net.to(memory_format=torch.channels_last)
+    return net.eval().requires_grad_(False)
 
 
 def stochastic_depth_of(model):
@@ -688,9 +770,15 @@ def mix_train_batch(args, batch_mix, batch, itr):
     return batch_mix.apply(batch), batch_mix.state
 
 
-def train_loss(criterion, output, target, mix, label_smoothing):
+def train_loss(criterion, output, target, mix, label_smoothing, teacher_logits=None, args=None):
     """Training loss of the eager loops: ``criterion`` or, for a mixed batch, the two-target
-    cross-entropy (fused kernel on CUDA) with the same label smoothing."""
+    cross-entropy (fused kernel on CUDA) with the same label smoothing.  With ``teacher_logits`` the
+    --distill_alpha / --distill_temperature objective of ``args`` (``reference_distillation_loss``)."""
+    if teacher_logits is not None:
+        from ..ops.fused_loss import reference_distillation_loss
+        return reference_distillation_loss(output.float(), target, teacher_logits.float(), args.distill_alpha,
+                                           args.distill_temperature, label_smoothing,
+                                           lam=None if mix is None else mix[0])[0]
     if mix is None:
         return criterion(output.float(), target)
     from ..ops.fused_loss import fused_cross_entropy

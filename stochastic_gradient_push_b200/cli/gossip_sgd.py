@@ -160,6 +160,8 @@ def main(argv=None):
     # --model_ema_decay: weight EMA, updated after every step (the last launch of the captured step)
     args._ema = common.make_model_ema(args, model)
     args._ema_due = False
+    # --distill_alpha: the frozen teacher, loaded from --teacher_checkpoint (never checkpointed)
+    args._teacher = common.load_teacher(args)
     args._trainer = None
     if args.cuda_graph and not args.all_reduce and args.fused and getattr(model, '_kernel', None):
         from ..ops.fused_loss import FusedCrossEntropyWithAccuracy
@@ -167,10 +169,12 @@ def main(argv=None):
         # the fused softmax-xent + prec@1/5 kernel, captured in the graph (same value as
         # nn.CrossEntropyLoss(label_smoothing=...); tests/test_fused_loss_gpu.py)
         args._trainer = GossipTrainer(model, optimizer,
-                                      FusedCrossEntropyWithAccuracy(label_smoothing=args.label_smoothing),
+                                      FusedCrossEntropyWithAccuracy(label_smoothing=args.label_smoothing,
+                                                                    distill_alpha=args.distill_alpha,
+                                                                    distill_temperature=args.distill_temperature),
                                       amp_dtype=torch.bfloat16 if args.amp else None,
                                       batch_mix=args._batch_mix, ema=args._ema,
-                                      accumulation_steps=args.accumulation_steps)
+                                      accumulation_steps=args.accumulation_steps, teacher=args._teacher)
     if args.eval_graph and args._trainer is None:
         raise ValueError('--eval_graph is not supported with transport %s: the captured evaluation is '
                          'GossipTrainer.evaluate, which runs on the CUDA kernel transport only'
@@ -220,6 +224,11 @@ def main(argv=None):
 
     loader, sampler = make_dataloader(args, train=True)
     val_loader = None if args.train_fast else make_dataloader(args, train=False)
+
+    if args._teacher is not None:
+        # a wrongly loaded teacher is the usual way distillation fails silently: its accuracy, once
+        evaluate(args, val_loader if val_loader is not None else make_dataloader(args, train=False),
+                 args._teacher, criterion, log, label='Teacher ', graph=False)
 
     start_itr, start_epoch = state['itr'], state['epoch']
     elapsed_time = state['elapsed_time']
@@ -301,6 +310,7 @@ def train(args, model, criterion, optimizer, batch_meter, data_meter, nn_meter, 
     trainer = getattr(args, '_trainer', None)
     batch_mix = getattr(args, '_batch_mix', None)
     ema = getattr(args, '_ema', None) if trainer is None else None    # (the trainer updates its own)
+    teacher = getattr(args, '_teacher', None) if trainer is None else None   # (the trainer runs its own)
     it = iter(loader)
     for _ in range(itr):            # resume mid-epoch: skip what was already consumed
         next(it, None)
@@ -338,9 +348,19 @@ def train(args, model, criterion, optimizer, batch_meter, data_meter, nn_meter, 
                 slot = trainer.step(batch, target)
             pending.append((slot, batch.size(0)))
         else:
+            if teacher is not None:
+                # the teacher is a bare module on the device (the wrapped student scatters its own input):
+                # one copy of the batch serves both
+                batch = batch.to(dev, non_blocking=True)
+                if args.channels_last and dev == 'cuda':
+                    batch = batch.contiguous(memory_format=torch.channels_last)
             with tracing.span('forward', itr=i), _autocast(args):
+                teacher_logits = None
+                if teacher is not None:
+                    with torch.no_grad():
+                        teacher_logits = teacher(batch)
                 output = model(batch)
-                loss = common.train_loss(criterion, output, target, mix, args.label_smoothing)
+                loss = common.train_loss(criterion, output, target, mix, args.label_smoothing, teacher_logits, args)
             if ema is not None and args._ema_due:
                 # c10d plane: the previous step's gossip was received and de-biased by the forward
                 # pre-hook just now; the EMA takes those parameters (and this forward's BN statistics)
@@ -491,11 +511,12 @@ def validate(args, val_loader, model, criterion, log):
     return evaluate(args, val_loader, model, criterion, log)[0]
 
 
-def evaluate(args, val_loader, model, criterion, log, label=''):
+def evaluate(args, val_loader, model, criterion, log, label='', graph=True):
     """(prec@1, prec@5) over the validation set, logged as `` * <label>Prec@1 .. Prec@5 ..``;
-    with --eval_graph through the trainer's captured evaluation"""
+    with --eval_graph (and ``graph``) through the trainer's captured evaluation of the trainer's model.
+    ``graph=False`` evaluates ``model`` itself (the --distill_alpha teacher) eagerly."""
     trainer = getattr(args, '_trainer', None)
-    if getattr(args, 'eval_graph', False) and trainer is not None:
+    if graph and getattr(args, 'eval_graph', False) and trainer is not None:
         r = trainer.evaluate((common.device_batch(args, features, train=False), target)
                              for features, target in val_loader)
         log.info(' * {label}Prec@1 {p1:.3f} Prec@5 {p5:.3f}'.format(label=label, p1=r.prec1, p5=r.prec5))

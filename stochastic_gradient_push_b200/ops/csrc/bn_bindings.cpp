@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 
 #include <atomic>
+#include <cmath>
 #include <cstring>
 #include <stdexcept>
 #include <string>
@@ -744,12 +745,13 @@ static torch::Tensor conv1x1_bn_eval(torch::Tensor x, torch::Tensor w, torch::Te
 // ---------------------------------------------------------------------------
 extern "C" {
 cudaError_t xent_launch_fwd(int dtype, const void* logits, const long long* target, float* lse, float* out3, int B,
-                            int C, float eps, const float* mix, cudaStream_t st);
+                            int C, float eps, const float* mix, const void* teacher, float alpha, float temp,
+                            cudaStream_t st);
 cudaError_t xent_launch_eval(int dtype, const void* logits, const long long* target, unsigned long long* acc, int B,
                              int C, cudaStream_t st);
 cudaError_t xent_launch_bwd(int dtype, const void* logits, const long long* target, const float* lse,
                             const float* grad_out, void* dlogits, int B, int C, float eps, const float* mix,
-                            cudaStream_t st);
+                            const void* teacher, float alpha, float temp, cudaStream_t st);
 cudaError_t batch_mix_launch(int out_dtype, const float* src, void* dst, const float* mix, int B, int C, int H,
                              int W, long long s_n, int s_c, int s_p, long long d_n, int d_c, int d_p,
                              cudaStream_t st);
@@ -781,40 +783,66 @@ static const float* xent_mix_ptr(const c10::optional<torch::Tensor>& mix, const 
     return mix->data_ptr<float>();
 }
 
-// returns (metrics[3] = mean loss (label-smoothed when label_smoothing > 0), prec@1 %, prec@5 %; lse[B]);
-// with mix: the two-target loss lam CE(z_i, t_i) + (1 - lam) CE(z_i, t_{B-1-i})
+// knowledge distillation: teacher logits of the logits' shape, dtype and device (contiguous), alpha in (0, 1],
+// temperature finite and > 0; None = plain (smoothed, mixed) cross-entropy (the DISTILL = false kernels)
+static const void* xent_teacher_ptr(const c10::optional<torch::Tensor>& teacher, const torch::Tensor& logits,
+                                    double alpha, double temperature)
+{
+    if (!teacher.has_value() || !teacher->defined()) return nullptr;
+    TORCH_CHECK(teacher->is_cuda() && teacher->get_device() == logits.get_device() &&
+                    teacher->scalar_type() == logits.scalar_type() && teacher->sizes() == logits.sizes() &&
+                    teacher->is_contiguous(),
+                "teacher_logits must be a contiguous tensor of the logits' shape, dtype and device");
+    TORCH_CHECK(alpha > 0.0 && alpha <= 1.0, "distill_alpha must be in (0, 1] with teacher logits");
+    TORCH_CHECK(std::isfinite(temperature) && temperature > 0.0, "distill_temperature must be finite and > 0");
+    return teacher->data_ptr();
+}
+
+// returns (metrics[3] = mean loss (label-smoothed when label_smoothing > 0), prec@1 %, prec@5 %; lse);
+// with mix: the two-target loss lam CE(z_i, t_i) + (1 - lam) CE(z_i, t_{B-1-i});
+// with teacher: (1 - alpha) CE + alpha T^2 KL(softmax(u / T) || softmax(z / T)), and lse = [lse, lseT, lseU] as
+// one fp32 [3, B] tensor (else [B])
 static std::vector<torch::Tensor> xent_forward(torch::Tensor logits, torch::Tensor target, double label_smoothing,
-                                               c10::optional<torch::Tensor> mix)
+                                               c10::optional<torch::Tensor> mix, c10::optional<torch::Tensor> teacher,
+                                               double alpha, double temperature)
 {
     TORCH_CHECK(xent_can_fuse(logits, target), "xent_forward: unsupported tensors");
     const float eps = xent_check_smoothing(label_smoothing);
     const float* mixp = xent_mix_ptr(mix, logits);
+    const void* tp = xent_teacher_ptr(teacher, logits, alpha, temperature);
     c10::cuda::CUDAGuard guard(logits.get_device());
     auto st = at::cuda::getCurrentCUDAStream();
     auto fopt = torch::TensorOptions().dtype(torch::kFloat32).device(logits.device());
     const int B = (int)logits.size(0), C = (int)logits.size(1);
     auto out3 = torch::empty({3}, fopt);
-    auto lse = torch::empty({B}, fopt);
+    auto lse = tp ? torch::empty({3, B}, fopt) : torch::empty({B}, fopt);
     BN_CHECK(cudaMemsetAsync(out3.data_ptr(), 0, 3 * sizeof(float), st));
     BN_CHECK(xent_launch_fwd(dtype_code(logits), logits.data_ptr(),
                              reinterpret_cast<const long long*>(target.data_ptr<int64_t>()),
-                             lse.data_ptr<float>(), out3.data_ptr<float>(), B, C, eps, mixp, st));
+                             lse.data_ptr<float>(), out3.data_ptr<float>(), B, C, eps, mixp, tp, (float)alpha,
+                             (float)temperature, st));
     return {out3, lse};
 }
 
 static torch::Tensor xent_backward(torch::Tensor logits, torch::Tensor target, torch::Tensor lse,
-                                   torch::Tensor grad_out, double label_smoothing, c10::optional<torch::Tensor> mix)
+                                   torch::Tensor grad_out, double label_smoothing, c10::optional<torch::Tensor> mix,
+                                   c10::optional<torch::Tensor> teacher, double alpha, double temperature)
 {
     TORCH_CHECK(xent_can_fuse(logits, target) && lse.is_cuda() && lse.scalar_type() == torch::kFloat32 &&
-                grad_out.is_cuda() && grad_out.scalar_type() == torch::kFloat32 && grad_out.numel() == 1);
+                lse.is_contiguous() && grad_out.is_cuda() && grad_out.scalar_type() == torch::kFloat32 &&
+                grad_out.numel() == 1);
     const float eps = xent_check_smoothing(label_smoothing);
     const float* mixp = xent_mix_ptr(mix, logits);
+    const void* tp = xent_teacher_ptr(teacher, logits, alpha, temperature);
+    const int64_t lse_per_row = tp ? 3 : 1;
+    TORCH_CHECK(lse.numel() == lse_per_row * logits.size(0),
+                "xent_backward: lse must hold 3 values per row with teacher logits, 1 without");
     c10::cuda::CUDAGuard guard(logits.get_device());
     auto dl = torch::empty_like(logits);
     BN_CHECK(xent_launch_bwd(dtype_code(logits), logits.data_ptr(),
                              reinterpret_cast<const long long*>(target.data_ptr<int64_t>()), lse.data_ptr<float>(),
                              grad_out.data_ptr<float>(), dl.data_ptr(), (int)logits.size(0), (int)logits.size(1), eps,
-                             mixp, at::cuda::getCurrentCUDAStream()));
+                             mixp, tp, (float)alpha, (float)temperature, at::cuda::getCurrentCUDAStream()));
     return dl;
 }
 
@@ -905,9 +933,11 @@ void bind_bn(py::module& mod)
     mod.attr("DROP_PATH_MAX_BLOCKS") = drop_path_max_blocks();
     mod.def("xent_can_fuse", &xent_can_fuse);
     mod.def("xent_forward", &xent_forward, py::arg("logits"), py::arg("target"), py::arg("label_smoothing") = 0.0,
-            py::arg("mix") = py::none());
+            py::arg("mix") = py::none(), py::arg("teacher") = py::none(), py::arg("alpha") = 0.0,
+            py::arg("temperature") = 1.0);
     mod.def("xent_backward", &xent_backward, py::arg("logits"), py::arg("target"), py::arg("lse"),
-            py::arg("grad_out"), py::arg("label_smoothing") = 0.0, py::arg("mix") = py::none());
+            py::arg("grad_out"), py::arg("label_smoothing") = 0.0, py::arg("mix") = py::none(),
+            py::arg("teacher") = py::none(), py::arg("alpha") = 0.0, py::arg("temperature") = 1.0);
     mod.def("xent_eval_accumulate", &xent_eval_accumulate, py::arg("logits"), py::arg("target"), py::arg("acc"));
     mod.def("batch_mix", &batch_mix, py::arg("src"), py::arg("out"), py::arg("mix"));
     mod.def("conv1x1_can_fuse", &conv1x1_can_fuse);

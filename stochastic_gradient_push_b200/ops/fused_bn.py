@@ -30,6 +30,7 @@ from __future__ import annotations
 
 import contextlib
 import os
+import threading
 
 import torch
 import torch.nn as nn
@@ -68,8 +69,14 @@ def bn_f32_map(split: bool):
         C.bn_f32_map(prev)
 
 
-# set by eval_bn_gemm(): eval-mode conv_bn_act calls the GEMM with BatchNorm in its epilogue
-_EVAL_GEMM = [False]
+class _ThreadFlag(threading.local):
+    on = False
+
+
+# set by eval_bn_gemm(): eval-mode conv_bn_act calls the GEMM with BatchNorm in its epilogue.  Per thread: a
+# distilling training step runs its teacher inside the block while ranks driven from other threads of the
+# process may be in their train-mode forward
+_EVAL_GEMM = _ThreadFlag()
 
 
 @contextlib.contextmanager
@@ -79,12 +86,12 @@ def eval_bn_gemm():
     the running statistics, the residual add and the ReLU in its epilogue (``C.conv1x1_bn_eval``)
     instead of the library convolution and a separate BatchNorm pass.  Outside it an eval forward runs
     as before, bit for bit.  ``GossipTrainer.evaluate`` uses it."""
-    prev = _EVAL_GEMM[0]
-    _EVAL_GEMM[0] = True
+    prev = _EVAL_GEMM.on
+    _EVAL_GEMM.on = True
     try:
         yield
     finally:
-        _EVAL_GEMM[0] = prev
+        _EVAL_GEMM.on = prev
 
 
 # set by precise_bn_stats(): the BNStatsAccumulator train-mode BatchNorm layers add their batch statistics to
@@ -417,7 +424,7 @@ class _Conv1x1BNActSplit(torch.autograd.Function):
 def _conv1x1_operands(conv, bn, x, residual, relu):
     """(x, fusable): x possibly cast the way autocast would; fusable says whether the wgmma
     conv + BN path covers this call."""
-    train_or_eval = bn.training or (_EVAL_GEMM[0] and not torch.is_grad_enabled())
+    train_or_eval = bn.training or (_EVAL_GEMM.on and not torch.is_grad_enabled())
     if not (USE_TCGEN05_CONV1X1 and not FORCE_REFERENCE and train_or_eval and bn.track_running_stats
             and x.is_cuda and native.available() and x.dim() == 4
             and conv.kernel_size == (1, 1) and conv.stride == (1, 1) and conv.padding == (0, 0)

@@ -27,9 +27,20 @@ targets, its own ``t_i`` and its partner's ``t_{B-1-i}``, weighted ``lam`` and `
 read by the kernels from ``state[0]``, so a captured graph follows each step's draw):
 ``loss_i = lam CE_eps(z_i, t_i) + (1 - lam) CE_eps(z_i, t_{B-1-i})``.  prec@1 / prec@5 still count
 against each row's own target.  ``mix=None`` runs exactly the one-target kernels.
+
+Knowledge distillation (``teacher_logits=u``, ``distill_alpha`` = alpha in (0, 1], ``distill_temperature`` =
+T > 0; Hinton et al. 2015): ``loss_i = (1 - alpha) CE_eps(z_i, .) + alpha T^2 KL(softmax(u_i / T) ||
+softmax(z_i / T))`` with ``CE_eps`` the (smoothed, mixed) cross-entropy above, averaged over the batch:
+``(1 - alpha) F.cross_entropy(z, y, label_smoothing=eps) + alpha T^2 F.kl_div(F.log_softmax(z / T),
+F.log_softmax(u / T), reduction='batchmean', log_target=True)`` when every target is valid.  The same two
+launches compute it, reading ``u`` once in each; ``metrics[0]`` is that combined objective and prec@1 /
+prec@5 are the student's.  The teacher logits get no gradient.  A row whose target (or partner target) is
+out of range adds neither term.  ``distill_alpha = 0`` without teacher logits runs exactly the kernels above.
 """
 
 from __future__ import annotations
+
+import math
 
 import torch
 import torch.nn as nn
@@ -43,6 +54,77 @@ def check_label_smoothing(label_smoothing) -> float:
     if not 0.0 <= eps <= 1.0:
         raise ValueError('label_smoothing must be in [0, 1], got %r' % (label_smoothing,))
     return eps
+
+
+def check_distill_args(distill_alpha, distill_temperature) -> tuple:
+    """``(alpha, T)`` as floats; ValueError unless alpha is in [0, 1] and T is finite and > 0."""
+    alpha, temp = float(distill_alpha), float(distill_temperature)
+    if not 0.0 <= alpha <= 1.0:
+        raise ValueError('distill_alpha must be in [0, 1], got %r' % (distill_alpha,))
+    if not (math.isfinite(temp) and temp > 0.0):
+        raise ValueError('distill_temperature must be finite and > 0, got %r' % (distill_temperature,))
+    return alpha, temp
+
+
+def _check_teacher_logits(logits, teacher_logits, alpha):
+    if alpha > 0.0 and teacher_logits is None:
+        raise ValueError('distill_alpha > 0 needs teacher_logits')
+    if teacher_logits is None:
+        return
+    if alpha == 0.0:
+        raise ValueError('teacher_logits were given with distill_alpha = 0')
+    if teacher_logits.shape != logits.shape or teacher_logits.dtype != logits.dtype:
+        raise ValueError('teacher_logits must have the logits\' shape and dtype: got %s %s for logits %s %s'
+                         % (tuple(teacher_logits.shape), teacher_logits.dtype, tuple(logits.shape), logits.dtype))
+    if teacher_logits.device != logits.device:
+        raise ValueError('teacher_logits must be on the logits\' device: got %s for %s'
+                         % (teacher_logits.device, logits.device))
+
+
+def reference_distillation_loss(logits: torch.Tensor, target: torch.Tensor, teacher_logits: torch.Tensor,
+                                distill_alpha: float, distill_temperature: float = 1.0,
+                                label_smoothing: float = 0.0, lam=None):
+    """(loss, prec@1 %, prec@5 %) of the distillation objective in plain PyTorch (fp32, fp64 for fp64
+    logits): ``mean_i [(1 - alpha) CE_eps(z_i, .) + alpha T^2 KL(softmax(u_i / T) || softmax(z_i / T))]``
+    with ``CE_eps`` the label-smoothed cross-entropy, or with ``lam`` (a float or 0-d tensor) the two-target
+    ``lam CE_eps(z_i, t_i) + (1 - lam) CE_eps(z_i, t_{B-1-i})``.  A row whose target (or partner target) is
+    out of range adds no loss (the mean still divides by B).  The teacher logits are detached; the
+    accuracies are the student's against each row's own target."""
+    eps = check_label_smoothing(label_smoothing)
+    alpha, temp = check_distill_args(distill_alpha, distill_temperature)
+    _check_teacher_logits(logits, teacher_logits, alpha)
+    ct = torch.float64 if logits.dtype == torch.float64 else torch.float32
+    lf = logits.to(ct)
+    B, C = lf.shape
+    valid = (target >= 0) & (target < C)
+    za = lf.gather(1, torch.where(valid, target, 0).view(-1, 1)).view(-1)
+    if lam is None:
+        zy = za
+    else:
+        lam = torch.as_tensor(lam, dtype=ct, device=lf.device)
+        tb = target.flip(0)
+        vb = (tb >= 0) & (tb < C)
+        valid = valid & vb
+        zb = lf.gather(1, torch.where(vb, tb, 0).view(-1, 1)).view(-1)
+        zy = lam * za + (1.0 - lam) * zb
+    ce = torch.logsumexp(lf, 1) - (1.0 - eps) * zy
+    if eps:
+        ce = ce - eps * lf.mean(1)
+    loss_i = (1.0 - alpha) * ce
+    if alpha > 0.0:
+        uf = teacher_logits.detach().to(ct)
+        kl = F.kl_div(F.log_softmax(lf / temp, 1), F.log_softmax(uf / temp, 1), reduction='none',
+                      log_target=True).sum(1)
+        loss_i = loss_i + (alpha * temp * temp) * kl
+    loss = torch.where(valid, loss_i, torch.zeros_like(loss_i)).sum() / B
+    with torch.no_grad():
+        k = min(5, C)
+        _, pred = lf.topk(k, 1, True, True)
+        hit = pred.eq(target.view(-1, 1))
+        scale = 100.0 / B
+        p1 = hit[:, :1].reshape(-1).float().sum() * scale
+        p5 = hit.reshape(-1).float().sum() * scale
+    return loss, p1, p5
 
 
 def reference_loss_and_accuracy(logits: torch.Tensor, target: torch.Tensor, label_smoothing: float = 0.0):
@@ -63,12 +145,13 @@ def reference_loss_and_accuracy(logits: torch.Tensor, target: torch.Tensor, labe
 class _FusedXent(torch.autograd.Function):
 
     @staticmethod
-    def forward(ctx, logits, target, label_smoothing, mix):
+    def forward(ctx, logits, target, label_smoothing, mix, teacher, alpha, temperature):
         C = native.load()
-        metrics, lse = C.xent_forward(logits, target, label_smoothing, mix)
+        metrics, lse = C.xent_forward(logits, target, label_smoothing, mix, teacher, alpha, temperature)
         ctx.save_for_backward(logits, target, lse)
         ctx.label_smoothing = label_smoothing
         ctx.mix = mix
+        ctx.distill = (teacher, alpha, temperature)
         ctx.mark_non_differentiable(metrics)
         return metrics[0], metrics
 
@@ -77,21 +160,34 @@ class _FusedXent(torch.autograd.Function):
         C = native.load()
         logits, target, lse = ctx.saved_tensors
         g = g_loss.reshape(1).to(torch.float32)
-        return C.xent_backward(logits, target, lse, g, ctx.label_smoothing, ctx.mix), None, None, None
+        dz = C.xent_backward(logits, target, lse, g, ctx.label_smoothing, ctx.mix, *ctx.distill)
+        return dz, None, None, None, None, None, None
 
 
 def fused_cross_entropy(logits: torch.Tensor, target: torch.Tensor, label_smoothing: float = 0.0,
-                        mix: torch.Tensor = None):
+                        mix: torch.Tensor = None, teacher_logits: torch.Tensor = None,
+                        distill_alpha: float = 0.0, distill_temperature: float = 1.0):
     """Returns ``(loss, metrics)``; ``metrics = [loss, prec@1 %, prec@5 %]`` (fp32, detached).
     ``label_smoothing`` in [0, 1], as in ``F.cross_entropy``.  ``mix``: the mix state of
-    ``batch_mix.BatchMix`` (two targets per row, see the module docstring), or None."""
+    ``batch_mix.BatchMix`` (two targets per row, see the module docstring), or None.
+    ``teacher_logits``: the teacher's logits (the logits' shape and dtype; no gradient), given exactly when
+    ``distill_alpha`` in [0, 1] is > 0; ``distill_temperature`` > 0 (see the module docstring)."""
     eps = check_label_smoothing(label_smoothing)
+    alpha, temp = check_distill_args(distill_alpha, distill_temperature)
+    _check_teacher_logits(logits, teacher_logits, alpha)
     if logits.is_cuda and native.available():
         lg = logits if logits.is_contiguous() else logits.contiguous()
         if native.load().xent_can_fuse(lg, target):
-            loss, metrics = _FusedXent.apply(lg, target, eps, mix)
+            u = None
+            if teacher_logits is not None:
+                u = teacher_logits.detach()
+                u = u if u.is_contiguous() else u.contiguous()
+            loss, metrics = _FusedXent.apply(lg, target, eps, mix, u, alpha, temp)
             return loss, metrics
-    if mix is None:
+    if teacher_logits is not None:
+        loss, p1, p5 = reference_distillation_loss(logits, target, teacher_logits, alpha, temp, eps,
+                                                   lam=None if mix is None else mix[0])
+    elif mix is None:
         loss, p1, p5 = reference_loss_and_accuracy(logits, target, eps)
     else:
         from .batch_mix import reference_mixed_loss_and_accuracy
@@ -120,18 +216,26 @@ def eval_accumulate(logits: torch.Tensor, target: torch.Tensor, acc: torch.Tenso
 
 class FusedCrossEntropyWithAccuracy(nn.Module):
     """Drop-in for ``nn.CrossEntropyLoss(label_smoothing=label_smoothing)`` (mean reduction) that
-    also measures accuracy."""
+    also measures accuracy.  With ``distill_alpha`` > 0 it is the distillation objective (module
+    docstring) and every call takes the teacher's logits."""
 
-    def __init__(self, label_smoothing: float = 0.0):
+    def __init__(self, label_smoothing: float = 0.0, distill_alpha: float = 0.0, distill_temperature: float = 1.0):
         super().__init__()
         self.label_smoothing = check_label_smoothing(label_smoothing)
+        self.distill_alpha, self.distill_temperature = check_distill_args(distill_alpha, distill_temperature)
         self.metrics = None
 
-    def forward(self, logits, target, mix=None):
+    def forward(self, logits, target, mix=None, teacher_logits=None):
         """``mix``: the device mix state of ``batch_mix.BatchMix`` for mixup / CutMix targets
-        (prec@1 / prec@5 then count against each row's own target), or None."""
-        loss, self.metrics = fused_cross_entropy(logits, target, self.label_smoothing, mix=mix)
+        (prec@1 / prec@5 then count against each row's own target), or None.  ``teacher_logits``:
+        the teacher's logits, given exactly when ``distill_alpha`` > 0."""
+        loss, self.metrics = fused_cross_entropy(logits, target, self.label_smoothing, mix=mix,
+                                                 teacher_logits=teacher_logits, distill_alpha=self.distill_alpha,
+                                                 distill_temperature=self.distill_temperature)
         return loss
 
     def extra_repr(self):
-        return 'label_smoothing=%g' % self.label_smoothing if self.label_smoothing else ''
+        parts = ['label_smoothing=%g' % self.label_smoothing] if self.label_smoothing else []
+        if self.distill_alpha:
+            parts.append('distill_alpha=%g, distill_temperature=%g' % (self.distill_alpha, self.distill_temperature))
+        return ', '.join(parts)

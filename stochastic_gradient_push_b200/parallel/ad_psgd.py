@@ -585,14 +585,17 @@ class _BilatEngineShim(object):
 
 def make_bilat_trainer(model: BilatGossipDataParallel, lr, criterion=None, amp_dtype=None,
                        use_cuda_graph=True, warmup_iters=3, channels_last=True, lars=False, batch_mix=None,
-                       ema=None):
+                       ema=None, teacher=None):
     """AD-PSGD counterpart of :class:`~.trainer.GossipTrainer`: forward + fused loss/accuracy +
     backward are captured ONCE as a CUDA graph; after every replay the gradients are handed to
     the gossip side with :meth:`BilatGossipDataParallel.handoff` (fused SGD on the gossip copy +
     model pull, enqueued on the daemon's stream under its lock).  The bilateral averaging itself
     runs asynchronously on the native daemon's low-priority stream the whole time.  ``batch_mix``:
     mixup / CutMix as in ``GossipTrainer``.  ``ema`` must be None: a weight EMA is not supported,
-    the gossip daemon rewrites the parameters concurrently on its own stream."""
+    the gossip daemon rewrites the parameters concurrently on its own stream.  ``teacher`` must be None
+    and the criterion must not distil: knowledge distillation is ``GossipTrainer``'s."""
+    if teacher is not None or getattr(criterion, 'distill_alpha', 0.0) > 0:
+        raise ValueError('knowledge distillation is not supported with AD-PSGD: only GossipTrainer runs a teacher')
     if ema is not None:
         raise ValueError('ModelEma is not supported with AD-PSGD: its gossip daemon rewrites the parameters '
                          'concurrently on another stream, so no launch sees a settled model')

@@ -63,6 +63,16 @@ draws its masks with one ``drop_path_draw`` launch, so ``own_launches_per_step``
 (k with ``accumulation_steps=k``: each micro-batch has its own masks), and every replay draws fresh
 ones.  ``update_bn`` (inside ``precise_bn_stats``) and ``evaluate`` (eval mode) draw nothing and scale
 nothing: precise statistics describe the network that evaluation runs.
+
+Knowledge distillation (``teacher=net``, with ``FusedCrossEntropyWithAccuracy(distill_alpha > 0)``): every
+(micro-)batch first runs the frozen teacher's eval-mode forward on the step's input -- under ``no_grad`` and
+``ops.fused_bn.eval_bn_gemm``, in the step's precision (a bf16 copy of the teacher with the bf16 twin, the
+trainer's autocast otherwise) -- and passes its logits to the fused loss, whose two launches replace the
+cross-entropy's one for one.  The teacher runs before the student forward, so nothing comes between the
+student's forward and its backward, and it sees the mixed batch under ``batch_mix``.  Its parameters and
+statistics never change and are not part of the arena, the gossip, the EMA or ``state_dict``;
+``own_launches_per_step`` grows by the teacher forward's launches.  ``evaluate`` and ``update_bn`` do not
+run it.
 """
 
 from __future__ import annotations
@@ -75,6 +85,8 @@ from typing import Callable, NamedTuple, Optional
 
 import torch
 
+import torch.nn as nn
+
 from ..ops.fused_bn import BNStatsAccumulator, eval_bn_gemm, precise_bn_stats
 from ..ops.fused_loss import FusedCrossEntropyWithAccuracy, eval_accumulate, eval_accumulator
 from ..optim import FusedGossipSGD
@@ -86,6 +98,43 @@ def check_accumulation_steps(k) -> int:
     if isinstance(k, bool) or not isinstance(k, numbers.Integral) or k < 1:
         raise ValueError('accumulation_steps must be an integer >= 1, got %r' % (k,))
     return int(k)
+
+
+def check_distill_teacher(teacher, criterion, device) -> None:
+    """ValueError unless ``teacher`` is given exactly when ``criterion`` is a
+    ``FusedCrossEntropyWithAccuracy`` with ``distill_alpha > 0``, and is an ``nn.Module`` whose
+    parameters and buffers all live on ``device``."""
+    distill = isinstance(criterion, FusedCrossEntropyWithAccuracy) and criterion.distill_alpha > 0
+    if teacher is None:
+        if distill:
+            raise ValueError('the criterion has distill_alpha = %g > 0 but no teacher was given'
+                             % criterion.distill_alpha)
+        return
+    if not isinstance(teacher, nn.Module):
+        raise ValueError('teacher must be an nn.Module, got %s' % type(teacher).__name__)
+    if not distill:
+        raise ValueError('a teacher needs the criterion FusedCrossEntropyWithAccuracy(distill_alpha > 0), got %r'
+                         % (criterion,))
+    device = torch.device(device)
+    for t in list(teacher.parameters()) + list(teacher.buffers()):
+        if t.device.type != device.type or (device.index is not None and t.device.index != device.index):
+            raise ValueError('the teacher must be on the trainer\'s device %s; it has a tensor on %s'
+                             % (device, t.device))
+
+
+def teacher_compute_twin(teacher: nn.Module) -> nn.Module:
+    """A copy of ``teacher`` for the bf16 compute twin's step: every parameter outside the normalisation
+    layers (the convolution and linear weights) in bf16; normalisation parameters and all buffers stay fp32.
+    Eval mode, no gradients."""
+    import copy
+    from torch.nn.modules.batchnorm import _NormBase
+    twin = copy.deepcopy(teacher)
+    norm_ids = set(id(p) for m in twin.modules() if isinstance(m, _NormBase) for p in m.parameters(recurse=False))
+    with torch.no_grad():
+        for p in twin.parameters():
+            if id(p) not in norm_ids:
+                p.data = p.data.to(torch.bfloat16)
+    return twin.eval().requires_grad_(False)
 
 
 class EvalResult(NamedTuple):
@@ -116,13 +165,17 @@ class GossipTrainer(object):
     def __init__(self, model: GossipDataParallel, optimizer: FusedGossipSGD,
                  criterion: Optional[Callable] = None, amp_dtype=torch.bfloat16,
                  use_cuda_graph: bool = True, warmup_iters: int = 3,
-                 channels_last: bool = True, batch_mix=None, ema=None, accumulation_steps: int = 1):
+                 channels_last: bool = True, batch_mix=None, ema=None, accumulation_steps: int = 1,
+                 teacher: Optional[nn.Module] = None):
         """``batch_mix``: an ``ops.batch_mix.BatchMix`` to train with mixup / CutMix (needs the
         fused criterion; the draw of each step comes from ``batch_mix.iteration``), or None.
         ``ema``: an ``ops.model_ema.ModelEma`` of ``model`` updated at the end of every step, or None.
         ``accumulation_steps``: k >= 1 forward/backward passes per step over equal row slices of the
         step batch, whose size must be divisible by k (see the module docstring); not with
-        ``nprocs_per_node > 1``."""
+        ``nprocs_per_node > 1``.  ``teacher``: a module on the trainer's device that maps the step's input to
+        ``[B, C]`` logits, to distil from (module docstring); given exactly when ``criterion`` is a
+        ``FusedCrossEntropyWithAccuracy`` with ``distill_alpha > 0``.  The trainer puts it in eval mode and
+        turns its gradients off."""
         accumulation_steps = check_accumulation_steps(accumulation_steps)
         if accumulation_steps > 1 and getattr(model, 'nprocs_per_node', 1) > 1:
             raise ValueError('accumulation_steps > 1 is not supported with nprocs_per_node > 1 (hierarchical '
@@ -141,6 +194,17 @@ class GossipTrainer(object):
         if accumulation_steps > 1 and not self.batched_grad_copy and getattr(model, '_twin', None):
             raise ValueError('accumulation_steps > 1 with the bf16 compute twin needs the batched gradient '
                              'copy (SGP_B200_BATCHED_GRAD_COPY=0 would sum its gradients in bf16)')
+        self._attach_teacher(teacher)
+
+    def _attach_teacher(self, teacher):
+        """checks ``teacher`` against the criterion and device, freezes it in eval mode and, with the bf16
+        compute twin, builds the bf16 copy the step runs"""
+        check_distill_teacher(teacher, self.criterion, self.device)
+        self.teacher = teacher
+        if teacher is None:
+            return
+        teacher.eval().requires_grad_(False)
+        self._teacher_net = teacher_compute_twin(teacher) if getattr(self.model, '_twin', None) else teacher
 
     def _init_runtime(self, device, criterion, amp_dtype, use_cuda_graph, warmup_iters, channels_last,
                       batch_mix=None, ema=None):
@@ -204,6 +268,8 @@ class GossipTrainer(object):
         self.eval_launches_per_batch = None
         self._bn_acc = None             # update_bn(): the fp64 BatchNorm statistics accumulator
         self.update_bn_launches_per_batch = None
+        self.teacher = None                 # GossipTrainer(teacher=...): the frozen teacher ...
+        self._teacher_net = None            # ... and what the step runs: it, or its bf16 copy
 
     # ------------------------------------------------------------------ #
     def _autocast(self):
@@ -225,16 +291,18 @@ class GossipTrainer(object):
         ``metrics_out``.  ``accumulate``: add the gradients to the arena instead of writing them."""
         twin = getattr(self.model, '_twin', None)
         net = None
+        # the teacher first: nothing may come between the student's forward and its backward
+        u = self._teacher_forward(x) if self._teacher_net is not None else None
         if twin:
             # bf16 twin: weights already live in bf16 (shadow arena), input buffer is bf16
             net = twin[0]
             net.train(self.model.module.training)
             out = net(x)
-            loss = self._loss(out, tgt)
+            loss = self._loss(out, tgt, u)
         else:
             with self._autocast():
                 out = self.model.module(x)
-                loss = self._loss(out, tgt)
+                loss = self._loss(out, tgt, u)
         self._backward(loss, net if twin else self.model.module, accumulate)
         metrics = getattr(self.criterion, 'metrics', None)
         if metrics is not None:
@@ -243,10 +311,17 @@ class GossipTrainer(object):
             metrics_out[0].copy_(loss.detach())
         return out
 
-    def _loss(self, out, tgt):
+    def _teacher_forward(self, x):
+        """the teacher's logits for input ``x``: eval mode, BatchNorm in the 1x1-conv GEMM epilogue, the step's
+        precision (as :meth:`evaluate` runs the student)"""
+        with torch.no_grad(), eval_bn_gemm(), self._eval_autocast():
+            return self._teacher_net(x)
+
+    def _loss(self, out, tgt, teacher_logits=None):
+        kw = {} if teacher_logits is None else {'teacher_logits': teacher_logits}
         if self.batch_mix is not None:            # two targets per row, lam from the device mix state
-            return self.criterion(out, tgt, mix=self.batch_mix.state)
-        return self.criterion(out if self._fused_loss else out.float(), tgt)
+            return self.criterion(out, tgt, mix=self.batch_mix.state, **kw)
+        return self.criterion(out if self._fused_loss else out.float(), tgt, **kw)
 
     def _backward(self, loss, net, accumulate=False):
         """``loss.backward()`` without ~160 per-parameter accumulate kernels: the flat gradient

@@ -166,11 +166,16 @@ def build_parser(adpsgd: bool = False) -> argparse.ArgumentParser:
                         "shards: pre-decoded uint8 shards under DATASET_DIR/{train,val} (python -m "
                         "stochastic_gradient_push_b200.data.make_shards) gathered by a background thread, "
                         "crop / flip / normalisation on the GPU (data/shards.py)")
-    p.add_argument('--auto_augment', default='none', choices=['none', 'ta_wide'],
-                   help='ta_wide: TrivialAugmentWide on the training images (torchvision\'s ResNet-50 recipe); '
-                        'with --data_format shards inside the GPU augment kernel (data.GpuAugment), with '
-                        '--data_format folder transforms.TrivialAugmentWide() after the flip.  Not with '
-                        'synthetic data')
+    p.add_argument('--auto_augment', default='none', choices=['none', 'ta_wide', 'ra', 'imagenet'],
+                   help='augmentation policy on the training images: ta_wide TrivialAugmentWide (torchvision\'s '
+                        'ResNet-50 recipe), ra RandAugment (--ra_num_ops, --ra_magnitude), imagenet AutoAugment '
+                        'with the ImageNet policy; with --data_format shards inside the GPU augment kernel '
+                        '(data.GpuAugment), with --data_format folder the torchvision transform after the '
+                        'flip.  Not with synthetic data')
+    p.add_argument('--ra_num_ops', default=2, type=int,
+                   help='--auto_augment ra: ops applied in sequence to each image, in [0, 4]')
+    p.add_argument('--ra_magnitude', default=9, type=int,
+                   help='--auto_augment ra: magnitude bin of every op, in [0, 30]')
     p.add_argument('--random_erase', default=0.0, type=float,
                    help='probability p in [0, 1] of RandomErasing(p, value=0) after the normalisation of each '
                         'training image (GPU augment kernel with --data_format shards, '
@@ -380,11 +385,16 @@ def check_mix_flags(args):
 
 
 def check_augment_flags(args):
-    """ValueError for --random_erase outside [0, 1], and for --auto_augment / --random_erase with
-    synthetic data (there are no images to augment)."""
+    """ValueError for --random_erase outside [0, 1], --ra_num_ops outside [0, 4], --ra_magnitude
+    outside [0, 30], and for --auto_augment / --random_erase with synthetic data (there are no images
+    to augment)."""
     p = getattr(args, 'random_erase', 0.0)
     if not 0.0 <= p <= 1.0:
         raise ValueError('--random_erase must be in [0, 1], got %r' % (p,))
+    for flag, hi in (('ra_num_ops', 4), ('ra_magnitude', 30)):
+        v = getattr(args, flag, 0)
+        if not 0 <= v <= hi:
+            raise ValueError('--%s must be in [0, %d], got %r' % (flag, hi, v))
     if (getattr(args, 'auto_augment', 'none') != 'none' or p > 0) and args.synthetic:
         raise ValueError('--auto_augment / --random_erase need image data (--dataset_dir); synthetic data '
                          'has no images to augment')
@@ -718,17 +728,22 @@ def make_dataloader(args, train=True):
 
 
 def folder_transforms(args, train=True):
-    """The ``--data_format folder`` pipeline: RandomResizedCrop, flip, [TrivialAugmentWide],
-    ToTensor, Normalize, [RandomErasing] for training (torchvision's recipe order), Resize +
-    CenterCrop for validation, which never augments."""
+    """The ``--data_format folder`` pipeline: RandomResizedCrop, flip, [TrivialAugmentWide |
+    RandAugment | AutoAugment], ToTensor, Normalize, [RandomErasing] for training (torchvision's
+    recipe order), Resize + CenterCrop for validation, which never augments."""
     import torchvision.transforms as transforms
     norm = transforms.Normalize(mean=[0.485, 0.456, 0.406], std=[0.229, 0.224, 0.225])
     if not train:
         return transforms.Compose([transforms.Resize(int(args.image_size * 256 / 224)),
                                    transforms.CenterCrop(args.image_size), transforms.ToTensor(), norm])
     steps = [transforms.RandomResizedCrop(args.image_size), transforms.RandomHorizontalFlip()]
-    if getattr(args, 'auto_augment', 'none') == 'ta_wide':
+    policy = getattr(args, 'auto_augment', 'none')
+    if policy == 'ta_wide':
         steps.append(transforms.TrivialAugmentWide())
+    elif policy == 'ra':
+        steps.append(transforms.RandAugment(num_ops=args.ra_num_ops, magnitude=args.ra_magnitude))
+    elif policy == 'imagenet':
+        steps.append(transforms.AutoAugment(transforms.AutoAugmentPolicy.IMAGENET))
     steps += [transforms.ToTensor(), norm]
     if getattr(args, 'random_erase', 0.0) > 0:
         steps.append(transforms.RandomErasing(p=args.random_erase))
@@ -747,7 +762,9 @@ def device_batch(args, batch, train=True):
         ta = getattr(args, 'auto_augment', 'none')
         aug = args._gpu_augment = GpuAugment(out_size=args.image_size, seed=args.seed * 7919 + args.rank,
                                              auto_augment=None if ta == 'none' else ta,
-                                             random_erase=getattr(args, 'random_erase', 0.0))
+                                             random_erase=getattr(args, 'random_erase', 0.0),
+                                             ra_num_ops=getattr(args, 'ra_num_ops', 2),
+                                             ra_magnitude=getattr(args, 'ra_magnitude', 9))
     return aug(batch.to(args.device, non_blocking=True), train=train)
 
 

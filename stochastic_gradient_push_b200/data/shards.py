@@ -25,6 +25,7 @@ training loader).
 
 from __future__ import annotations
 
+import functools
 import json
 import math
 import os
@@ -245,13 +246,54 @@ TA_WIDE_OPS = ('Identity', 'ShearX', 'ShearY', 'TranslateX', 'TranslateY', 'Rota
 TA_WIDE_SIGNED = frozenset(TA_WIDE_OPS[1:10])
 TA_WIDE_BINS = 31
 GEOMETRIC_OPS = frozenset(TA_WIDE_OPS[1:6])
+# every op the augment kernel applies (its op ids): AutoAugment's ImageNet policy adds Invert
+AUGMENT_OPS = TA_WIDE_OPS + ('Invert',)
+# RandAugment (Cubuk et al. 2020) as torchvision.transforms.v2.RandAugment draws it: num_ops ops, each
+# uniform over TA_WIDE_OPS, at bin `magnitude` of 31, a random sign for the signed ops
+RA_BINS = 31
+RA_MAX_OPS = 4
+# AutoAugment's ImageNet policy (Cubuk et al. 2019) as torchvision.transforms.v2.AutoAugment holds it:
+# one of these 25 sub-policies uniformly, each (op, probability, bin of 10) applied with its probability
+AA_BINS = 10
+AUTO_AUGMENT_IMAGENET = (
+    (('Posterize', 0.4, 8), ('Rotate', 0.6, 9)),
+    (('Solarize', 0.6, 5), ('AutoContrast', 0.6, None)),
+    (('Equalize', 0.8, None), ('Equalize', 0.6, None)),
+    (('Posterize', 0.6, 7), ('Posterize', 0.6, 6)),
+    (('Equalize', 0.4, None), ('Solarize', 0.2, 4)),
+    (('Equalize', 0.4, None), ('Rotate', 0.8, 8)),
+    (('Solarize', 0.6, 3), ('Equalize', 0.6, None)),
+    (('Posterize', 0.8, 5), ('Equalize', 1.0, None)),
+    (('Rotate', 0.2, 3), ('Solarize', 0.6, 8)),
+    (('Equalize', 0.6, None), ('Posterize', 0.4, 6)),
+    (('Rotate', 0.8, 8), ('Color', 0.4, 0)),
+    (('Rotate', 0.4, 9), ('Equalize', 0.6, None)),
+    (('Equalize', 0.0, None), ('Equalize', 0.8, None)),
+    (('Invert', 0.6, None), ('Equalize', 1.0, None)),
+    (('Color', 0.6, 4), ('Contrast', 1.0, 8)),
+    (('Rotate', 0.8, 8), ('Color', 1.0, 2)),
+    (('Color', 0.8, 8), ('Solarize', 0.8, 7)),
+    (('Sharpness', 0.4, 7), ('Invert', 0.6, None)),
+    (('ShearX', 0.6, 5), ('Equalize', 1.0, None)),
+    (('Color', 0.4, 0), ('Equalize', 0.6, None)),
+    (('Equalize', 0.4, None), ('Solarize', 0.2, 4)),
+    (('Solarize', 0.6, 5), ('AutoContrast', 0.6, None)),
+    (('Invert', 0.6, None), ('Equalize', 1.0, None)),
+    (('Color', 0.6, 4), ('Contrast', 1.0, 8)),
+    (('Equalize', 0.8, None), ('Equalize', 0.6, None)),
+)
 ERASE_SCALE = (0.02, 0.33)
 ERASE_RATIO = (0.3, 3.3)
 ERASE_ATTEMPTS = 10
 # dynamic shared memory one CTA may use on sm_90 (227 KB); the augment kernel keeps the whole
 # out x out x 3 uint8 crop there plus its per-op tables
 SM90_SMEM_PER_CTA = 232448
-AUGMENT_ROW = 24
+# the augment kernel's per-image rows: one op (TrivialAugment, erasing only), or a chain of up to
+# AUGMENT_MAX_OPS ops (RandAugment, AutoAugment); op k >= 2 at AUGMENT_CHAIN_COL + 9 (k - 2)
+AUGMENT_ROW_ONE_OP = 24
+AUGMENT_ROW = 48
+AUGMENT_MAX_OPS = 4
+AUGMENT_CHAIN_COL = 19
 
 
 def ta_wide_magnitudes(num_bins: int = TA_WIDE_BINS) -> dict:
@@ -267,6 +309,20 @@ def ta_wide_magnitudes(num_bins: int = TA_WIDE_BINS) -> dict:
     }
 
 
+def policy_magnitudes(num_bins: int, size: int) -> dict:
+    """op name (every op of :data:`AUGMENT_OPS`) -> magnitude per bin of RandAugment's and
+    AutoAugment's shared space for ``size x size`` images (fp32 values as torchvision's v2 tables
+    hold them; None for the ops without a magnitude).  RandAugment takes 31 bins, AutoAugment 10."""
+    lin = lambda hi: torch.linspace(0.0, hi, num_bins)  # noqa: E731
+    return {
+        'Identity': None, 'ShearX': lin(0.3), 'ShearY': lin(0.3), 'TranslateX': lin(150.0 / 331.0 * size),
+        'TranslateY': lin(150.0 / 331.0 * size), 'Rotate': lin(30.0), 'Brightness': lin(0.9), 'Color': lin(0.9),
+        'Contrast': lin(0.9), 'Sharpness': lin(0.9),
+        'Posterize': (8 - (torch.arange(num_bins) / ((num_bins - 1) / 4))).round().int(),
+        'Solarize': torch.linspace(1.0, 0.0, num_bins), 'AutoContrast': None, 'Equalize': None, 'Invert': None,
+    }
+
+
 def augment_smem_bytes(out: int) -> int:
     """Shared memory of one augment-kernel CTA for ``out x out`` output images (the kernel's
     ``aug_smem_bytes``)."""
@@ -277,10 +333,11 @@ class AugmentParams(NamedTuple):
     """Per-sample parameters of one training batch (CPU tensors, ``n`` rows each).
 
     ``cx, cy, w, h, flip``: the RandomResizedCrop box as fractions of the stored image and the flip
-    sign (fp32, :meth:`GpuAugment.sample_boxes`); ``op``: int64 index into :data:`TA_WIDE_OPS`;
-    ``magnitude``: float64, the signed magnitude torchvision would pass to the op (0 for the ops
-    without one); ``erase``: int64 ``[n, 4]`` box ``(top, left, height, width)`` in output pixels,
-    height 0 = no box."""
+    sign (fp32, :meth:`GpuAugment.sample_boxes`); ``op``: int64 index into :data:`AUGMENT_OPS`,
+    ``[n]`` for one op per sample or ``[n, K]`` for a chain of ``K <= 4`` ops applied left to right;
+    ``magnitude``: float64, shaped as ``op``, the signed magnitude torchvision would pass to the op (0
+    for the ops without one); ``erase``: int64 ``[n, 4]`` box ``(top, left, height, width)`` in output
+    pixels, height 0 = no box."""
     cx: torch.Tensor
     cy: torch.Tensor
     w: torch.Tensor
@@ -326,6 +383,14 @@ def ta_wide_matrix(op: str, magnitude: float, size: int) -> List[float]:
     raise ValueError('%s is not a geometric op' % op)
 
 
+@functools.lru_cache(maxsize=4096)
+def _geometric_columns(op: str, magnitude: float, size: int) -> np.ndarray:
+    """a geometric op's six row entries: torchvision's _affine_grid rescaling theta^T / [w / 2, h / 2]
+    of :func:`ta_wide_matrix`, in fp32.  Cached: a policy draws few distinct (op, magnitude) pairs."""
+    m = np.asarray(ta_wide_matrix(op, magnitude, size), dtype=np.float32)
+    return m / np.float32(0.5 * size)
+
+
 class GpuAugment(object):
     """uint8 ``[B, S, S, 3]`` -> normalised ``[B, 3, out, out]`` (channels-last memory format).
 
@@ -334,18 +399,21 @@ class GpuAugment(object):
     scale); evaluation: centre crop of ``out / eval_ratio`` resized to ``out`` (the reference's
     ``Resize(256) + CenterCrop(224)`` when the shards were stored at 256).
 
-    ``auto_augment='ta_wide'`` adds TrivialAugmentWide and ``random_erase=p`` adds
+    ``auto_augment`` adds an augmentation policy on the uint8 crop: ``'ta_wide'`` TrivialAugmentWide,
+    ``'ra'`` RandAugment (``ra_num_ops`` ops at bin ``ra_magnitude`` of 31, torchvision v2 semantics),
+    ``'imagenet'`` AutoAugment with the ImageNet policy; ``random_erase=p`` adds
     ``RandomErasing(p, value=0)`` after the normalisation, in torchvision's recipe order.  With
     either on, a training batch on the GPU is ONE launch of the sm_90a augment kernel
     (``csrc/augment_kernels.cu``): the crop rounded to uint8 as torchvision's uint8 pipeline
-    rounds it, the op, the normalisation and the erase box.  Their draws come from a second
+    rounds it, the op or chain of ops (each on the uint8 result of the one before), the
+    normalisation and the erase box.  Their draws come from a second
     generator, so the crop boxes and flips of a seed do not depend on these options.  CPU batches
     take the reference composition (``ops.oracle.reference_augment``); evaluation never augments."""
 
     def __init__(self, out_size: int = 224, scale=(0.08, 1.0), ratio=(3.0 / 4.0, 4.0 / 3.0),
                  mean=IMAGENET_MEAN, std=IMAGENET_STD, dtype=torch.float32, eval_ratio: float = 0.875,
                  seed: int = 0, channels_last: bool = True, auto_augment: Optional[str] = None,
-                 random_erase: float = 0.0):
+                 random_erase: float = 0.0, ra_num_ops: int = 2, ra_magnitude: int = 9):
         self.out = int(out_size)
         self.scale, self.ratio = scale, ratio
         self.mean, self.std = tuple(mean), tuple(std)
@@ -354,12 +422,16 @@ class GpuAugment(object):
         self.channels_last = channels_last
         self._gen = torch.Generator().manual_seed(int(seed))
         self._consts = {}
-        if auto_augment not in (None, 'ta_wide'):
-            raise ValueError("auto_augment must be None or 'ta_wide', got %r" % (auto_augment,))
+        if auto_augment not in (None, 'ta_wide', 'ra', 'imagenet'):
+            raise ValueError("auto_augment must be None, 'ta_wide', 'ra' or 'imagenet', got %r" % (auto_augment,))
         if not 0.0 <= float(random_erase) <= 1.0:
             raise ValueError('random_erase must be in [0, 1], got %r' % (random_erase,))
+        for name, v, hi in (('ra_num_ops', ra_num_ops, RA_MAX_OPS), ('ra_magnitude', ra_magnitude, RA_BINS - 1)):
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not 0 <= v <= hi:
+                raise ValueError('%s must be an integer in [0, %d], got %r' % (name, hi, v))
         self.auto_augment = auto_augment
         self.random_erase = float(random_erase)
+        self.ra_num_ops, self.ra_magnitude = int(ra_num_ops), int(ra_magnitude)
         if self.augments and augment_smem_bytes(self.out) > SM90_SMEM_PER_CTA:
             raise ValueError('out_size %d needs %d bytes of shared memory per image with auto_augment / '
                              'random_erase; an sm_90 CTA has %d' % (self.out, augment_smem_bytes(self.out),
@@ -368,14 +440,24 @@ class GpuAugment(object):
         tables = ta_wide_magnitudes()
         self._table = torch.stack([torch.zeros(TA_WIDE_BINS, dtype=torch.float64) if tables[k] is None
                                    else tables[k].double() for k in TA_WIDE_OPS])
-        self._signed = torch.tensor([k in TA_WIDE_SIGNED for k in TA_WIDE_OPS])
+        self._signed = torch.tensor([k in TA_WIDE_SIGNED for k in AUGMENT_OPS])
+        # RandAugment: each op's magnitude at the fixed bin; AutoAugment: per sub-policy and slot the
+        # op id, its probability (fp32, as torchvision compares it) and its magnitude
+        space = policy_magnitudes(RA_BINS, self.out)
+        self._ra_mag = torch.tensor([0.0 if space[k] is None else float(space[k][self.ra_magnitude])
+                                     for k in AUGMENT_OPS], dtype=torch.float64)
+        space = policy_magnitudes(AA_BINS, self.out)
+        self._aa_op = torch.tensor([[AUGMENT_OPS.index(o) for o, _, _ in sub] for sub in AUTO_AUGMENT_IMAGENET])
+        self._aa_prob = torch.tensor([[p for _, p, _ in sub] for sub in AUTO_AUGMENT_IMAGENET], dtype=torch.float32)
+        self._aa_mag = torch.tensor([[0.0 if b is None else float(space[o][b]) for o, _, b in sub]
+                                     for sub in AUTO_AUGMENT_IMAGENET], dtype=torch.float64)
         self._ring = None
         self._events = [None] * RING_SLOTS
         self._slot = 0
 
     @property
     def augments(self) -> bool:
-        """True when training batches take the augment kernel (TrivialAugment or erasing on)."""
+        """True when training batches take the augment kernel (a policy or erasing on)."""
         return self.auto_augment is not None or self.random_erase > 0
 
     def _norm(self, device):
@@ -415,9 +497,13 @@ class GpuAugment(object):
 
     def sample_params(self, n: int) -> AugmentParams:
         """The next training batch's :class:`AugmentParams`: crop boxes and flips from
-        :meth:`sample_boxes`, then, from the second generator, per sample, TrivialAugmentWide's op
-        (uniform over :data:`TA_WIDE_OPS`), bin (uniform over 31) and sign (negative with
-        probability 1/2, signed ops only), and RandomErasing's box: with probability ``p``, up to
+        :meth:`sample_boxes`, then, from the second generator, per sample, the policy's ops and
+        RandomErasing's box.  TrivialAugmentWide (``op`` ``[n]``): the op (uniform over
+        :data:`TA_WIDE_OPS`), bin (uniform over 31) and sign (negative with probability 1/2, signed
+        ops only).  RandAugment (``op`` ``[n, ra_num_ops]``): each op uniform over :data:`TA_WIDE_OPS`
+        at bin ``ra_magnitude``, then each sign.  AutoAugment (``op`` ``[n, 2]``): the sub-policy
+        (uniform over 25), whether each of its ops applies (Identity otherwise), then each sign.
+        RandomErasing: with probability ``p``, up to
         10 attempts of area fraction U(0.02, 0.33) and log aspect ratio U(log 0.3, log 3.3),
         ``h = round(sqrt(area r))``, ``w = round(sqrt(area / r))``; the first box strictly inside
         the image is placed at a uniform integer position, none if no attempt fits."""
@@ -431,6 +517,19 @@ class GpuAugment(object):
             negate = torch.rand(n, generator=g) <= 0.5
             sign = torch.where(negate & self._signed[op], -1.0, 1.0).double()
             magnitude = self._table[op, bins] * sign
+        elif self.auto_augment == 'ra':
+            k = self.ra_num_ops
+            op = torch.randint(len(TA_WIDE_OPS), (n, k), generator=g)
+            negate = torch.rand(n, k, generator=g) <= 0.5
+            sign = torch.where(negate & self._signed[op], -1.0, 1.0).double()
+            magnitude = self._ra_mag[op] * sign
+        elif self.auto_augment == 'imagenet':
+            sub = torch.randint(len(AUTO_AUGMENT_IMAGENET), (n,), generator=g)
+            on = torch.rand(n, 2, generator=g) <= self._aa_prob[sub]
+            negate = torch.rand(n, 2, generator=g) <= 0.5
+            op = torch.where(on, self._aa_op[sub], 0)
+            sign = torch.where(negate & self._signed[op], -1.0, 1.0).double()
+            magnitude = torch.where(on, self._aa_mag[sub], 0.0) * sign
         erase = torch.zeros(n, 4, dtype=torch.int64)
         if self.random_erase > 0:
             size = self.out
@@ -456,51 +555,60 @@ class GpuAugment(object):
         return AugmentParams(cx, cy, w, h, flip, op, magnitude, erase)
 
     def kernel_rows(self, params: AugmentParams, S: int) -> np.ndarray:
-        """fp32 ``[n, AUGMENT_ROW]``: the augment kernel's per-image rows for ``params`` (layout in
-        ``csrc/augment_kernels.cu``).  Every op scalar is rounded to fp32 the way torch rounds a
-        Python scalar against an fp32 tensor."""
-        n = len(params.op)
-        out = self.out
-        rows = np.zeros((n, AUGMENT_ROW), dtype=np.float32)
+        """fp32 ``[n, AUGMENT_ROW_ONE_OP]`` for one op per sample (``params.op`` ``[n]``), else
+        ``[n, AUGMENT_ROW]`` with op k of the chain at its columns and Identity after the last: the
+        augment kernel's per-image rows for ``params`` (layout in ``csrc/augment_kernels.cu``).  Every
+        op scalar is rounded to fp32 the way torch rounds a Python scalar against an fp32 tensor."""
+        op, mag = params.op.numpy(), params.magnitude.numpy()
+        chain = op.ndim == 2
+        if not chain:
+            op, mag = op[:, None], mag[:, None]
+        n, k = op.shape
+        if k > AUGMENT_MAX_OPS:
+            raise ValueError('the augment kernel applies at most %d ops per image, got %d' % (AUGMENT_MAX_OPS, k))
+        rows = np.zeros((n, AUGMENT_ROW if chain else AUGMENT_ROW_ONE_OP), dtype=np.float32)
         rows[:, 0:6] = self.crop_theta(params.cx, params.cy, params.w, params.h, params.flip).reshape(n, 6).numpy()
-        op = params.op.numpy()
-        mag = params.magnitude.numpy()
-        rows[:, 6] = op
-        is_op = lambda *names: np.isin(op, [TA_WIDE_OPS.index(k) for k in names])  # noqa: E731
-        sel = is_op('Brightness', 'Color', 'Contrast')
-        rows[sel, 7] = 1.0 + mag[sel]
-        sel = is_op('Color', 'Contrast', 'Sharpness')
-        rows[sel, 8] = 1.0 - (1.0 + mag[sel])
-        sel = is_op('Posterize')
-        bits = mag[sel].astype(np.int64)
-        rows[sel, 7] = np.where(bits >= 8, 255, ((1 << bits) - 1) << np.maximum(8 - bits, 0))
-        sel = is_op('Solarize')
-        rows[sel, 7] = 255.0 * mag[sel]
-        half = np.float32(0.5 * out)
-        for i in np.nonzero(is_op(*GEOMETRIC_OPS))[0]:
-            m = np.asarray(ta_wide_matrix(TA_WIDE_OPS[op[i]], float(mag[i]), out), dtype=np.float32)
-            rows[i, 9:15] = m / half           # torchvision's _affine_grid: theta^T / [w / 2, h / 2] in fp32
+        for j in range(k):
+            col = 6 if j == 0 else AUGMENT_CHAIN_COL + 9 * (j - 1)
+            self._op_columns(rows[:, col:col + 9], op[:, j], mag[:, j])
         e = params.erase.numpy()
         rows[:, 15], rows[:, 16], rows[:, 17], rows[:, 18] = e[:, 0], e[:, 0] + e[:, 2], e[:, 1], e[:, 1] + e[:, 3]
         return rows
 
+    def _op_columns(self, cols: np.ndarray, op: np.ndarray, mag: np.ndarray):
+        """one op's 9 row columns: id, two scalars, the geometric ops' six matrix entries"""
+        out = self.out
+        cols[:, 0] = op
+        is_op = lambda *names: np.isin(op, [AUGMENT_OPS.index(k) for k in names])  # noqa: E731
+        sel = is_op('Brightness', 'Color', 'Contrast')
+        cols[sel, 1] = 1.0 + mag[sel]
+        sel = is_op('Color', 'Contrast', 'Sharpness')
+        cols[sel, 2] = 1.0 - (1.0 + mag[sel])
+        sel = is_op('Posterize')
+        bits = mag[sel].astype(np.int64)
+        cols[sel, 1] = np.where(bits >= 8, 255, ((1 << bits) - 1) << np.maximum(8 - bits, 0))
+        sel = is_op('Solarize')
+        cols[sel, 1] = 255.0 * mag[sel]
+        for i in np.nonzero(is_op(*GEOMETRIC_OPS))[0]:
+            cols[i, 3:9] = _geometric_columns(AUGMENT_OPS[op[i]], float(mag[i]), out)
+
     def _stage_rows(self, rows: np.ndarray, device) -> torch.Tensor:
         """``rows`` -> a fresh device tensor through ONE non-blocking H2D copy from a slot of a
         pinned ring; a slot is rewritten only after the copy that last read it has executed."""
-        n = rows.shape[0]
-        if self._ring is None or self._ring.shape[1] < n:
+        n, width = rows.shape
+        if self._ring is None or self._ring.shape[1] < n * width:
             for ev in self._events:
                 if ev is not None:
                     ev.synchronize()
-            self._ring = torch.empty(RING_SLOTS, n, AUGMENT_ROW, dtype=torch.float32, pin_memory=True)
+            self._ring = torch.empty(RING_SLOTS, n * width, dtype=torch.float32, pin_memory=True)
             self._events = [None] * RING_SLOTS
         slot = self._slot
         self._slot = (slot + 1) % RING_SLOTS
         if self._events[slot] is not None:
             self._events[slot].synchronize()
-        host = self._ring[slot, :n]
+        host = self._ring[slot, :n * width].view(n, width)
         host.numpy()[:] = rows
-        dev_rows = torch.empty(n, AUGMENT_ROW, dtype=torch.float32, device=device)
+        dev_rows = torch.empty(n, width, dtype=torch.float32, device=device)
         dev_rows.copy_(host, non_blocking=True)
         ev = self._events[slot] = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(device))
@@ -508,7 +616,7 @@ class GpuAugment(object):
 
     def apply(self, batch_u8: torch.Tensor, params: AugmentParams) -> torch.Tensor:
         """The training output of ``batch_u8`` for explicit per-sample ``params``: crop, round to
-        uint8, TrivialAugmentWide op, normalise, erase.  CUDA: one launch of the sm_90a augment
+        uint8, the op or chain of ops, normalise, erase.  CUDA: one launch of the sm_90a augment
         kernel (a missing extension is an error) and no host synchronisation; CPU: the reference
         composition ``ops.oracle.reference_augment``."""
         assert batch_u8.dtype == torch.uint8 and batch_u8.dim() == 4 and batch_u8.shape[-1] == 3

@@ -1018,13 +1018,15 @@ static void grad_accumulate(const std::vector<torch::Tensor>& dst, const std::ve
 // ---------------------------------------------------------------------------
 extern "C" {
 int sgp_augment_row();
+int sgp_augment_row_one_op();
 long long sgp_augment_smem_bytes(int out);
-cudaError_t sgp_launch_augment(const uint8_t* src, const float* rows, void* dst, int out_dtype, int B, int S, int out,
-                               const float* mean, const float* inv, cudaStream_t st);
+cudaError_t sgp_launch_augment(const uint8_t* src, const float* rows, int row_len, void* dst, int out_dtype, int B,
+                               int S, int out, const float* mean, const float* inv, cudaStream_t st);
 }
 
-// src: uint8 [B, S, S, 3] contiguous; rows: fp32 [B, AUGMENT_ROW] per-image parameters; out: [B, 3, o, o]
-// channels_last fp32 / bf16.  One launch on the current stream.
+// src: uint8 [B, S, S, 3] contiguous; rows: fp32 [B, AUGMENT_ROW_ONE_OP] (one op per image) or
+// [B, AUGMENT_ROW] (a chain of up to 4) per-image parameters; out: [B, 3, o, o] channels_last fp32 / bf16.
+// One launch on the current stream.
 static void gpu_augment(torch::Tensor src, torch::Tensor rows, torch::Tensor out, std::vector<double> mean,
                         std::vector<double> inv)
 {
@@ -1032,7 +1034,8 @@ static void gpu_augment(torch::Tensor src, torch::Tensor rows, torch::Tensor out
                 src.size(3) == 3 && src.is_contiguous(), "gpu_augment: src must be a contiguous uint8 [B, S, S, 3] CUDA tensor");
     const int64_t B = src.size(0);
     TORCH_CHECK(rows.is_cuda() && rows.scalar_type() == torch::kFloat32 && rows.is_contiguous() && rows.dim() == 2 &&
-                rows.size(0) == B && rows.size(1) == sgp_augment_row(), "gpu_augment: rows must be fp32 [B, AUGMENT_ROW]");
+                rows.size(0) == B && (rows.size(1) == sgp_augment_row_one_op() || rows.size(1) == sgp_augment_row()),
+                "gpu_augment: rows must be fp32 [B, AUGMENT_ROW_ONE_OP] or [B, AUGMENT_ROW]");
     TORCH_CHECK(out.is_cuda() && (out.scalar_type() == torch::kFloat32 || out.scalar_type() == torch::kBFloat16) &&
                 out.dim() == 4 && out.size(0) == B && out.size(1) == 3 && out.size(2) == out.size(3) &&
                 out.is_contiguous(at::MemoryFormat::ChannelsLast),
@@ -1045,9 +1048,9 @@ static void gpu_augment(torch::Tensor src, torch::Tensor rows, torch::Tensor out
                 "gpu_augment: the output size needs more shared memory than one CTA can have");
     const float m[3] = {(float)mean[0], (float)mean[1], (float)mean[2]};
     const float v[3] = {(float)inv[0], (float)inv[1], (float)inv[2]};
-    SGP_CUDA_CHECK(sgp_launch_augment(src.data_ptr<uint8_t>(), rows.data_ptr<float>(), out.data_ptr(),
-                                      out.scalar_type() == torch::kFloat32 ? 1 : 0, (int)B, (int)src.size(1), o, m, v,
-                                      at::cuda::getCurrentCUDAStream()));
+    SGP_CUDA_CHECK(sgp_launch_augment(src.data_ptr<uint8_t>(), rows.data_ptr<float>(), (int)rows.size(1),
+                                      out.data_ptr(), out.scalar_type() == torch::kFloat32 ? 1 : 0, (int)B,
+                                      (int)src.size(1), o, m, v, at::cuda::getCurrentCUDAStream()));
 }
 
 void bind_bn(py::module& mod);   // bn_bindings.cpp
@@ -1085,8 +1088,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, mod)
     mod.attr("ACCUM_CHUNK") = sgp_accum_chunk();
     mod.attr("ACCUM_MAX_SEGS") = sgp_accum_max_segs();
     mod.def("gpu_augment", &gpu_augment, py::arg("src"), py::arg("rows"), py::arg("out"), py::arg("mean"),
-            py::arg("inv"), "crop + TrivialAugmentWide op + normalise + erase of a uint8 batch: one launch");
+            py::arg("inv"), "crop + augmentation ops + normalise + erase of a uint8 batch: one launch");
     mod.attr("AUGMENT_ROW") = sgp_augment_row();
+    mod.attr("AUGMENT_ROW_ONE_OP") = sgp_augment_row_one_op();
     mod.def("augment_smem_bytes", &sgp_augment_smem_bytes, py::arg("out"),
             "dynamic shared memory one CTA of gpu_augment needs for an out x out image");
 

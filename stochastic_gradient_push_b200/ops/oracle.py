@@ -54,9 +54,9 @@ def mix_columns(xs: Sequence[torch.Tensor], ws: Sequence[float], graphs, mixings
 
 
 def ta_wide_op(img: torch.Tensor, op: str, magnitude: float) -> torch.Tensor:
-    """TrivialAugmentWide's op ``op`` at the signed ``magnitude`` on a uint8 ``[3, H, W]`` image,
-    through ``torchvision.transforms.v2.functional`` with the arguments TrivialAugmentWide passes
-    (nearest interpolation, fill 0)."""
+    """The augmentation op ``op`` (any of ``data.shards.AUGMENT_OPS``) at the signed ``magnitude`` on a
+    uint8 ``[3, H, W]`` image, through ``torchvision.transforms.v2.functional`` with the arguments
+    TrivialAugmentWide, RandAugment and AutoAugment pass (nearest interpolation, fill 0)."""
     import math
     import torchvision.transforms.v2.functional as TF
     from torchvision.transforms import InterpolationMode
@@ -90,26 +90,35 @@ def ta_wide_op(img: torch.Tensor, op: str, magnitude: float) -> torch.Tensor:
         return TF.autocontrast(img)
     if op == 'Equalize':
         return TF.equalize(img)
-    raise ValueError('unknown TrivialAugmentWide op %r' % (op,))
+    if op == 'Invert':
+        return TF.invert(img)
+    raise ValueError('unknown augmentation op %r' % (op,))
 
 
 def reference_augment(batch_u8: torch.Tensor, theta: torch.Tensor, ops, magnitudes, erase, out_size: int,
                       mean: torch.Tensor, inv: torch.Tensor) -> torch.Tensor:
     """What the augment kernel computes, in plain PyTorch + torchvision: ``grid_sample`` of the
     uint8 NHWC batch with the crop maps ``theta`` (bilinear, border, align_corners=False), rounded
-    to uint8; the TrivialAugmentWide op ``data.shards.TA_WIDE_OPS[ops[i]]`` at ``magnitudes[i]``
-    per sample; ``(v - mean) * inv`` in fp32; 0 inside each ``erase[i] = (top, left, h, w)`` box.
-    Returns fp32 ``[n, 3, out, out]`` in channels-last memory format."""
+    to uint8; per sample the op ``data.shards.AUGMENT_OPS[ops[i]]`` at ``magnitudes[i]``, or with
+    ``[n, K]`` ops and magnitudes the ops ``ops[i, 0]``, ..., ``ops[i, K - 1]`` left to right, each on
+    the uint8 result of the one before; ``(v - mean) * inv`` in fp32; 0 inside each
+    ``erase[i] = (top, left, h, w)`` box.  Returns fp32 ``[n, 3, out, out]`` in channels-last memory
+    format."""
     import torch.nn.functional as F
-    from ..data.shards import TA_WIDE_OPS
+    from ..data.shards import AUGMENT_OPS
     n = batch_u8.shape[0]
     x = batch_u8.permute(0, 3, 1, 2).float()
     grid = F.affine_grid(theta.to(x.device), (n, 3, out_size, out_size), align_corners=False)
     crop = F.grid_sample(x, grid, mode='bilinear', padding_mode='border', align_corners=False)
     crop = crop.round().clamp(0, 255).to(torch.uint8)
     y = torch.empty(n, 3, out_size, out_size)
+    ops, magnitudes = torch.as_tensor(ops), torch.as_tensor(magnitudes)
+    if ops.dim() == 1:
+        ops, magnitudes = ops[:, None], magnitudes[:, None]
     for i in range(n):
-        img = ta_wide_op(crop[i], TA_WIDE_OPS[int(ops[i])], float(magnitudes[i]))
+        img = crop[i]
+        for op, magnitude in zip(ops[i].tolist(), magnitudes[i].tolist()):
+            img = ta_wide_op(img, AUGMENT_OPS[int(op)], float(magnitude))
         y[i] = (img.float() - mean[0]) * inv[0]
         top, left, h, w = (int(v) for v in erase[i])
         y[i, :, top:top + h, left:left + w] = 0.0
